@@ -17,7 +17,7 @@ OBJDIR = os.path.join(HERE, "build")
 LIB = os.path.join(LIBDIR, "libb2points.so")
 
 SOURCES = ["b2_context.cu", "b2_cloud.cu", "b2_voxelmap.cu", "b2_kdtree.cu", "b2_factors.cu"]
-HEADERS = ["b2_internal.hpp", "b2_device.cuh", "b2_kdtree.cuh", "b2_factor_kernel_ws.cuh", "b2_factor_kernel_v2.cuh", "b2_factor_kernel_split.cuh", "b2_factor_kernel_sr.cuh", os.path.join("..", "..", "include", "b2points.h")]
+HEADERS = ["b2_internal.hpp", "b2_device.cuh", "b2_kdtree.cuh", "b2_factor_kernel_ws.cuh", os.path.join("..", "..", "include", "b2points.h")]
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 HOST_CXX = "/usr/bin/g++"
@@ -49,7 +49,7 @@ def _compile(src, verbose, defines=(), tag=""):
 
 
 def build(force: bool = False, verbose: bool = False, defines=(), tag: str = "") -> str:
-    """`defines` / `tag` build an experimental variant (e.g. defines=["B2_THREADS=384"], tag="_t384") next to the default library."""
+    """`defines` / `tag` build an experimental variant (e.g. defines=["B2_WS_RING=512"], tag="_r512") next to the default library."""
     os.makedirs(LIBDIR, exist_ok=True)
     os.makedirs(OBJDIR, exist_ok=True)
     lib = LIB if not tag else LIB.replace(".so", tag + ".so")

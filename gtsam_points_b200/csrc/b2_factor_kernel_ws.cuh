@@ -1,5 +1,5 @@
 // b2_factor_kernel_ws.cuh -- the hot kernel: warp-specialised fused correspondence search + linearization.
-// Included by b2_factors.cu after the shared pieces (FactorDesc, accumulate_point, warp_reduce32, epilogue).
+// Included by b2_factors.cu after the shared pieces (FactorDesc, accumulate_point_f, warp_reduce32, epilogue).
 //
 // Why warp specialisation.  One correspondence is the dependent chain
 //     coordinates -> rotate/floor/hash -> bucket group -> voxel id -> voxel record + source covariance -> ~155 FP64 ops
@@ -45,15 +45,7 @@ static_assert(kP % 4 == 0 && kC % 4 == 0, "setmaxnreg works on warpgroups of 4 w
 static_assert(kP % kC == 0, "every accumulate warp drains the same number of rings");
 static_assert((kRing & (kRing - 1)) == 0 && kRing >= 2 * 32 * kIPL + kWarpPoints, "ring capacity: a tile's hits + one batch of publication lag + one batch");
 static_assert(kWarpPoints * 4 % 128 == 0 || kPPL == 1, "coordinate prefetch works on whole lines");
-constexpr size_t kRingBytes = static_cast<size_t>(kP) * 2 * kRing * sizeof(double2);
-#ifndef B2_WS_KD_SMEM_STACK
-#define B2_WS_KD_SMEM_STACK 0
-#endif
-#ifndef B2_WS_HEAD_FENCE
-#define B2_WS_HEAD_FENCE 1
-#endif
-// dynamic shared memory of a launch: the rings, then (kd-tree kinds) one traversal-stack block per probe warp
-constexpr size_t kDynSmemBytes = kRingBytes + (B2_WS_KD_SMEM_STACK ? static_cast<size_t>(kP) * kKdSmemStackBytes : 0);
+constexpr size_t kRingBytes = static_cast<size_t>(kP) * 2 * kRing * sizeof(double2);  // dynamic shared memory of a launch
 
 constexpr unsigned kSpinLimit = 1u << 25;  // polls (with sleeps: >= 2 s, typically tens of seconds) before a wait traps: a protocol bug must not hang the GPU
 
@@ -357,19 +349,19 @@ factor_kernel(const FactorDesc* __restrict__ descs, const uint32_t* __restrict__
         pt_ahead = next_tile(pt_ahead);
       }
 
-      // coordinates (and, in error mode, the frozen correspondences) of a tile are loaded into registers one tile ahead
-      // of their use: the L2 prefetch above brings them close, this takes the remaining L2 round trip off the chain
+      // coordinates (and, in error mode, the frozen correspondences) of a tile, read at the start of its iteration: the L2
+      // prefetch above has brought them close
       struct Coords {
         PT x[kPPL], y[kPPL], z[kPPL];
         int cid[kPPL];
       };
-      auto load_coords = [&](uint32_t pt, bool in_run) {
+      auto load_coords = [&](uint32_t pt) {
         Coords c;
         const uint32_t b0 = pt * kTile + p * kWarpPoints + lane;
 #pragma unroll
         for (int k = 0; k < kPPL; k++) {
           const uint32_t i = b0 + k * 32;
-          const uint32_t j = (in_run && i < n) ? i : 0u;  // out-of-range lanes read element 0 (always allocated) and are masked through ok
+          const uint32_t j = i < n ? i : 0u;  // out-of-range lanes read element 0 (always allocated) and are masked through ok
           c.x[k] = __ldg(px + j);
           c.y[k] = __ldg(px + n_pad + j);
           c.z[k] = __ldg(px + 2 * n_pad + j);
@@ -378,19 +370,11 @@ factor_kernel(const FactorDesc* __restrict__ descs, const uint32_t* __restrict__
         }
         return c;
       };
-#if B2_WS_COORDS_AHEAD
-      Coords c_next = load_coords(pt_cur, tile < run_end);
-#endif
 #pragma unroll 1
       for (; tile < run_end; tile++, pt_cur = next_tile(pt_cur), pt_ahead = next_tile(pt_ahead)) {
         if (tile + kPrefetchAhead < run_end) prefetch_tile(pt_ahead);
         const uint32_t base = pt_cur * kTile + p * kWarpPoints + lane;
-#if B2_WS_COORDS_AHEAD
-        const Coords c = c_next;
-        c_next = load_coords(next_tile(pt_cur), tile + 1 < run_end);
-#else
-        const Coords c = load_coords(pt_cur, true);
-#endif
+        const Coords c = load_coords(pt_cur);
         // kPPL independent points per lane: their dependent chains (rotate -> floor -> hash -> bucket group -> match) interleave
         double u[kPPL][3];
         int cx[kPPL], cy[kPPL], cz[kPPL], id[kPPL];
@@ -435,12 +419,7 @@ factor_kernel(const FactorDesc* __restrict__ descs, const uint32_t* __restrict__
               }
             } else {
               double sq;
-#if B2_WS_KD_SMEM_STACK
-              id[k] = kdtree_nn1_warp_smem(tv, __dadd_rn(u[k][0], tvec(0)), __dadd_rn(u[k][1], tvec(1)), __dadd_rn(u[k][2], tvec(2)), ok[k], max_sq, &sq,
-                                           dyn_smem + kRingBytes + static_cast<size_t>(p) * kKdSmemStackBytes, lane);
-#else
               id[k] = kdtree_nn1_warp(tv, __dadd_rn(u[k][0], tvec(0)), __dadd_rn(u[k][1], tvec(1)), __dadd_rn(u[k][2], tvec(2)), ok[k], max_sq, &sq);
-#endif
             }
             if (ok[k]) corr[base + k * 32] = id[k];
           }
@@ -461,14 +440,12 @@ factor_kernel(const FactorDesc* __restrict__ descs, const uint32_t* __restrict__
             const unsigned long long bits = static_cast<unsigned long long>(base + k * 32) | (static_cast<unsigned long long>(static_cast<uint32_t>(id[k])) << 32);
             ring[slot] = make_double2(u[k][0], u[k][1]);
             ring[kRing + slot] = make_double2(u[k][2], __longlong_as_double(static_cast<long long>(bits)));
-#if B2_WS_PREFETCH_OPERANDS
             // the accumulate warp will gather these: start them towards L2 now
             const char* rec = reinterpret_cast<const char*>(records + static_cast<size_t>(id[k]) * kRecordDoubles);
             prefetch_l2(rec);
             prefetch_l2(rec + 72);
-#endif
           }
-          if (B2_WS_PREFETCH_OPERANDS && KIND <= 1 && lane < 12) {
+          if (KIND <= 1 && lane < 12) {
             // covariance lines of this 32-point group: 6 planes x 2 halves of 16 points
             const uint32_t half = lane & 1, plane = lane >> 1;
             if ((mask[k] >> (16 * half)) & 0xffffu) prefetch_l2(cv + plane * n_pad + (base - lane) + k * 32 + 16 * half);
@@ -557,11 +534,7 @@ factor_kernel(const FactorDesc* __restrict__ descs, const uint32_t* __restrict__
         // Hand back the slots of every batch taken so far.  All lanes must have finished reading them: converge the warp,
         // then release (independent thread scheduling gives no such guarantee by itself).
         __syncwarp();
-#if B2_WS_HEAD_FENCE
         if (lane == 0) st_release(&sh.head[p], hd);
-#else
-        if (lane == 0) st_volatile(&sh.head[p], hd);
-#endif
         uint32_t nb = 0u;
         bool fin = false;
         {

@@ -49,27 +49,10 @@ __device__ __forceinline__ KdNodeGPU load_node(const KdNodeGPU* p) {
 // bound = max over the splits on the path that separate the lane's query from the subtree of (q_axis - thresh)^2, a node is
 // skipped only if best <= bound holds for every lane, and distances use the CPU path's operation order.
 // Must be called by all 32 lanes; lanes with active == false take part in the votes but never need anything.
-// Traversal stack of the packet walk.  The node stack is warp-uniform; the per-lane lower bounds are kept as float32 rounded
-// TOWARDS ZERO (a smaller lower bound only makes the walk visit a node it could have skipped: the search stays exact).
-// In shared memory: kKdSmemStackBytes per warp, laid out [level][lane]; in local memory when no shared block is given.
-constexpr int kKdSmemDepth = 32;  // the device build is balanced (depth <= ceil(log2(n / leaf)) + 1 <= 28 for 2^31 points)
-constexpr uint32_t kKdSmemStackBytes = kKdSmemDepth * (32u * 4u + 4u);
-struct KdSmemStack {
-  float* bound;    // [kKdSmemDepth][32]
-  uint32_t* node;  // [kKdSmemDepth]
-};
-__device__ __forceinline__ KdSmemStack kd_smem_stack(void* warp_block) {
-  KdSmemStack s;
-  s.bound = static_cast<float*>(warp_block);
-  s.node = reinterpret_cast<uint32_t*>(s.bound + kKdSmemDepth * 32);
-  return s;
-}
-
-template <bool SMEM>
-__device__ __forceinline__ int kdtree_nn1_warp_impl(const KdTreeView& t, double qx, double qy, double qz, bool active, double max_sq, double* out_sq, KdSmemStack ss, int lane) {
+__device__ __forceinline__ int kdtree_nn1_warp(const KdTreeView& t, double qx, double qy, double qz, bool active, double max_sq, double* out_sq) {
   constexpr unsigned kFull = 0xffffffffu;
-  uint32_t stack_node[SMEM ? 1 : kKdStackDepth];
-  double stack_bound[SMEM ? 1 : kKdStackDepth];
+  uint32_t stack_node[kKdStackDepth];
+  double stack_bound[kKdStackDepth];
   int sp = 0;
   double best = active ? max_sq : 0.0;
   int best_j = -1;
@@ -88,14 +71,8 @@ __device__ __forceinline__ int kdtree_nn1_warp_impl(const KdTreeView& t, double 
         const bool go_left = nl >= nr;                 // uniform: the side most needy lanes are on
         const bool mine = (left == go_left);           // this lane's query lies on the side we descend into
         const double sep = bound > d2 ? bound : d2;    // bound of the side this lane's query is NOT on
-        if (SMEM) {
-          if (sp >= kKdSmemDepth) __trap();
-          if (lane == 0) ss.node[sp] = go_left ? n.a + 1u : n.a;
-          ss.bound[sp * 32 + lane] = __double2float_rz(mine ? sep : bound);
-        } else {
-          stack_node[sp] = go_left ? n.a + 1u : n.a;
-          stack_bound[sp] = mine ? sep : bound;
-        }
+        stack_node[sp] = go_left ? n.a + 1u : n.a;
+        stack_bound[sp] = mine ? sep : bound;
         sp++;
         node_idx = go_left ? n.a : n.a + 1u;
         bound = mine ? bound : sep;
@@ -126,23 +103,11 @@ __device__ __forceinline__ int kdtree_nn1_warp_impl(const KdTreeView& t, double 
     }
     if (sp == 0) break;
     sp--;
-    if (SMEM) {
-      __syncwarp();  // lane 0's node store of this level is visible to the warp
-      node_idx = ss.node[sp];
-      bound = static_cast<double>(ss.bound[sp * 32 + lane]);
-    } else {
-      node_idx = stack_node[sp];
-      bound = stack_bound[sp];
-    }
+    node_idx = stack_node[sp];
+    bound = stack_bound[sp];
   }
   *out_sq = active ? best : max_sq;
   return active ? best_j : -1;
-}
-__device__ __forceinline__ int kdtree_nn1_warp(const KdTreeView& t, double qx, double qy, double qz, bool active, double max_sq, double* out_sq) {
-  return kdtree_nn1_warp_impl<false>(t, qx, qy, qz, active, max_sq, out_sq, KdSmemStack{nullptr, nullptr}, 0);
-}
-__device__ __forceinline__ int kdtree_nn1_warp_smem(const KdTreeView& t, double qx, double qy, double qz, bool active, double max_sq, double* out_sq, void* warp_stack_block, int lane) {
-  return kdtree_nn1_warp_impl<true>(t, qx, qy, qz, active, max_sq, out_sq, kd_smem_stack(warp_stack_block), lane);
 }
 
 // k nearest neighbours, packet form: like kdtree_nn1_warp, each lane additionally keeps its k best candidates, sorted by

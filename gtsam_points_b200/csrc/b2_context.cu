@@ -24,7 +24,7 @@ b2_status fail(b2_status st, const char* fmt, ...) {
 
 }  // namespace b2
 
-b2_status b2_ctx::ensure_stage(size_t host_bytes, size_t dev_bytes) {
+b2_status b2_ctx::ensure_stage(size_t host_bytes) {
   // the new buffer is allocated BEFORE the old one is released: a failed allocation leaves the context usable
   if (host_bytes > h_stage_bytes) {
     const size_t want = b2::round_up(host_bytes * 2, 4096);
@@ -36,14 +36,6 @@ b2_status b2_ctx::ensure_stage(size_t host_bytes, size_t dev_bytes) {
     }
     h_stage = fresh;
     h_stage_bytes = want;
-  }
-  if (dev_bytes > d_stage_bytes) {
-    const size_t want = b2::round_up(dev_bytes * 2, 4096);
-    void* fresh = nullptr;
-    B2_CUDA(cudaMalloc(&fresh, want));
-    if (d_stage) cudaFree(d_stage);
-    d_stage = fresh;
-    d_stage_bytes = want;
   }
   return B2_OK;
 }
@@ -112,7 +104,6 @@ b2_status b2_ctx_destroy(b2_ctx* ctx) {
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
   if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
-  if (ctx->d_stage) cudaFree(ctx->d_stage);
   if (ctx->h_done) cudaFreeHost(const_cast<unsigned int*>(ctx->h_done));
   if (ctx->d_done_counter) cudaFree(ctx->d_done_counter);
   if (ctx->owns_stream) cudaStreamDestroy(ctx->stream);

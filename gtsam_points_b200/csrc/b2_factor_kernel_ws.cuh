@@ -424,9 +424,9 @@ factor_kernel(const FactorDesc* __restrict__ descs, const uint32_t* __restrict__
               }
             } else if (KIND == 4) {
               // iVox: the neighbour voxels of the transformed point (offset order) through the bucket table, their point slots in
-              // order; the ivox's point counts travel in leaf_pts, slots per voxel | neighbour mode << 8 in pad1
-              id[k] = ok[k] ? ivox_nn1(buckets, bucket_mask, inv_leaf, records, static_cast<const uint32_t*>(dg->leaf_pts), static_cast<int>(dg->pad1 & 0xffu),
-                                       static_cast<int>(dg->pad1 >> 8), __dadd_rn(u[k][0], tvec(0)), __dadd_rn(u[k][1], tvec(1)), __dadd_rn(u[k][2], tvec(2)), max_sq, nullptr)
+              // order; the ivox's point counts travel in leaf_pts, slots per voxel | neighbour mode << 8 in ivox_slots_mode
+              id[k] = ok[k] ? ivox_nn1(buckets, bucket_mask, inv_leaf, records, static_cast<const uint32_t*>(dg->leaf_pts), static_cast<int>(dg->ivox_slots_mode & 0xffu),
+                                       static_cast<int>(dg->ivox_slots_mode >> 8), __dadd_rn(u[k][0], tvec(0)), __dadd_rn(u[k][1], tvec(1)), __dadd_rn(u[k][2], tvec(2)), max_sq, nullptr)
                             : -1;
             } else {
               double sq;

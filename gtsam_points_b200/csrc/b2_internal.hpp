@@ -78,8 +78,6 @@ struct b2_ctx {
   // pinned staging for poses (H2D) and results (D2H), grown on demand
   void* h_stage = nullptr;
   size_t h_stage_bytes = 0;
-  void* d_stage = nullptr;
-  size_t d_stage_bytes = 0;
 
   // completion word of zero-copy host calls (pinned + mapped) and the device counter behind it
   volatile unsigned int* h_done = nullptr;
@@ -87,7 +85,7 @@ struct b2_ctx {
   unsigned int* d_done_counter = nullptr;
   unsigned int done_seq = 0;
 
-  b2_status ensure_stage(size_t host_bytes, size_t dev_bytes);
+  b2_status ensure_stage(size_t host_bytes);
 };
 
 struct b2_cloud {

@@ -13,6 +13,8 @@
 //     correspondences in the caller's order.
 #include <cub/device/device_radix_sort.cuh>
 
+#include <memory>
+
 #include "b2_internal.hpp"
 
 namespace b2 {
@@ -145,13 +147,6 @@ __global__ void gather_planes_kernel(const double* __restrict__ pts, int pstride
   }
 }
 
-struct DevBuf {
-  void* p = nullptr;
-  ~DevBuf() {
-    if (p) cudaFree(p);
-  }
-};
-
 }  // namespace
 }  // namespace b2
 
@@ -171,25 +166,18 @@ b2_status b2_cloud_create(b2_ctx* ctx, const double* points, int point_stride, c
   B2_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
 
-  b2_cloud* c = new b2_cloud;
+  auto c = std::make_unique<b2_cloud>();
   c->ctx = ctx;
   c->n = n;
   c->n_pad = round_up(n > 0 ? n : 1, 32);
-  // every early return below (B2_CUDA included) releases the half-built cloud; disarmed right before success
-  struct Guard {
-    b2_cloud* c;
-    ~Guard() {
-      if (c) b2_cloud_destroy(c);
-    }
-  } guard{c};
 
-  DevBuf raw_p, raw_c, d_res, d_keys, d_keys2, d_idx, d_tmp;
+  DeviceBuffer raw_p, raw_c, d_res, d_keys, d_keys2, d_idx, d_tmp;
   if (n > 0) {
-    B2_CUDA(cudaMalloc(&raw_p.p, n * point_stride * sizeof(double)));
-    B2_CUDA(cudaMemcpyAsync(raw_p.p, points, n * point_stride * sizeof(double), cudaMemcpyHostToDevice, st));
+    B2_TRY(raw_p.alloc(n * point_stride * sizeof(double)));
+    B2_CUDA(cudaMemcpyAsync(raw_p.get(), points, n * point_stride * sizeof(double), cudaMemcpyHostToDevice, st));
     if (covs) {
-      B2_CUDA(cudaMalloc(&raw_c.p, n * cov_stride * sizeof(double)));
-      B2_CUDA(cudaMemcpyAsync(raw_c.p, covs, n * cov_stride * sizeof(double), cudaMemcpyHostToDevice, st));
+      B2_TRY(raw_c.alloc(n * cov_stride * sizeof(double)));
+      B2_CUDA(cudaMemcpyAsync(raw_c.get(), covs, n * cov_stride * sizeof(double), cudaMemcpyHostToDevice, st));
     }
   }
 
@@ -200,13 +188,12 @@ b2_status b2_cloud_create(b2_ctx* ctx, const double* points, int point_stride, c
   }
   h_res.flags = 0;
   if (n > 0) {
-    B2_CUDA(cudaMalloc(&d_res.p, sizeof(ScanResult)));
-    B2_CUDA(cudaMemcpyAsync(d_res.p, &h_res, sizeof(ScanResult), cudaMemcpyHostToDevice, st));
+    B2_TRY(d_res.alloc(sizeof(ScanResult)));
+    B2_CUDA(cudaMemcpyAsync(d_res.get(), &h_res, sizeof(ScanResult), cudaMemcpyHostToDevice, st));
     const int grid = static_cast<int>(std::min<size_t>((n + 255) / 256, static_cast<size_t>(ctx->sm_count) * 8));
-    scan_raw_kernel<<<grid, 256, 0, st>>>(static_cast<const double*>(raw_p.p), point_stride, static_cast<const double*>(raw_c.p), cov_stride, n,
-                                          static_cast<ScanResult*>(d_res.p));
+    scan_raw_kernel<<<grid, 256, 0, st>>>(raw_p.as<const double>(), point_stride, raw_c.as<const double>(), cov_stride, n, d_res.as<ScanResult>());
     B2_CUDA(cudaGetLastError());
-    B2_CUDA(cudaMemcpyAsync(&h_res, d_res.p, sizeof(ScanResult), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(cudaMemcpyAsync(&h_res, d_res.get(), sizeof(ScanResult), cudaMemcpyDeviceToHost, st));
     B2_CUDA(cudaStreamSynchronize(st));
     if (h_res.flags & 4u) {
       return fail(B2_ERR_INVALID_ARGUMENT, "b2_cloud_create: non-finite coordinate or covariance entry");
@@ -219,8 +206,6 @@ b2_status b2_cloud_create(b2_ctx* ctx, const double* points, int point_stride, c
   c->cov_bytes = covs ? (force64 ? 8 : (compact || !(h_res.flags & 2u)) ? 4 : 8) : 0;
   c->reordered = !(flags & B2_CLOUD_NO_REORDER) && n > 1;
 
-  auto cleanup_fail = [&](b2_status s) { return s; };  // the guard above releases the cloud
-
   // Morton permutation
   if (c->reordered) {
     double mn[3], mx[3];
@@ -230,58 +215,43 @@ b2_status b2_cloud_create(b2_ctx* ctx, const double* points, int point_stride, c
     }
     const double extent = std::max(std::max(mx[0] - mn[0], mx[1] - mn[1]), std::max(mx[2] - mn[2], 1e-9));
     const double scale = 65535.0 / extent;
-    cudaError_t e;
-    if ((e = cudaMalloc(&d_keys.p, n * sizeof(unsigned long long))) != cudaSuccess || (e = cudaMalloc(&d_keys2.p, n * sizeof(unsigned long long))) != cudaSuccess ||
-        (e = cudaMalloc(&d_idx.p, n * sizeof(uint32_t))) != cudaSuccess || (e = cudaMalloc(reinterpret_cast<void**>(&c->d_perm), n * sizeof(uint32_t))) != cudaSuccess) {
-      return cleanup_fail(fail(B2_ERR_OUT_OF_MEMORY, "b2_cloud_create: %s", cudaGetErrorString(e)));
-    }
-    morton_keys_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(static_cast<const double*>(raw_p.p), point_stride, n, mn[0], mn[1], mn[2], scale,
-                                                                              static_cast<unsigned long long*>(d_keys.p), static_cast<uint32_t*>(d_idx.p));
-    size_t tmp_bytes = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, static_cast<unsigned long long*>(d_keys.p), static_cast<unsigned long long*>(d_keys2.p),
-                                    static_cast<uint32_t*>(d_idx.p), c->d_perm, static_cast<int>(n), 0, 48, st);
-    if ((e = cudaMalloc(&d_tmp.p, tmp_bytes ? tmp_bytes : 16)) != cudaSuccess) return cleanup_fail(fail(B2_ERR_OUT_OF_MEMORY, "b2_cloud_create: %s", cudaGetErrorString(e)));
-    e = cub::DeviceRadixSort::SortPairs(d_tmp.p, tmp_bytes, static_cast<unsigned long long*>(d_keys.p), static_cast<unsigned long long*>(d_keys2.p),
-                                        static_cast<uint32_t*>(d_idx.p), c->d_perm, static_cast<int>(n), 0, 48, st);
-    if (e != cudaSuccess) return cleanup_fail(fail(B2_ERR_CUDA, "b2_cloud_create: radix sort: %s", cudaGetErrorString(e)));
-    c->device_bytes += n * sizeof(uint32_t);
+    B2_TRY(d_keys.alloc(n * sizeof(unsigned long long)));
+    B2_TRY(d_keys2.alloc(n * sizeof(unsigned long long)));
+    B2_TRY(d_idx.alloc(n * sizeof(uint32_t)));
+    B2_TRY(c->d_perm.alloc(n * sizeof(uint32_t)));
+    morton_keys_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(raw_p.as<const double>(), point_stride, n, mn[0], mn[1], mn[2], scale,
+                                                                              d_keys.as<unsigned long long>(), d_idx.as<uint32_t>());
+    B2_TRY(cub_run(d_tmp, st, [&](void* t, size_t& b) {
+      return cub::DeviceRadixSort::SortPairs(t, b, d_keys.as<unsigned long long>(), d_keys2.as<unsigned long long>(), d_idx.as<uint32_t>(), c->d_perm.as<uint32_t>(),
+                                             static_cast<int>(n), 0, 48, st);
+    }));
   }
 
   // planes
-  {
-    cudaError_t e;
-    if ((e = cudaMalloc(&c->d_points, 3 * c->n_pad * c->point_bytes)) != cudaSuccess) return cleanup_fail(fail(B2_ERR_OUT_OF_MEMORY, "b2_cloud_create: %s", cudaGetErrorString(e)));
-    c->device_bytes += 3 * c->n_pad * c->point_bytes;
-    if (covs) {
-      if ((e = cudaMalloc(&c->d_covs, 6 * c->n_pad * c->cov_bytes)) != cudaSuccess) return cleanup_fail(fail(B2_ERR_OUT_OF_MEMORY, "b2_cloud_create: %s", cudaGetErrorString(e)));
-      c->device_bytes += 6 * c->n_pad * c->cov_bytes;
-    }
-    const unsigned grid = static_cast<unsigned>((c->n_pad + 255) / 256);
-    const double* rp = static_cast<const double*>(raw_p.p);
-    const double* rc = static_cast<const double*>(raw_c.p);
-    if (c->point_bytes == 4 && c->cov_bytes != 8)
-      gather_planes_kernel<float, float><<<grid, 256, 0, st>>>(rp, point_stride, rc, cov_stride, c->d_perm, n, c->n_pad, static_cast<float*>(c->d_points), static_cast<float*>(c->d_covs));
-    else if (c->point_bytes == 4)
-      gather_planes_kernel<float, double><<<grid, 256, 0, st>>>(rp, point_stride, rc, cov_stride, c->d_perm, n, c->n_pad, static_cast<float*>(c->d_points), static_cast<double*>(c->d_covs));
-    else if (c->cov_bytes != 8)
-      gather_planes_kernel<double, float><<<grid, 256, 0, st>>>(rp, point_stride, rc, cov_stride, c->d_perm, n, c->n_pad, static_cast<double*>(c->d_points), static_cast<float*>(c->d_covs));
-    else
-      gather_planes_kernel<double, double><<<grid, 256, 0, st>>>(rp, point_stride, rc, cov_stride, c->d_perm, n, c->n_pad, static_cast<double*>(c->d_points), static_cast<double*>(c->d_covs));
-    if ((e = cudaGetLastError()) != cudaSuccess) return cleanup_fail(fail(B2_ERR_CUDA, "b2_cloud_create: gather: %s", cudaGetErrorString(e)));
-    if ((e = cudaStreamSynchronize(st)) != cudaSuccess) return cleanup_fail(fail(B2_ERR_CUDA, "b2_cloud_create: %s", cudaGetErrorString(e)));
-  }
+  B2_TRY(c->d_points.alloc(3 * c->n_pad * c->point_bytes));
+  if (covs) B2_TRY(c->d_covs.alloc(6 * c->n_pad * c->cov_bytes));
+  const unsigned grid = static_cast<unsigned>((c->n_pad + 255) / 256);
+  const double* rp = raw_p.as<const double>();
+  const double* rc = raw_c.as<const double>();
+  const uint32_t* perm = c->d_perm.as<const uint32_t>();
+  if (c->point_bytes == 4 && c->cov_bytes != 8)
+    gather_planes_kernel<float, float><<<grid, 256, 0, st>>>(rp, point_stride, rc, cov_stride, perm, n, c->n_pad, c->d_points.as<float>(), c->d_covs.as<float>());
+  else if (c->point_bytes == 4)
+    gather_planes_kernel<float, double><<<grid, 256, 0, st>>>(rp, point_stride, rc, cov_stride, perm, n, c->n_pad, c->d_points.as<float>(), c->d_covs.as<double>());
+  else if (c->cov_bytes != 8)
+    gather_planes_kernel<double, float><<<grid, 256, 0, st>>>(rp, point_stride, rc, cov_stride, perm, n, c->n_pad, c->d_points.as<double>(), c->d_covs.as<float>());
+  else
+    gather_planes_kernel<double, double><<<grid, 256, 0, st>>>(rp, point_stride, rc, cov_stride, perm, n, c->n_pad, c->d_points.as<double>(), c->d_covs.as<double>());
+  B2_CUDA(cudaGetLastError());
+  B2_CUDA(cudaStreamSynchronize(st));
 
-  guard.c = nullptr;
-  *out = c;
+  *out = c.release();
   return B2_OK;
 }
 
 b2_status b2_cloud_destroy(b2_cloud* c) {
   if (!c) return B2_OK;
   cudaSetDevice(c->ctx->device);
-  if (c->d_points) cudaFree(c->d_points);
-  if (c->d_covs) cudaFree(c->d_covs);
-  if (c->d_perm) cudaFree(c->d_perm);
   delete c;
   return B2_OK;
 }
@@ -293,7 +263,7 @@ b2_status b2_cloud_get_info(const b2_cloud* c, b2_cloud_info* info) {
   info->cov_bytes = c->cov_bytes;
   info->reordered = c->reordered ? 1 : 0;
   info->reserved = 0;
-  info->device_bytes = c->device_bytes;
+  info->device_bytes = c->device_bytes();
   return B2_OK;
 }
 

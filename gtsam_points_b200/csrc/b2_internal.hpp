@@ -4,10 +4,13 @@
 
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
+#include <initializer_list>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/b2points.h"
@@ -37,6 +40,93 @@ b2_status fail(b2_status st, const char* fmt, ...);
     b2_status _s = (expr);         \
     if (_s != B2_OK) return _s;    \
   } while (0)
+
+// ---- device memory --------------------------------------------------------------------------------
+// One cudaMalloc allocation and its size in bytes.  Move-only: a move hands the allocation over, a copy does not compile.
+// The destructor frees without selecting a device.  That is safe because a handle is destroyed, and a scratch buffer goes out
+// of scope, while its device is current: every *_destroy calls cudaSetDevice first, every other entry point before it allocates.
+class DeviceBuffer {
+ public:
+  DeviceBuffer() = default;
+  DeviceBuffer(const DeviceBuffer&) = delete;
+  DeviceBuffer& operator=(const DeviceBuffer&) = delete;
+  DeviceBuffer(DeviceBuffer&& o) noexcept : p_(std::exchange(o.p_, nullptr)), bytes_(std::exchange(o.bytes_, 0)) {}
+  DeviceBuffer& operator=(DeviceBuffer&& o) noexcept {
+    if (this != &o) {
+      reset();
+      p_ = std::exchange(o.p_, nullptr);
+      bytes_ = std::exchange(o.bytes_, 0);
+    }
+    return *this;
+  }
+  ~DeviceBuffer() { reset(); }
+
+  // frees what the buffer holds, then allocates `bytes`; B2_CUDA's status on failure (the buffer is then empty)
+  b2_status alloc(size_t bytes) {
+    reset();
+    const cudaError_t e = cudaMalloc(&p_, bytes);
+    if (e != cudaSuccess) {
+      p_ = nullptr;
+      return fail(e == cudaErrorMemoryAllocation ? B2_ERR_OUT_OF_MEMORY : B2_ERR_CUDA, "cudaMalloc(%zu bytes) -> %s", bytes, cudaGetErrorString(e));
+    }
+    bytes_ = bytes;
+    return B2_OK;
+  }
+  void reset() {
+    if (p_) cudaFree(p_);
+    p_ = nullptr;
+    bytes_ = 0;
+  }
+  void* get() const { return p_; }
+  template <typename T>
+  T* as() const {
+    return static_cast<T*>(p_);
+  }
+  size_t bytes() const { return bytes_; }
+  explicit operator bool() const { return p_ != nullptr; }
+
+ private:
+  void* p_ = nullptr;
+  size_t bytes_ = 0;
+};
+
+// ---- CUB two-phase calls ---------------------------------------------------------------------------
+// A CUB device algorithm is written once, as `call(void* temp, size_t& temp_bytes) -> cudaError_t`: called with temp == nullptr
+// it only reports the temporary storage it needs.
+
+template <typename Call>
+cudaError_t cub_query(Call& call, size_t& need) {
+  size_t bytes = 0;
+  const cudaError_t e = call(nullptr, bytes);
+  need = std::max(need, bytes);
+  return e;
+}
+
+// Makes `scratch` large enough for every call given (16 bytes at least), so calls that share it share one allocation.  A scratch
+// that already holds memory is replaced only after `st` has drained, since queued work may still use it.
+template <typename... Calls>
+b2_status cub_reserve(DeviceBuffer& scratch, cudaStream_t st, Calls&... calls) {
+  size_t need = 16;
+  for (cudaError_t e : {cub_query(calls, need)...}) B2_CUDA(e);
+  if (scratch.bytes() >= need) return B2_OK;
+  if (scratch) B2_CUDA(cudaStreamSynchronize(st));
+  return scratch.alloc(need);
+}
+
+// Runs `call` with `scratch` as its temporary storage; cub_reserve has sized `scratch` for it.
+template <typename Call>
+b2_status cub_launch(DeviceBuffer& scratch, Call&& call) {
+  size_t bytes = scratch.bytes();
+  B2_CUDA(call(scratch.get(), bytes));
+  return B2_OK;
+}
+
+// Asks for the temporary storage of `call`, grows `scratch` to it if needed, then runs `call`.
+template <typename Call>
+b2_status cub_run(DeviceBuffer& scratch, cudaStream_t st, Call&& call) {
+  B2_TRY(cub_reserve(scratch, st, call));
+  return cub_launch(scratch, call);
+}
 
 inline size_t round_up(size_t x, size_t m) { return (x + m - 1) / m * m; }
 inline uint64_t next_pow2(uint64_t x) {
@@ -95,10 +185,10 @@ struct b2_cloud {
   int point_bytes = 0;   // 4 or 8
   int cov_bytes = 0;     // 0, 4 or 8
   bool reordered = false;
-  void* d_points = nullptr;  // 3 planes (x, y, z) of n_pad elements
-  void* d_covs = nullptr;    // 6 planes (c00, c01, c02, c11, c12, c22) of n_pad elements
-  uint32_t* d_perm = nullptr;  // stored position -> caller index (nullptr if not reordered)
-  size_t device_bytes = 0;
+  b2::DeviceBuffer d_points;  // 3 planes (x, y, z) of n_pad elements
+  b2::DeviceBuffer d_covs;    // 6 planes (c00, c01, c02, c11, c12, c22) of n_pad elements
+  b2::DeviceBuffer d_perm;    // uint32: stored position -> caller index (empty if not reordered)
+  size_t device_bytes() const { return d_points.bytes() + d_covs.bytes() + d_perm.bytes(); }
 };
 
 struct b2_voxelmap {
@@ -107,18 +197,18 @@ struct b2_voxelmap {
   double inv_resolution = 0.0;
   size_t num_voxels = 0;
   size_t num_buckets = 0;  // power of two
-  b2::VoxelBucket* d_buckets = nullptr;
-  double* d_records = nullptr;   // num_voxels x 10
-  int32_t* d_coords = nullptr;   // num_voxels x 3 (id order), kept for download
-  size_t device_bytes = 0;
+  b2::DeviceBuffer d_buckets;  // num_buckets VoxelBucket
+  b2::DeviceBuffer d_records;  // double: capacity x rec_doubles
+  b2::DeviceBuffer d_coords;   // int32: capacity x 3 (id order), kept for download
   // incremental insertion state (ann/incremental_voxelmap.hpp:13-28): LRU bookkeeping as in the CPU map
-  uint32_t* d_lru = nullptr;     // per voxel: lru_counter value of the last insert() that touched it
+  b2::DeviceBuffer d_lru;        // uint32 per voxel: lru_counter value of the last insert() that touched it
   size_t capacity = 0;           // voxels the record / coord / lru arrays can hold
   size_t lru_horizon = 10, lru_clear_cycle = 10, lru_counter = 0;
   uint64_t generation = 0;       // bumped whenever the device pointers / voxel ids change: factor sets refresh their descriptors
   // per-voxel payload: kRecordDoubles for a Gaussian voxel map; an iVox keeps `stride` point records per voxel plus a point count
   size_t rec_doubles = b2::kRecordDoubles;
-  uint32_t* d_counts = nullptr;  // iVox only: points stored per voxel (slots 0..count-1 of its records are occupied)
+  b2::DeviceBuffer d_counts;     // iVox only, uint32: points stored per voxel (slots 0..count-1 of its records are occupied)
+  size_t device_bytes() const { return d_buckets.bytes() + d_records.bytes() + d_coords.bytes() + d_lru.bytes() + d_counts.bytes(); }
 };
 
 // IncrementalVoxelMap<FlatContainer> / iVox (ann/incremental_voxelmap.hpp, ann/flat_container.hpp, ann/ivox.hpp): the voxel-keyed
@@ -136,12 +226,11 @@ struct b2_kdtree {
   b2_ctx* ctx = nullptr;
   size_t n = 0;
   size_t num_nodes = 0;
-  b2::KdNodeGPU* d_nodes = nullptr;
-  void* d_leaf_points = nullptr;     // leaf-order records: float4 (x, y, z, 0) if leaf_f32 else 4 doubles (x, y, z, 0)
-  bool leaf_f32 = false;             // every coordinate is exactly float32-representable
+  b2::DeviceBuffer d_nodes;        // KdNodeGPU
+  b2::DeviceBuffer d_leaf_points;  // leaf-order records: float4 (x, y, z, 0) if leaf_f32 else 4 doubles (x, y, z, 0)
+  bool leaf_f32 = false;           // every coordinate is exactly float32-representable
   size_t n_pad = 0;
-  uint32_t* d_leaf_index = nullptr;  // leaf position -> caller index
-  size_t device_bytes = 0;
+  b2::DeviceBuffer d_leaf_index;   // uint32: leaf position -> caller index
 };
 
 enum b2_factor_kind { B2_FACTOR_VGICP = 0, B2_FACTOR_GICP = 1, B2_FACTOR_ICP = 2, B2_FACTOR_ICP_PLANE = 3, B2_FACTOR_GICP_IVOX = 4 };
@@ -160,9 +249,9 @@ struct b2_factor {
   double last_corr_delta[16] = {0};
   bool has_corr = false;  // correspondences have been established at last_corr_delta
   uint64_t params_gen = 0;  // bumped by every setter that changes a value factor sets have copied into their device descriptors
-  int32_t* d_corr = nullptr;       // per stored source position: voxel id / target leaf position, -1 = none
-  double* d_target_records = nullptr;  // GICP: target records in leaf order (Nt x 10), owned
-  double* d_lin_pose = nullptr;        // 16 doubles: the linearization point, written by the linearize kernel's epilogue
+  b2::DeviceBuffer d_corr;            // int32 per stored source position: voxel id / target leaf position, -1 = none
+  b2::DeviceBuffer d_target_records;  // double: kd-tree factors' target records in leaf order (Nt x 10)
+  b2::DeviceBuffer d_lin_pose;        // 16 doubles: the linearization point, written by the linearize kernel's epilogue
   bool linearized = false;
   uint64_t corr_gen = 0;  // iVox GICP: map generation the stored correspondences were associated against
   double lin_delta[16] = {0};

@@ -18,6 +18,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <memory>
 #include <vector>
 
 #include <cub/cub.cuh>
@@ -186,14 +187,6 @@ __global__ void knn1_kernel(KdTreeView tree, const double* __restrict__ q, int q
   if (out_sq) out_sq[i] = sq;
 }
 
-struct DevBuf {
-  void* p = nullptr;
-  ~DevBuf() {
-    if (p) cudaFree(p);
-  }
-};
-
-
 // ---- k nearest neighbours (k <= B2_KNN_MAX_K) and covariance estimation on top of it ------------------------------------
 constexpr int kKnnWarps = 4;  // warps per CTA of the k-NN kernels (scratch: k x 32 x 12 bytes per warp)
 
@@ -340,6 +333,8 @@ __global__ void __launch_bounds__(kKnnWarps * 32) covariance_kernel(KdTreeView v
 
 size_t knn_smem_bytes(int k) { return static_cast<size_t>(kKnnWarps) * k * 32 * (sizeof(double) + sizeof(int)); }
 
+KdTreeView tree_view(const b2_kdtree* t) { return KdTreeView{t->d_nodes.as<const KdNodeGPU>(), t->d_leaf_points.get(), t->leaf_f32 ? 1 : 0}; }
+
 }  // namespace
 }  // namespace b2
 
@@ -357,144 +352,121 @@ b2_status b2_kdtree_create(b2_ctx* ctx, const double* points, int point_stride, 
   B2_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
 
-  b2_kdtree* t = new b2_kdtree;
+  auto t = std::make_unique<b2_kdtree>();
   t->ctx = ctx;
   t->n = n;
   t->n_pad = round_up(std::max<size_t>(n, 1), 32);
-  auto bail = [&](b2_status stt) {
-    b2_kdtree_destroy(t);
-    return stt;
-  };
-#define KD_CUDA(expr)                                                                                                     \
-  do {                                                                                                                    \
-    cudaError_t _e = (expr);                                                                                              \
-    if (_e != cudaSuccess) return bail(fail(_e == cudaErrorMemoryAllocation ? B2_ERR_OUT_OF_MEMORY : B2_ERR_CUDA, "b2_kdtree_create: %s -> %s", #expr, cudaGetErrorString(_e))); \
-  } while (0)
 
   if (n == 0) {  // an empty tree: one empty leaf
     const KdNodeGPU root{0.0, 0u, 4u};
-    KD_CUDA(cudaMalloc(reinterpret_cast<void**>(&t->d_nodes), sizeof(KdNodeGPU)));
-    KD_CUDA(cudaMalloc(&t->d_leaf_points, 32));
-    KD_CUDA(cudaMalloc(reinterpret_cast<void**>(&t->d_leaf_index), sizeof(uint32_t)));
-    KD_CUDA(cudaMemcpyAsync(t->d_nodes, &root, sizeof(root), cudaMemcpyHostToDevice, st));
-    KD_CUDA(cudaStreamSynchronize(st));
+    B2_TRY(t->d_nodes.alloc(sizeof(KdNodeGPU)));
+    B2_TRY(t->d_leaf_points.alloc(32));
+    B2_TRY(t->d_leaf_index.alloc(sizeof(uint32_t)));
+    B2_CUDA(cudaMemcpyAsync(t->d_nodes.get(), &root, sizeof(root), cudaMemcpyHostToDevice, st));
+    B2_CUDA(cudaStreamSynchronize(st));
     t->num_nodes = 1;
     t->leaf_f32 = true;
-    *out = t;
+    *out = t.release();
     return B2_OK;
   }
 
   const unsigned grid_n = static_cast<unsigned>((n + 255) / 256);
-  DevBuf d_pts, d_flags2, d_orderB, d_keysA, d_keysB, d_tmp, d_levelA, d_levelB, d_flag, d_rank, d_bbox, d_axis, d_segb, d_sege, d_scan_tmp;
-  KD_CUDA(cudaMalloc(&d_pts.p, n * point_stride * sizeof(double)));
-  KD_CUDA(cudaMemcpyAsync(d_pts.p, points, n * point_stride * sizeof(double), cudaMemcpyHostToDevice, st));
-  const double* dp = static_cast<const double*>(d_pts.p);
+  DeviceBuffer d_pts, d_flags2, d_orderB, d_keysA, d_keysB, d_tmp, d_levelA, d_levelB, d_flag, d_rank, d_bbox, d_axis, d_segb, d_sege, d_scan_tmp;
+  B2_TRY(d_pts.alloc(n * point_stride * sizeof(double)));
+  B2_CUDA(cudaMemcpyAsync(d_pts.get(), points, n * point_stride * sizeof(double), cudaMemcpyHostToDevice, st));
+  const double* dp = d_pts.as<const double>();
 
   // point scan: identity permutation, "is every coordinate float32-representable", "is every coordinate finite"
-  KD_CUDA(cudaMalloc(reinterpret_cast<void**>(&t->d_leaf_index), n * sizeof(uint32_t)));
-  KD_CUDA(cudaMalloc(&d_orderB.p, n * sizeof(uint32_t)));
-  KD_CUDA(cudaMalloc(&d_flags2.p, 2 * sizeof(unsigned int)));
-  KD_CUDA(cudaMemsetAsync(d_flags2.p, 0, 2 * sizeof(unsigned int), st));
-  uint32_t* order = t->d_leaf_index;                     // the two permutation buffers swap roles level by level;
-  uint32_t* order_alt = static_cast<uint32_t*>(d_orderB.p);  // the final one is copied into t->d_leaf_index if needed
-  scan_points_kernel<<<grid_n, 256, 0, st>>>(dp, point_stride, n, static_cast<unsigned int*>(d_flags2.p), static_cast<unsigned int*>(d_flags2.p) + 1, order);
-  KD_CUDA(cudaGetLastError());
+  B2_TRY(t->d_leaf_index.alloc(n * sizeof(uint32_t)));
+  B2_TRY(d_orderB.alloc(n * sizeof(uint32_t)));
+  B2_TRY(d_flags2.alloc(2 * sizeof(unsigned int)));
+  B2_CUDA(cudaMemsetAsync(d_flags2.get(), 0, 2 * sizeof(unsigned int), st));
+  uint32_t* order = t->d_leaf_index.as<uint32_t>();  // the two permutation buffers swap roles level by level;
+  uint32_t* order_alt = d_orderB.as<uint32_t>();     // the final one is copied into t->d_leaf_index if needed
+  scan_points_kernel<<<grid_n, 256, 0, st>>>(dp, point_stride, n, d_flags2.as<unsigned int>(), d_flags2.as<unsigned int>() + 1, order);
+  B2_CUDA(cudaGetLastError());
   unsigned int h_flags2[2] = {0u, 0u};
-  KD_CUDA(cudaMemcpyAsync(h_flags2, d_flags2.p, sizeof(h_flags2), cudaMemcpyDeviceToHost, st));
-  KD_CUDA(cudaStreamSynchronize(st));
-  if (h_flags2[1]) return bail(fail(B2_ERR_INVALID_ARGUMENT, "b2_kdtree_create: non-finite coordinate"));
+  B2_CUDA(cudaMemcpyAsync(h_flags2, d_flags2.get(), sizeof(h_flags2), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  if (h_flags2[1]) return fail(B2_ERR_INVALID_ARGUMENT, "b2_kdtree_create: non-finite coordinate");
   t->leaf_f32 = h_flags2[0] == 0u;
 
   const size_t max_nodes = 2 * n + 1;
   const size_t max_level = n / 2 + 2;  // nodes per level (every node of a level below the root holds >= kMaxLeaf / 2 >= 2 points)
-  KD_CUDA(cudaMalloc(reinterpret_cast<void**>(&t->d_nodes), max_nodes * sizeof(KdNodeGPU)));
-  KD_CUDA(cudaMalloc(&d_keysA.p, n * sizeof(unsigned long long)));
-  KD_CUDA(cudaMalloc(&d_keysB.p, n * sizeof(unsigned long long)));
-  KD_CUDA(cudaMalloc(&d_levelA.p, max_level * sizeof(Range)));
-  KD_CUDA(cudaMalloc(&d_levelB.p, max_level * sizeof(Range)));
-  KD_CUDA(cudaMalloc(&d_flag.p, max_level * sizeof(uint32_t)));
-  KD_CUDA(cudaMalloc(&d_rank.p, max_level * sizeof(uint32_t)));
-  KD_CUDA(cudaMalloc(&d_bbox.p, max_level * 6 * sizeof(unsigned long long)));
-  KD_CUDA(cudaMalloc(&d_axis.p, max_level * sizeof(int)));
-  KD_CUDA(cudaMalloc(&d_segb.p, max_level * sizeof(uint32_t)));
-  KD_CUDA(cudaMalloc(&d_sege.p, max_level * sizeof(uint32_t)));
-  size_t scan_bytes = 0;
-  KD_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, static_cast<const uint32_t*>(d_flag.p), static_cast<uint32_t*>(d_rank.p), static_cast<int>(max_level), st));
-  KD_CUDA(cudaMalloc(&d_scan_tmp.p, std::max<size_t>(scan_bytes, 16)));
-  size_t sort_bytes = 0;
+  B2_TRY(t->d_nodes.alloc(max_nodes * sizeof(KdNodeGPU)));
+  B2_TRY(d_keysA.alloc(n * sizeof(unsigned long long)));
+  B2_TRY(d_keysB.alloc(n * sizeof(unsigned long long)));
+  B2_TRY(d_levelA.alloc(max_level * sizeof(Range)));
+  B2_TRY(d_levelB.alloc(max_level * sizeof(Range)));
+  B2_TRY(d_flag.alloc(max_level * sizeof(uint32_t)));
+  B2_TRY(d_rank.alloc(max_level * sizeof(uint32_t)));
+  B2_TRY(d_bbox.alloc(max_level * 6 * sizeof(unsigned long long)));
+  B2_TRY(d_axis.alloc(max_level * sizeof(int)));
+  B2_TRY(d_segb.alloc(max_level * sizeof(uint32_t)));
+  B2_TRY(d_sege.alloc(max_level * sizeof(uint32_t)));
+  uint32_t* flag = d_flag.as<uint32_t>();
+  uint32_t* rank = d_rank.as<uint32_t>();
+  // rank = exclusive scan of the split flags of a level's `count` nodes; its scratch is sized once, for the largest level
+  auto scan_level = [&](size_t count) {
+    return [&, count](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, flag, rank, static_cast<int>(count), st); };
+  };
+  auto largest_scan = scan_level(max_level);
+  B2_TRY(cub_reserve(d_scan_tmp, st, largest_scan));
   const Range root{0u, static_cast<uint32_t>(n)};
-  KD_CUDA(cudaMemcpyAsync(d_levelA.p, &root, sizeof(root), cudaMemcpyHostToDevice, st));
-  Range* cur = static_cast<Range*>(d_levelA.p);
-  Range* nxt = static_cast<Range*>(d_levelB.p);
-  uint32_t* flag = static_cast<uint32_t*>(d_flag.p);
-  uint32_t* rank = static_cast<uint32_t*>(d_rank.p);
+  B2_CUDA(cudaMemcpyAsync(d_levelA.get(), &root, sizeof(root), cudaMemcpyHostToDevice, st));
+  Range* cur = d_levelA.as<Range>();
+  Range* nxt = d_levelB.as<Range>();
   uint32_t count = 1u, level_base = 0u, total = 1u;
   int depth = 0;
   while (count > 0u) {
-    if (++depth > kKdStackDepth) return bail(fail(B2_ERR_INVALID_STATE, "b2_kdtree_create: tree deeper than the traversal stack (%d levels)", kKdStackDepth));
+    if (++depth > kKdStackDepth) return fail(B2_ERR_INVALID_STATE, "b2_kdtree_create: tree deeper than the traversal stack (%d levels)", kKdStackDepth);
     const unsigned gl = (count + 255u) / 256u;
     classify_level_kernel<<<gl, 256, 0, st>>>(cur, count, flag);
-    KD_CUDA(cudaGetLastError());
-    KD_CUDA(cub::DeviceScan::ExclusiveSum(d_scan_tmp.p, scan_bytes, flag, rank, static_cast<int>(count), st));
+    B2_CUDA(cudaGetLastError());
+    B2_TRY(cub_launch(d_scan_tmp, scan_level(count)));
     uint32_t last_rank = 0u, last_flag = 0u;  // number of nodes to split on this level = rank[count-1] + flag[count-1]
-    KD_CUDA(cudaMemcpyAsync(&last_rank, rank + (count - 1u), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    KD_CUDA(cudaMemcpyAsync(&last_flag, flag + (count - 1u), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    KD_CUDA(cudaStreamSynchronize(st));
+    B2_CUDA(cudaMemcpyAsync(&last_rank, rank + (count - 1u), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(cudaMemcpyAsync(&last_flag, flag + (count - 1u), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(cudaStreamSynchronize(st));
     const uint32_t internal = last_rank + last_flag;
     if (internal > 0u) {
-      init_bbox_kernel<<<(internal * 6u + 255u) / 256u, 256, 0, st>>>(static_cast<unsigned long long*>(d_bbox.p), internal);
-      bbox_level_kernel<<<grid_n, 256, 0, st>>>(dp, point_stride, n, order, cur, count, flag, rank, static_cast<unsigned long long*>(d_bbox.p));
-      axis_level_kernel<<<gl, 256, 0, st>>>(cur, count, flag, rank, static_cast<const unsigned long long*>(d_bbox.p), static_cast<int*>(d_axis.p),
-                                            static_cast<uint32_t*>(d_segb.p), static_cast<uint32_t*>(d_sege.p));
-      keys_level_kernel<<<grid_n, 256, 0, st>>>(dp, point_stride, n, order, cur, count, flag, rank, static_cast<const int*>(d_axis.p),
-                                                static_cast<unsigned long long*>(d_keysA.p));
-      KD_CUDA(cudaGetLastError());
+      init_bbox_kernel<<<(internal * 6u + 255u) / 256u, 256, 0, st>>>(d_bbox.as<unsigned long long>(), internal);
+      bbox_level_kernel<<<grid_n, 256, 0, st>>>(dp, point_stride, n, order, cur, count, flag, rank, d_bbox.as<unsigned long long>());
+      axis_level_kernel<<<gl, 256, 0, st>>>(cur, count, flag, rank, d_bbox.as<const unsigned long long>(), d_axis.as<int>(), d_segb.as<uint32_t>(), d_sege.as<uint32_t>());
+      keys_level_kernel<<<grid_n, 256, 0, st>>>(dp, point_stride, n, order, cur, count, flag, rank, d_axis.as<const int>(), d_keysA.as<unsigned long long>());
+      B2_CUDA(cudaGetLastError());
       // positions outside the sorted segments (finished leaves) keep their element
-      KD_CUDA(cudaMemcpyAsync(order_alt, order, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
-      size_t need = 0;
-      KD_CUDA(cub::DeviceSegmentedSort::StableSortPairs(nullptr, need, static_cast<const unsigned long long*>(d_keysA.p), static_cast<unsigned long long*>(d_keysB.p),
-                                                        static_cast<const uint32_t*>(order), order_alt, static_cast<int>(n), static_cast<int>(internal),
-                                                        static_cast<const uint32_t*>(d_segb.p), static_cast<const uint32_t*>(d_sege.p), st));
-      if (need > sort_bytes) {
-        KD_CUDA(cudaStreamSynchronize(st));
-        if (d_tmp.p) cudaFree(d_tmp.p);
-        d_tmp.p = nullptr;
-        KD_CUDA(cudaMalloc(&d_tmp.p, need));
-        sort_bytes = need;
-      }
-      KD_CUDA(cub::DeviceSegmentedSort::StableSortPairs(d_tmp.p, need, static_cast<const unsigned long long*>(d_keysA.p), static_cast<unsigned long long*>(d_keysB.p),
-                                                        static_cast<const uint32_t*>(order), order_alt, static_cast<int>(n), static_cast<int>(internal),
-                                                        static_cast<const uint32_t*>(d_segb.p), static_cast<const uint32_t*>(d_sege.p), st));
+      B2_CUDA(cudaMemcpyAsync(order_alt, order, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
+      // the sort's scratch only grows, so later levels reuse it
+      B2_TRY(cub_run(d_tmp, st, [&](void* tmp, size_t& bytes) {
+        return cub::DeviceSegmentedSort::StableSortPairs(tmp, bytes, d_keysA.as<const unsigned long long>(), d_keysB.as<unsigned long long>(), static_cast<const uint32_t*>(order),
+                                                         order_alt, static_cast<int>(n), static_cast<int>(internal), d_segb.as<const uint32_t>(), d_sege.as<const uint32_t>(), st);
+      }));
       std::swap(order, order_alt);
     }
-    emit_level_kernel<<<gl, 256, 0, st>>>(dp, point_stride, order, cur, count, level_base, flag, rank, static_cast<const int*>(d_axis.p), total, t->d_nodes, nxt);
-    KD_CUDA(cudaGetLastError());
+    emit_level_kernel<<<gl, 256, 0, st>>>(dp, point_stride, order, cur, count, level_base, flag, rank, d_axis.as<const int>(), total, t->d_nodes.as<KdNodeGPU>(), nxt);
+    B2_CUDA(cudaGetLastError());
     level_base = total;
     total += 2u * internal;
     count = 2u * internal;
     std::swap(cur, nxt);
   }
   t->num_nodes = total;
-  if (order != t->d_leaf_index) KD_CUDA(cudaMemcpyAsync(t->d_leaf_index, order, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
+  if (order != t->d_leaf_index.as<uint32_t>()) B2_CUDA(cudaMemcpyAsync(t->d_leaf_index.get(), order, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
 
   // leaf-order point records: float32 when that is lossless, else float64
   const size_t rec_bytes = t->leaf_f32 ? 4 * sizeof(float) : 4 * sizeof(double);
-  KD_CUDA(cudaMalloc(&t->d_leaf_points, n * rec_bytes));
-  leaf_records_kernel<<<grid_n, 256, 0, st>>>(dp, point_stride, n, t->d_leaf_index, t->leaf_f32 ? 1 : 0, t->d_leaf_points);
-  KD_CUDA(cudaGetLastError());
-  KD_CUDA(cudaStreamSynchronize(st));
-  t->device_bytes = max_nodes * sizeof(KdNodeGPU) + n * rec_bytes + n * sizeof(uint32_t);
-#undef KD_CUDA
-  *out = t;
+  B2_TRY(t->d_leaf_points.alloc(n * rec_bytes));
+  leaf_records_kernel<<<grid_n, 256, 0, st>>>(dp, point_stride, n, t->d_leaf_index.as<const uint32_t>(), t->leaf_f32 ? 1 : 0, t->d_leaf_points.get());
+  B2_CUDA(cudaGetLastError());
+  B2_CUDA(cudaStreamSynchronize(st));
+  *out = t.release();
   return B2_OK;
 }
 
 b2_status b2_kdtree_destroy(b2_kdtree* t) {
   if (!t) return B2_OK;
   cudaSetDevice(t->ctx->device);
-  if (t->d_nodes) cudaFree(t->d_nodes);
-  if (t->d_leaf_points) cudaFree(t->d_leaf_points);
-  if (t->d_leaf_index) cudaFree(t->d_leaf_index);
   delete t;
   return B2_OK;
 }
@@ -507,17 +479,16 @@ b2_status b2_kdtree_knn1(const b2_kdtree* t, const double* queries, int query_st
   if (nq == 0) return B2_OK;
   B2_CUDA(cudaSetDevice(t->ctx->device));
   cudaStream_t st = t->ctx->stream;
-  DevBuf dq, di, ds;
-  B2_CUDA(cudaMalloc(&dq.p, nq * query_stride * sizeof(double)));
-  B2_CUDA(cudaMalloc(&di.p, nq * sizeof(long long)));
-  B2_CUDA(cudaMalloc(&ds.p, nq * sizeof(double)));
-  B2_CUDA(cudaMemcpyAsync(dq.p, queries, nq * query_stride * sizeof(double), cudaMemcpyHostToDevice, st));
-  KdTreeView view{t->d_nodes, t->d_leaf_points, t->leaf_f32 ? 1 : 0};
-  knn1_kernel<<<static_cast<unsigned>((nq + 127) / 128), 128, 0, st>>>(view, static_cast<const double*>(dq.p), query_stride, nq, max_sq_dist, t->d_leaf_index,
-                                                                      static_cast<long long*>(di.p), static_cast<double*>(ds.p));
+  DeviceBuffer dq, di, ds;
+  B2_TRY(dq.alloc(nq * query_stride * sizeof(double)));
+  B2_TRY(di.alloc(nq * sizeof(long long)));
+  B2_TRY(ds.alloc(nq * sizeof(double)));
+  B2_CUDA(cudaMemcpyAsync(dq.get(), queries, nq * query_stride * sizeof(double), cudaMemcpyHostToDevice, st));
+  knn1_kernel<<<static_cast<unsigned>((nq + 127) / 128), 128, 0, st>>>(tree_view(t), dq.as<const double>(), query_stride, nq, max_sq_dist, t->d_leaf_index.as<const uint32_t>(),
+                                                                      di.as<long long>(), ds.as<double>());
   B2_CUDA(cudaGetLastError());
-  if (out_index) B2_CUDA(cudaMemcpyAsync(out_index, di.p, nq * sizeof(long long), cudaMemcpyDeviceToHost, st));
-  if (out_sq_dist) B2_CUDA(cudaMemcpyAsync(out_sq_dist, ds.p, nq * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (out_index) B2_CUDA(cudaMemcpyAsync(out_index, di.get(), nq * sizeof(long long), cudaMemcpyDeviceToHost, st));
+  if (out_sq_dist) B2_CUDA(cudaMemcpyAsync(out_sq_dist, ds.get(), nq * sizeof(double), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
   return B2_OK;
 }
@@ -532,12 +503,11 @@ b2_status b2_kdtree_knn(const b2_kdtree* t, const double* queries, int query_str
   if (k == 1) return b2_kdtree_knn1(t, queries, query_stride, nq, max_sq_dist, out_index, out_sq_dist);
   B2_CUDA(cudaSetDevice(t->ctx->device));
   cudaStream_t st = t->ctx->stream;
-  DevBuf dq, di, ds;
-  B2_CUDA(cudaMalloc(&dq.p, nq * query_stride * sizeof(double)));
-  B2_CUDA(cudaMalloc(&di.p, nq * k * sizeof(long long)));
-  B2_CUDA(cudaMalloc(&ds.p, nq * k * sizeof(double)));
-  B2_CUDA(cudaMemcpyAsync(dq.p, queries, nq * query_stride * sizeof(double), cudaMemcpyHostToDevice, st));
-  KdTreeView view{t->d_nodes, t->d_leaf_points, t->leaf_f32 ? 1 : 0};
+  DeviceBuffer dq, di, ds;
+  B2_TRY(dq.alloc(nq * query_stride * sizeof(double)));
+  B2_TRY(di.alloc(nq * k * sizeof(long long)));
+  B2_TRY(ds.alloc(nq * k * sizeof(double)));
+  B2_CUDA(cudaMemcpyAsync(dq.get(), queries, nq * query_stride * sizeof(double), cudaMemcpyHostToDevice, st));
   const size_t smem = knn_smem_bytes(k);
   B2_CUDA(cudaFuncSetAttribute(reinterpret_cast<const void*>(knn_kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   if (t->n == 0) {
@@ -547,11 +517,11 @@ b2_status b2_kdtree_knn(const b2_kdtree* t, const double* queries, int query_str
     if (out_sq_dist) std::memcpy(out_sq_dist, sq.data(), sq.size() * sizeof(double));
     return B2_OK;
   }
-  knn_kernel<<<static_cast<unsigned>((nq + kKnnWarps * 32 - 1) / (kKnnWarps * 32)), kKnnWarps * 32, smem, st>>>(view, static_cast<const double*>(dq.p), query_stride, nq, k, max_sq_dist,
-                                                                                                             t->d_leaf_index, static_cast<long long*>(di.p), static_cast<double*>(ds.p));
+  knn_kernel<<<static_cast<unsigned>((nq + kKnnWarps * 32 - 1) / (kKnnWarps * 32)), kKnnWarps * 32, smem, st>>>(tree_view(t), dq.as<const double>(), query_stride, nq, k, max_sq_dist,
+                                                                                                             t->d_leaf_index.as<const uint32_t>(), di.as<long long>(), ds.as<double>());
   B2_CUDA(cudaGetLastError());
-  if (out_index) B2_CUDA(cudaMemcpyAsync(out_index, di.p, nq * k * sizeof(long long), cudaMemcpyDeviceToHost, st));
-  if (out_sq_dist) B2_CUDA(cudaMemcpyAsync(out_sq_dist, ds.p, nq * k * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (out_index) B2_CUDA(cudaMemcpyAsync(out_index, di.get(), nq * k * sizeof(long long), cudaMemcpyDeviceToHost, st));
+  if (out_sq_dist) B2_CUDA(cudaMemcpyAsync(out_sq_dist, ds.get(), nq * k * sizeof(double), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
   return B2_OK;
 }
@@ -564,15 +534,14 @@ b2_status b2_kdtree_estimate_covariances(const b2_kdtree* t, int k_neighbors, co
   B2_CUDA(cudaSetDevice(t->ctx->device));
   cudaStream_t st = t->ctx->stream;
   const double ev[3] = {eigen_values ? eigen_values[0] : 1e-3, eigen_values ? eigen_values[1] : 1.0, eigen_values ? eigen_values[2] : 1.0};  // covariance_estimation.hpp:19
-  DevBuf dc;
-  B2_CUDA(cudaMalloc(&dc.p, n * 9 * sizeof(double)));
-  KdTreeView view{t->d_nodes, t->d_leaf_points, t->leaf_f32 ? 1 : 0};
+  DeviceBuffer dc;
+  B2_TRY(dc.alloc(n * 9 * sizeof(double)));
   const size_t smem = knn_smem_bytes(k_neighbors);
   B2_CUDA(cudaFuncSetAttribute(reinterpret_cast<const void*>(covariance_kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-  covariance_kernel<<<static_cast<unsigned>((n + kKnnWarps * 32 - 1) / (kKnnWarps * 32)), kKnnWarps * 32, smem, st>>>(view, n, k_neighbors, ev[0], ev[1], ev[2], t->d_leaf_index,
-                                                                                                                 static_cast<double*>(dc.p));
+  covariance_kernel<<<static_cast<unsigned>((n + kKnnWarps * 32 - 1) / (kKnnWarps * 32)), kKnnWarps * 32, smem, st>>>(tree_view(t), n, k_neighbors, ev[0], ev[1], ev[2],
+                                                                                                                 t->d_leaf_index.as<const uint32_t>(), dc.as<double>());
   B2_CUDA(cudaGetLastError());
-  B2_CUDA(cudaMemcpyAsync(out_cov3x3, dc.p, n * 9 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(out_cov3x3, dc.get(), n * 9 * sizeof(double), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
   return B2_OK;
 }

@@ -21,23 +21,13 @@
 
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <vector>
 
 #include "b2_device.cuh"
 
 namespace b2 {
 namespace {
-
-struct DevBuf {
-  void* p = nullptr;
-  ~DevBuf() {
-    if (p) cudaFree(p);
-  }
-  template <typename T>
-  T* as() {
-    return static_cast<T*>(p);
-  }
-};
 
 __device__ __forceinline__ uint32_t bias32(int v) { return static_cast<uint32_t>(v) ^ 0x80000000u; }
 
@@ -429,36 +419,20 @@ struct MinU64 {
 // load factor <= 0.25 (see b2_device.cuh: one-round-trip lookups)
 size_t bucket_count_for(size_t num_voxels) { return static_cast<size_t>(next_pow2(std::max<uint64_t>(64, 4 * static_cast<uint64_t>(num_voxels)))); }
 
-void release_map(b2_voxelmap* vm) {
-  cudaSetDevice(vm->ctx->device);
-  if (vm->d_buckets) cudaFree(vm->d_buckets);
-  if (vm->d_records) cudaFree(vm->d_records);
-  if (vm->d_coords) cudaFree(vm->d_coords);
-  if (vm->d_lru) cudaFree(vm->d_lru);
-  if (vm->d_counts) cudaFree(vm->d_counts);
-  vm->d_buckets = nullptr, vm->d_records = nullptr, vm->d_coords = nullptr, vm->d_lru = nullptr, vm->d_counts = nullptr;
-}
-
-b2_status alloc_map(b2_ctx* ctx, double resolution, size_t V, b2_voxelmap** out) {
-  b2_voxelmap* vm = new b2_voxelmap;
-  vm->ctx = ctx;
-  vm->resolution = resolution;
-  vm->inv_resolution = 1.0 / resolution;  // ann/impl/incremental_voxelmap_impl.hpp:14
-  vm->num_voxels = V;
-  vm->num_buckets = bucket_count_for(V);
-  cudaError_t e;
-  const size_t vr = std::max<size_t>(V, 1);
-  vm->capacity = vr;
-  if ((e = cudaMalloc(reinterpret_cast<void**>(&vm->d_buckets), vm->num_buckets * sizeof(VoxelBucket))) != cudaSuccess ||
-      (e = cudaMalloc(reinterpret_cast<void**>(&vm->d_records), vr * kRecordDoubles * sizeof(double))) != cudaSuccess ||
-      (e = cudaMalloc(reinterpret_cast<void**>(&vm->d_coords), vr * 3 * sizeof(int32_t))) != cudaSuccess ||
-      (e = cudaMalloc(reinterpret_cast<void**>(&vm->d_lru), vr * sizeof(uint32_t))) != cudaSuccess ||
-      (e = cudaMemsetAsync(vm->d_lru, 0, vr * sizeof(uint32_t), ctx->stream)) != cudaSuccess) {
-    b2_voxelmap_destroy(vm);
-    return fail(B2_ERR_OUT_OF_MEMORY, "voxelmap allocation: %s", cudaGetErrorString(e));
-  }
-  vm->device_bytes = vm->num_buckets * sizeof(VoxelBucket) + vr * (kRecordDoubles * sizeof(double) + 3 * sizeof(int32_t) + sizeof(uint32_t));
-  *out = vm;
+// An empty Gaussian voxel map laid out for V voxels: a bucket table for V (contents left to the caller) and per-voxel arrays
+// for max(V, 1) voxels, LRU zeroed
+b2_status init_map(b2_voxelmap& vm, b2_ctx* ctx, double resolution, size_t V) {
+  vm.ctx = ctx;
+  vm.resolution = resolution;
+  vm.inv_resolution = 1.0 / resolution;  // ann/impl/incremental_voxelmap_impl.hpp:14
+  vm.num_voxels = V;
+  vm.num_buckets = bucket_count_for(V);
+  vm.capacity = std::max<size_t>(V, 1);
+  B2_TRY(vm.d_buckets.alloc(vm.num_buckets * sizeof(VoxelBucket)));
+  B2_TRY(vm.d_records.alloc(vm.capacity * kRecordDoubles * sizeof(double)));
+  B2_TRY(vm.d_coords.alloc(vm.capacity * 3 * sizeof(int32_t)));
+  B2_TRY(vm.d_lru.alloc(vm.capacity * sizeof(uint32_t)));
+  B2_CUDA(cudaMemsetAsync(vm.d_lru.get(), 0, vm.capacity * sizeof(uint32_t), ctx->stream));
   return B2_OK;
 }
 
@@ -467,38 +441,22 @@ b2_status reserve_voxels(b2_voxelmap* vm, size_t want) {
   if (want <= vm->capacity) return B2_OK;
   const size_t cap = std::max(want, vm->capacity * 2);
   const size_t rd = vm->rec_doubles;
-  const bool counted = vm->d_counts != nullptr;
   cudaStream_t st = vm->ctx->stream;
-  double* rec = nullptr;
-  int32_t* coords = nullptr;
-  uint32_t* lru = nullptr;
-  uint32_t* counts = nullptr;
-  cudaError_t e;
-  if ((e = cudaMalloc(reinterpret_cast<void**>(&rec), cap * rd * sizeof(double))) != cudaSuccess ||
-      (e = cudaMalloc(reinterpret_cast<void**>(&coords), cap * 3 * sizeof(int32_t))) != cudaSuccess ||
-      (e = cudaMalloc(reinterpret_cast<void**>(&lru), cap * sizeof(uint32_t))) != cudaSuccess ||
-      (counted && (e = cudaMalloc(reinterpret_cast<void**>(&counts), cap * sizeof(uint32_t))) != cudaSuccess)) {
-    if (rec) cudaFree(rec);
-    if (coords) cudaFree(coords);
-    if (lru) cudaFree(lru);
-    return fail(B2_ERR_OUT_OF_MEMORY, "voxelmap growth: %s", cudaGetErrorString(e));
-  }
+  DeviceBuffer rec, coords, lru, counts;
+  B2_TRY(rec.alloc(cap * rd * sizeof(double)));
+  B2_TRY(coords.alloc(cap * 3 * sizeof(int32_t)));
+  B2_TRY(lru.alloc(cap * sizeof(uint32_t)));
+  if (vm->d_counts) B2_TRY(counts.alloc(cap * sizeof(uint32_t)));
   const size_t V = vm->num_voxels;
   if (V) {
-    cudaMemcpyAsync(rec, vm->d_records, V * rd * sizeof(double), cudaMemcpyDeviceToDevice, st);
-    cudaMemcpyAsync(coords, vm->d_coords, V * 3 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st);
-    cudaMemcpyAsync(lru, vm->d_lru, V * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st);
-    if (counted) cudaMemcpyAsync(counts, vm->d_counts, V * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st);
+    B2_CUDA(cudaMemcpyAsync(rec.get(), vm->d_records.get(), V * rd * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    B2_CUDA(cudaMemcpyAsync(coords.get(), vm->d_coords.get(), V * 3 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    B2_CUDA(cudaMemcpyAsync(lru.get(), vm->d_lru.get(), V * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
+    if (counts) B2_CUDA(cudaMemcpyAsync(counts.get(), vm->d_counts.get(), V * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
   }
-  if ((e = cudaStreamSynchronize(st)) != cudaSuccess) {
-    cudaFree(rec), cudaFree(coords), cudaFree(lru);
-    if (counts) cudaFree(counts);
-    return fail(B2_ERR_CUDA, "voxelmap growth: %s", cudaGetErrorString(e));
-  }
-  cudaFree(vm->d_records), cudaFree(vm->d_coords), cudaFree(vm->d_lru);
-  vm->d_records = rec, vm->d_coords = coords, vm->d_lru = lru;
-  if (counted) cudaFree(vm->d_counts), vm->d_counts = counts;
-  vm->device_bytes += (cap - vm->capacity) * (rd * sizeof(double) + 3 * sizeof(int32_t) + sizeof(uint32_t) + (counted ? sizeof(uint32_t) : 0));
+  B2_CUDA(cudaStreamSynchronize(st));
+  vm->d_records = std::move(rec), vm->d_coords = std::move(coords), vm->d_lru = std::move(lru);
+  if (counts) vm->d_counts = std::move(counts);
   vm->capacity = cap;
   return B2_OK;
 }
@@ -508,17 +466,16 @@ b2_status rebuild_table(b2_voxelmap* vm) {
   cudaStream_t st = vm->ctx->stream;
   const size_t nb = bucket_count_for(vm->num_voxels);
   if (nb != vm->num_buckets) {
-    VoxelBucket* fresh = nullptr;
-    B2_CUDA(cudaMalloc(reinterpret_cast<void**>(&fresh), nb * sizeof(VoxelBucket)));
+    DeviceBuffer fresh;
+    B2_TRY(fresh.alloc(nb * sizeof(VoxelBucket)));
     cudaStreamSynchronize(st);
-    cudaFree(vm->d_buckets);
-    vm->device_bytes += (nb - vm->num_buckets) * sizeof(VoxelBucket);
-    vm->d_buckets = fresh;
+    vm->d_buckets = std::move(fresh);
     vm->num_buckets = nb;
   }
-  B2_CUDA(cudaMemsetAsync(vm->d_buckets, 0xFF, vm->num_buckets * sizeof(VoxelBucket), st));
+  B2_CUDA(cudaMemsetAsync(vm->d_buckets.get(), 0xFF, vm->num_buckets * sizeof(VoxelBucket), st));
   if (vm->num_voxels) {
-    insert_buckets_kernel<<<static_cast<unsigned>((vm->num_voxels + 127) / 128), 128, 0, st>>>(vm->d_coords, vm->num_voxels, vm->d_buckets, static_cast<uint32_t>(vm->num_buckets / kGroup - 1));
+    insert_buckets_kernel<<<static_cast<unsigned>((vm->num_voxels + 127) / 128), 128, 0, st>>>(vm->d_coords.as<int32_t>(), vm->num_voxels, vm->d_buckets.as<VoxelBucket>(),
+                                                                                               static_cast<uint32_t>(vm->num_buckets / kGroup - 1));
     B2_CUDA(cudaGetLastError());
   }
   vm->generation++;
@@ -532,8 +489,8 @@ b2_status rebuild_table(b2_voxelmap* vm) {
 // voxel r of the batch (first-touch order) is segment seg_of_rank[r] starting at seg_start[.], with integer coordinate
 // batch_coords[r], id existing_id[r] in the map (-1: new) and, if new, rank new_rank[r] among the new voxels.
 struct BatchSegments {
-  DevBuf raw_p, raw_c, key_z, key_z2, idx_a, idx_b, key_xy, key_xy2, flags, seg_incl, tmp;
-  DevBuf seg_start, seg_first, seg_first2, seg_iota, seg_of_rank, tmp2, batch_coords, existing_id, is_new, new_rank;
+  DeviceBuffer raw_p, raw_c, key_z, key_z2, idx_a, idx_b, key_xy, key_xy2, flags, seg_incl, tmp;
+  DeviceBuffer seg_start, seg_first, seg_first2, seg_iota, seg_of_rank, tmp2, batch_coords, existing_id, is_new, new_rank;
   size_t B = 0, num_new = 0;  // voxels touched by the batch / of them new
   const uint32_t* idx() { return idx_a.as<uint32_t>(); }
 };
@@ -544,74 +501,71 @@ b2_status segment_batch(b2_voxelmap* vm, const double* points, int point_stride,
   cudaStream_t st = vm->ctx->stream;
   const double inv_leaf = vm->inv_resolution;
   const size_t V_old = vm->num_voxels;
-  DevBuf &raw_p = s.raw_p, &raw_c = s.raw_c, &key_z = s.key_z, &key_z2 = s.key_z2, &idx_a = s.idx_a, &idx_b = s.idx_b, &key_xy = s.key_xy, &key_xy2 = s.key_xy2,
-         &flags = s.flags, &seg_incl = s.seg_incl, &tmp = s.tmp;
-  DevBuf &seg_start = s.seg_start, &seg_first = s.seg_first, &seg_first2 = s.seg_first2, &seg_iota = s.seg_iota, &seg_of_rank = s.seg_of_rank, &tmp2 = s.tmp2,
-         &batch_coords = s.batch_coords, &existing_id = s.existing_id, &is_new = s.is_new, &new_rank = s.new_rank;
-  B2_CUDA(cudaMalloc(&raw_p.p, n * point_stride * sizeof(double)));
-  if (covs) B2_CUDA(cudaMalloc(&raw_c.p, n * cov_stride * sizeof(double)));
-  B2_CUDA(cudaMemcpyAsync(raw_p.p, points, n * point_stride * sizeof(double), cudaMemcpyHostToDevice, st));
-  if (covs) B2_CUDA(cudaMemcpyAsync(raw_c.p, covs, n * cov_stride * sizeof(double), cudaMemcpyHostToDevice, st));
-  B2_CUDA(cudaMalloc(&key_z.p, n * 4));
-  B2_CUDA(cudaMalloc(&key_z2.p, n * 4));
-  B2_CUDA(cudaMalloc(&idx_a.p, n * 4));
-  B2_CUDA(cudaMalloc(&idx_b.p, n * 4));
-  B2_CUDA(cudaMalloc(&key_xy.p, n * 8));
-  B2_CUDA(cudaMalloc(&key_xy2.p, n * 8));
-  B2_CUDA(cudaMalloc(&flags.p, n * 4));
-  B2_CUDA(cudaMalloc(&seg_incl.p, n * 4));
+  DeviceBuffer &raw_p = s.raw_p, &raw_c = s.raw_c, &key_z = s.key_z, &key_z2 = s.key_z2, &idx_a = s.idx_a, &idx_b = s.idx_b, &key_xy = s.key_xy, &key_xy2 = s.key_xy2,
+               &flags = s.flags, &seg_incl = s.seg_incl, &tmp = s.tmp;
+  DeviceBuffer &seg_start = s.seg_start, &seg_first = s.seg_first, &seg_first2 = s.seg_first2, &seg_iota = s.seg_iota, &seg_of_rank = s.seg_of_rank, &tmp2 = s.tmp2,
+               &batch_coords = s.batch_coords, &existing_id = s.existing_id, &is_new = s.is_new, &new_rank = s.new_rank;
+  B2_TRY(raw_p.alloc(n * point_stride * sizeof(double)));
+  if (covs) B2_TRY(raw_c.alloc(n * cov_stride * sizeof(double)));
+  B2_CUDA(cudaMemcpyAsync(raw_p.get(), points, n * point_stride * sizeof(double), cudaMemcpyHostToDevice, st));
+  if (covs) B2_CUDA(cudaMemcpyAsync(raw_c.get(), covs, n * cov_stride * sizeof(double), cudaMemcpyHostToDevice, st));
+  B2_TRY(key_z.alloc(n * 4));
+  B2_TRY(key_z2.alloc(n * 4));
+  B2_TRY(idx_a.alloc(n * 4));
+  B2_TRY(idx_b.alloc(n * 4));
+  B2_TRY(key_xy.alloc(n * 8));
+  B2_TRY(key_xy2.alloc(n * 8));
+  B2_TRY(flags.alloc(n * 4));
+  B2_TRY(seg_incl.alloc(n * 4));
 
   const unsigned grid = static_cast<unsigned>((n + 255) / 256);
   const double* rp = raw_p.as<double>();
   const int ni = static_cast<int>(n);
 
-  size_t t1 = 0, t2 = 0, t3 = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, t1, key_z.as<uint32_t>(), key_z2.as<uint32_t>(), idx_a.as<uint32_t>(), idx_b.as<uint32_t>(), ni, 0, 32, st);
-  cub::DeviceRadixSort::SortPairs(nullptr, t2, key_xy.as<unsigned long long>(), key_xy2.as<unsigned long long>(), idx_b.as<uint32_t>(), idx_a.as<uint32_t>(), ni, 0, 64, st);
-  cub::DeviceScan::InclusiveSum(nullptr, t3, flags.as<uint32_t>(), seg_incl.as<uint32_t>(), ni, st);
-  const size_t tmp_bytes = std::max(std::max(t1, t2), std::max(t3, static_cast<size_t>(16)));
-  B2_CUDA(cudaMalloc(&tmp.p, tmp_bytes));
-
   // pass 1: stable sort by z; pass 2: stable sort by (x, y)  => lexicographic (x, y, z), insertion order inside a voxel
+  auto sort_z = [&](void* t, size_t& b) {
+    return cub::DeviceRadixSort::SortPairs(t, b, key_z.as<uint32_t>(), key_z2.as<uint32_t>(), idx_a.as<uint32_t>(), idx_b.as<uint32_t>(), ni, 0, 32, st);
+  };
+  auto sort_xy = [&](void* t, size_t& b) {
+    return cub::DeviceRadixSort::SortPairs(t, b, key_xy.as<unsigned long long>(), key_xy2.as<unsigned long long>(), idx_b.as<uint32_t>(), idx_a.as<uint32_t>(), ni, 0, 64, st);
+  };
+  auto scan_heads = [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, flags.as<uint32_t>(), seg_incl.as<uint32_t>(), ni, st); };
+  B2_TRY(cub_reserve(tmp, st, sort_z, sort_xy, scan_heads));
+
   point_coord_keys_kernel<<<grid, 256, 0, st>>>(rp, point_stride, n, inv_leaf, key_z.as<uint32_t>(), idx_a.as<uint32_t>());
-  size_t tb = tmp_bytes;
-  B2_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, key_z.as<uint32_t>(), key_z2.as<uint32_t>(), idx_a.as<uint32_t>(), idx_b.as<uint32_t>(), ni, 0, 32, st));
+  B2_TRY(cub_launch(tmp, sort_z));
   gather_xy_keys_kernel<<<grid, 256, 0, st>>>(rp, point_stride, n, inv_leaf, idx_b.as<uint32_t>(), key_xy.as<unsigned long long>());
-  tb = tmp_bytes;
-  B2_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, key_xy.as<unsigned long long>(), key_xy2.as<unsigned long long>(), idx_b.as<uint32_t>(), idx_a.as<uint32_t>(), ni, 0, 64, st));
+  B2_TRY(cub_launch(tmp, sort_xy));
   const uint32_t* idx = idx_a.as<uint32_t>();
 
   head_flags_kernel<<<grid, 256, 0, st>>>(rp, point_stride, n, inv_leaf, idx, flags.as<uint32_t>());
-  tb = tmp_bytes;
-  B2_CUDA(cub::DeviceScan::InclusiveSum(tmp.p, tb, flags.as<uint32_t>(), seg_incl.as<uint32_t>(), ni, st));
+  B2_TRY(cub_launch(tmp, scan_heads));
   uint32_t B32 = 0;
   B2_CUDA(cudaMemcpyAsync(&B32, seg_incl.as<uint32_t>() + (n - 1), 4, cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
   const size_t B = B32;  // voxels touched by this batch
 
-  B2_CUDA(cudaMalloc(&seg_start.p, B * 4));
-  B2_CUDA(cudaMalloc(&seg_first.p, B * 4));
-  B2_CUDA(cudaMalloc(&seg_first2.p, B * 4));
-  B2_CUDA(cudaMalloc(&seg_iota.p, B * 4));
-  B2_CUDA(cudaMalloc(&seg_of_rank.p, B * 4));
-  B2_CUDA(cudaMalloc(&batch_coords.p, B * 12));
-  B2_CUDA(cudaMalloc(&existing_id.p, B * 4));
-  B2_CUDA(cudaMalloc(&is_new.p, B * 4));
-  B2_CUDA(cudaMalloc(&new_rank.p, B * 4));
+  B2_TRY(seg_start.alloc(B * 4));
+  B2_TRY(seg_first.alloc(B * 4));
+  B2_TRY(seg_first2.alloc(B * 4));
+  B2_TRY(seg_iota.alloc(B * 4));
+  B2_TRY(seg_of_rank.alloc(B * 4));
+  B2_TRY(batch_coords.alloc(B * 12));
+  B2_TRY(existing_id.alloc(B * 4));
+  B2_TRY(is_new.alloc(B * 4));
+  B2_TRY(new_rank.alloc(B * 4));
   segment_heads_kernel<<<grid, 256, 0, st>>>(n, flags.as<uint32_t>(), seg_incl.as<uint32_t>(), idx, seg_start.as<uint32_t>(), seg_first.as<uint32_t>(), seg_iota.as<uint32_t>());
-  size_t t4 = 0, t5 = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, t4, seg_first.as<uint32_t>(), seg_first2.as<uint32_t>(), seg_iota.as<uint32_t>(), seg_of_rank.as<uint32_t>(), static_cast<int>(B), 0, 32, st);
-  cub::DeviceScan::ExclusiveSum(nullptr, t5, is_new.as<uint32_t>(), new_rank.as<uint32_t>(), static_cast<int>(B), st);
-  size_t tb2 = std::max<size_t>(std::max(t4, t5), 16);
-  B2_CUDA(cudaMalloc(&tmp2.p, tb2));
-  size_t tbb = tb2;
-  B2_CUDA(cub::DeviceRadixSort::SortPairs(tmp2.p, tbb, seg_first.as<uint32_t>(), seg_first2.as<uint32_t>(), seg_iota.as<uint32_t>(), seg_of_rank.as<uint32_t>(), static_cast<int>(B), 0, 32, st));
+  auto sort_first_touch = [&](void* t, size_t& b) {
+    return cub::DeviceRadixSort::SortPairs(t, b, seg_first.as<uint32_t>(), seg_first2.as<uint32_t>(), seg_iota.as<uint32_t>(), seg_of_rank.as<uint32_t>(), static_cast<int>(B), 0, 32, st);
+  };
+  auto rank_new = [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, is_new.as<uint32_t>(), new_rank.as<uint32_t>(), static_cast<int>(B), st); };
+  B2_TRY(cub_reserve(tmp2, st, sort_first_touch, rank_new));
+  B2_TRY(cub_launch(tmp2, sort_first_touch));
 
   const unsigned vgrid = static_cast<unsigned>((B + 127) / 128);
-  batch_voxels_kernel<<<vgrid, 128, 0, st>>>(rp, point_stride, B, inv_leaf, idx, seg_start.as<uint32_t>(), seg_of_rank.as<uint32_t>(), vm->d_buckets,
+  batch_voxels_kernel<<<vgrid, 128, 0, st>>>(rp, point_stride, B, inv_leaf, idx, seg_start.as<uint32_t>(), seg_of_rank.as<uint32_t>(), vm->d_buckets.as<VoxelBucket>(),
                                              static_cast<uint32_t>(vm->num_buckets / kGroup - 1), V_old, batch_coords.as<int32_t>(), existing_id.as<int32_t>(), is_new.as<uint32_t>());
-  tbb = tb2;
-  B2_CUDA(cub::DeviceScan::ExclusiveSum(tmp2.p, tbb, is_new.as<uint32_t>(), new_rank.as<uint32_t>(), static_cast<int>(B), st));
+  B2_TRY(cub_launch(tmp2, rank_new));
   uint32_t last_rank = 0, last_new = 0;
   B2_CUDA(cudaMemcpyAsync(&last_rank, new_rank.as<uint32_t>() + (B - 1), 4, cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaMemcpyAsync(&last_new, is_new.as<uint32_t>() + (B - 1), 4, cudaMemcpyDeviceToHost, st));
@@ -628,15 +582,12 @@ b2_status lru_sweep_and_rebuild(b2_voxelmap* vm) {
   vm->lru_counter++;
   if (vm->lru_counter % vm->lru_clear_cycle == 0 && vm->num_voxels > 0) {
     const size_t V = vm->num_voxels;
-    DevBuf keep, pos, tmp3, rec2, coords2, lru2, counts2;
-    B2_CUDA(cudaMalloc(&keep.p, V * 4));
-    B2_CUDA(cudaMalloc(&pos.p, V * 4));
+    DeviceBuffer keep, pos, tmp3, rec2, coords2, lru2, counts2;
+    B2_TRY(keep.alloc(V * 4));
+    B2_TRY(pos.alloc(V * 4));
     const unsigned g = static_cast<unsigned>((V + 255) / 256);
-    lru_keep_flags_kernel<<<g, 256, 0, st>>>(vm->d_lru, V, static_cast<uint32_t>(vm->lru_horizon), static_cast<uint32_t>(vm->lru_counter), keep.as<uint32_t>());
-    size_t t6 = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, t6, keep.as<uint32_t>(), pos.as<uint32_t>(), static_cast<int>(V), st);
-    B2_CUDA(cudaMalloc(&tmp3.p, std::max<size_t>(t6, 16)));
-    B2_CUDA(cub::DeviceScan::ExclusiveSum(tmp3.p, t6, keep.as<uint32_t>(), pos.as<uint32_t>(), static_cast<int>(V), st));
+    lru_keep_flags_kernel<<<g, 256, 0, st>>>(vm->d_lru.as<uint32_t>(), V, static_cast<uint32_t>(vm->lru_horizon), static_cast<uint32_t>(vm->lru_counter), keep.as<uint32_t>());
+    B2_TRY(cub_run(tmp3, st, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, keep.as<uint32_t>(), pos.as<uint32_t>(), static_cast<int>(V), st); }));
     uint32_t last_pos = 0, last_keep = 0;
     B2_CUDA(cudaMemcpyAsync(&last_pos, pos.as<uint32_t>() + (V - 1), 4, cudaMemcpyDeviceToHost, st));
     B2_CUDA(cudaMemcpyAsync(&last_keep, keep.as<uint32_t>() + (V - 1), 4, cudaMemcpyDeviceToHost, st));
@@ -644,18 +595,16 @@ b2_status lru_sweep_and_rebuild(b2_voxelmap* vm) {
     const size_t kept = static_cast<size_t>(last_pos) + last_keep;
     if (kept != V) {
       const size_t cap = vm->capacity;
-      B2_CUDA(cudaMalloc(&rec2.p, cap * vm->rec_doubles * sizeof(double)));
-      B2_CUDA(cudaMalloc(&coords2.p, cap * 3 * sizeof(int32_t)));
-      B2_CUDA(cudaMalloc(&lru2.p, cap * sizeof(uint32_t)));
-      if (vm->d_counts) B2_CUDA(cudaMalloc(&counts2.p, cap * sizeof(uint32_t)));
-      lru_compact_kernel<<<g, 256, 0, st>>>(keep.as<uint32_t>(), pos.as<uint32_t>(), V, vm->rec_doubles, vm->d_records, vm->d_coords, vm->d_lru, vm->d_counts, rec2.as<double>(),
-                                            coords2.as<int32_t>(), lru2.as<uint32_t>(), counts2.as<uint32_t>());
+      B2_TRY(rec2.alloc(cap * vm->rec_doubles * sizeof(double)));
+      B2_TRY(coords2.alloc(cap * 3 * sizeof(int32_t)));
+      B2_TRY(lru2.alloc(cap * sizeof(uint32_t)));
+      if (vm->d_counts) B2_TRY(counts2.alloc(cap * sizeof(uint32_t)));
+      lru_compact_kernel<<<g, 256, 0, st>>>(keep.as<uint32_t>(), pos.as<uint32_t>(), V, vm->rec_doubles, vm->d_records.as<double>(), vm->d_coords.as<int32_t>(), vm->d_lru.as<uint32_t>(),
+                                            vm->d_counts.as<uint32_t>(), rec2.as<double>(), coords2.as<int32_t>(), lru2.as<uint32_t>(), counts2.as<uint32_t>());
       B2_CUDA(cudaGetLastError());
       B2_CUDA(cudaStreamSynchronize(st));
-      std::swap(vm->d_records, *reinterpret_cast<double**>(&rec2.p));
-      std::swap(vm->d_coords, *reinterpret_cast<int32_t**>(&coords2.p));
-      std::swap(vm->d_lru, *reinterpret_cast<uint32_t**>(&lru2.p));
-      if (vm->d_counts) std::swap(vm->d_counts, *reinterpret_cast<uint32_t**>(&counts2.p));
+      vm->d_records = std::move(rec2), vm->d_coords = std::move(coords2), vm->d_lru = std::move(lru2);
+      if (counts2) vm->d_counts = std::move(counts2);
       vm->num_voxels = kept;
     }
   }
@@ -714,18 +663,14 @@ b2_status b2_voxelmap_create_from_voxels(b2_ctx* ctx, double resolution, const i
     rec[9] = num_points ? static_cast<double>(num_points[r]) : 1.0;
   }
 
-  b2_voxelmap* vm = nullptr;
-  B2_TRY(alloc_map(ctx, resolution, V, &vm));
+  auto vm = std::make_unique<b2_voxelmap>();
+  B2_TRY(init_map(*vm, ctx, resolution, V));
   cudaStream_t st = ctx->stream;
-  cudaError_t e;
-  if ((e = cudaMemcpyAsync(vm->d_buckets, buckets.data(), nb * sizeof(VoxelBucket), cudaMemcpyHostToDevice, st)) != cudaSuccess ||
-      (e = cudaMemcpyAsync(vm->d_records, records.data(), records.size() * sizeof(double), cudaMemcpyHostToDevice, st)) != cudaSuccess ||
-      (V > 0 && (e = cudaMemcpyAsync(vm->d_coords, coords, V * 3 * sizeof(int32_t), cudaMemcpyHostToDevice, st)) != cudaSuccess) ||
-      (e = cudaStreamSynchronize(st)) != cudaSuccess) {
-    b2_voxelmap_destroy(vm);
-    return fail(B2_ERR_CUDA, "b2_voxelmap_create_from_voxels: %s", cudaGetErrorString(e));
-  }
-  *out = vm;
+  B2_CUDA(cudaMemcpyAsync(vm->d_buckets.get(), buckets.data(), nb * sizeof(VoxelBucket), cudaMemcpyHostToDevice, st));
+  B2_CUDA(cudaMemcpyAsync(vm->d_records.get(), records.data(), records.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+  if (V > 0) B2_CUDA(cudaMemcpyAsync(vm->d_coords.get(), coords, V * 3 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  *out = vm.release();
   return B2_OK;
 }
 
@@ -769,7 +714,7 @@ b2_status b2_voxelmap_insert(b2_voxelmap* vm, const double* points, int point_st
     const unsigned vgrid = static_cast<unsigned>((B + 127) / 128);
     accumulate_voxels_kernel<<<vgrid, 128, 0, st>>>(sg.raw_p.as<double>(), point_stride, sg.raw_c.as<double>(), cov_stride, n, B, sg.idx(), sg.seg_start.as<uint32_t>(), sg.seg_of_rank.as<uint32_t>(),
                                                     sg.batch_coords.as<int32_t>(), sg.existing_id.as<int32_t>(), sg.new_rank.as<uint32_t>(), V_old, static_cast<uint32_t>(vm->lru_counter),
-                                                    vm->d_records, vm->d_coords, vm->d_lru);
+                                                    vm->d_records.as<double>(), vm->d_coords.as<int32_t>(), vm->d_lru.as<uint32_t>());
     B2_CUDA(cudaGetLastError());
     vm->num_voxels = V_old + num_new;
     B2_CUDA(cudaStreamSynchronize(st));  // the scratch buffers above are released at scope exit
@@ -787,20 +732,17 @@ b2_status b2_voxelmap_create_from_points(b2_ctx* ctx, double resolution, const d
   B2_REQUIRE(cov_stride == 9 || cov_stride == 16, "b2_voxelmap_create_from_points: cov_stride must be 9 or 16");
   B2_REQUIRE(n == 0 || (points && covs), "b2_voxelmap_create_from_points: points and covs are required");  // reference: GaussianVoxel::add reads covs
   B2_REQUIRE(n < (1ull << 31), "b2_voxelmap_create_from_points: at most 2^31-1 points");
-  b2_voxelmap* vm = nullptr;
-  B2_TRY(b2_voxelmap_create(ctx, resolution, &vm));
-  const b2_status st = b2_voxelmap_insert(vm, points, point_stride, covs, cov_stride, n);  // the one-shot build IS the first insert
-  if (st != B2_OK) {
-    b2_voxelmap_destroy(vm);
-    return st;
-  }
-  *out = vm;
+  b2_voxelmap* created = nullptr;
+  B2_TRY(b2_voxelmap_create(ctx, resolution, &created));
+  std::unique_ptr<b2_voxelmap> vm(created);
+  B2_TRY(b2_voxelmap_insert(vm.get(), points, point_stride, covs, cov_stride, n));  // the one-shot build IS the first insert
+  *out = vm.release();
   return B2_OK;
 }
 
 b2_status b2_voxelmap_destroy(b2_voxelmap* vm) {
   if (!vm) return B2_OK;
-  release_map(vm);
+  cudaSetDevice(vm->ctx->device);
   delete vm;
   return B2_OK;
 }
@@ -810,7 +752,7 @@ b2_status b2_voxelmap_get_info(const b2_voxelmap* vm, b2_voxelmap_info* info) {
   info->num_voxels = vm->num_voxels;
   info->num_buckets = vm->num_buckets;
   info->resolution = vm->resolution;
-  info->device_bytes = vm->device_bytes;
+  info->device_bytes = vm->device_bytes();
   return B2_OK;
 }
 
@@ -821,8 +763,8 @@ b2_status b2_voxelmap_download(const b2_voxelmap* vm, int32_t* coords, double* m
   B2_CUDA(cudaSetDevice(vm->ctx->device));
   cudaStream_t st = vm->ctx->stream;
   std::vector<double> rec(V * kRecordDoubles);
-  B2_CUDA(cudaMemcpyAsync(rec.data(), vm->d_records, rec.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
-  if (coords) B2_CUDA(cudaMemcpyAsync(coords, vm->d_coords, V * 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(rec.data(), vm->d_records.get(), rec.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (coords) B2_CUDA(cudaMemcpyAsync(coords, vm->d_coords.get(), V * 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
   for (size_t r = 0; r < V; r++) {
     const double* q = &rec[r * kRecordDoubles];
@@ -919,7 +861,7 @@ b2_status b2_voxelmap_load(b2_ctx* ctx, const char* path, b2_voxelmap** out) {
 
 b2_status b2_overlap(const b2_voxelmap* const* targets, size_t num_targets, const b2_cloud* source, const double* Ts_target_source, double* out_overlap) {
   B2_REQUIRE(targets && source && Ts_target_source && out_overlap && num_targets > 0, "b2_overlap: NULL / empty argument");
-  B2_REQUIRE(source->d_points != nullptr, "error: source points have not been allocated!!");
+  B2_REQUIRE(source->d_points, "error: source points have not been allocated!!");
   b2_ctx* ctx = source->ctx;
   B2_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
@@ -927,7 +869,7 @@ b2_status b2_overlap(const b2_voxelmap* const* targets, size_t num_targets, cons
   for (size_t j = 0; j < num_targets; j++) {
     B2_REQUIRE(targets[j] != nullptr, "error: Failed to cast target voxelmap to GaussianVoxelMapGPU!!");  // gaussian_voxelmap_gpu_funcs.cu:70-75
     B2_REQUIRE(targets[j]->ctx->device == ctx->device, "b2_overlap: map %zu lives on another device", j);
-    maps[j].buckets = targets[j]->d_buckets;
+    maps[j].buckets = targets[j]->d_buckets.as<const VoxelBucket>();
     maps[j].mask = static_cast<uint32_t>(targets[j]->num_buckets / kGroup - 1);
     maps[j].pad = 0;
     maps[j].inv_leaf = targets[j]->inv_resolution;
@@ -937,19 +879,19 @@ b2_status b2_overlap(const b2_voxelmap* const* targets, size_t num_targets, cons
     *out_overlap = 0.0;
     return B2_OK;
   }
-  DevBuf d_maps, d_count;
-  B2_CUDA(cudaMalloc(&d_maps.p, maps.size() * sizeof(OverlapMap)));
-  B2_CUDA(cudaMalloc(&d_count.p, sizeof(unsigned long long)));
-  B2_CUDA(cudaMemcpyAsync(d_maps.p, maps.data(), maps.size() * sizeof(OverlapMap), cudaMemcpyHostToDevice, st));
-  B2_CUDA(cudaMemsetAsync(d_count.p, 0, sizeof(unsigned long long), st));
+  DeviceBuffer d_maps, d_count;
+  B2_TRY(d_maps.alloc(maps.size() * sizeof(OverlapMap)));
+  B2_TRY(d_count.alloc(sizeof(unsigned long long)));
+  B2_CUDA(cudaMemcpyAsync(d_maps.get(), maps.data(), maps.size() * sizeof(OverlapMap), cudaMemcpyHostToDevice, st));
+  B2_CUDA(cudaMemsetAsync(d_count.get(), 0, sizeof(unsigned long long), st));
   const unsigned grid = static_cast<unsigned>((source->n + 255) / 256);
   if (source->point_bytes == 4)
-    overlap_kernel<float><<<grid, 256, 0, st>>>(static_cast<const float*>(source->d_points), source->n, source->n_pad, d_maps.as<OverlapMap>(), static_cast<int>(num_targets), d_count.as<unsigned long long>());
+    overlap_kernel<float><<<grid, 256, 0, st>>>(source->d_points.as<const float>(), source->n, source->n_pad, d_maps.as<OverlapMap>(), static_cast<int>(num_targets), d_count.as<unsigned long long>());
   else
-    overlap_kernel<double><<<grid, 256, 0, st>>>(static_cast<const double*>(source->d_points), source->n, source->n_pad, d_maps.as<OverlapMap>(), static_cast<int>(num_targets), d_count.as<unsigned long long>());
+    overlap_kernel<double><<<grid, 256, 0, st>>>(source->d_points.as<const double>(), source->n, source->n_pad, d_maps.as<OverlapMap>(), static_cast<int>(num_targets), d_count.as<unsigned long long>());
   B2_CUDA(cudaGetLastError());
   unsigned long long cnt = 0;
-  B2_CUDA(cudaMemcpyAsync(&cnt, d_count.p, sizeof(cnt), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(&cnt, d_count.get(), sizeof(cnt), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
   *out_overlap = static_cast<double>(cnt) / static_cast<double>(source->n);  // gaussian_voxelmap_cpu_funcs.cpp:142
   return B2_OK;
@@ -962,10 +904,10 @@ b2_status b2_merge_frames(b2_ctx* ctx, const double* poses, const b2_cloud* cons
   size_t total = 0;
   bool have_covs = true;
   for (size_t f = 0; f < num_frames; f++) {
-    B2_REQUIRE(frames[f] != nullptr && (frames[f]->n == 0 || frames[f]->d_points != nullptr), "error: frame %zu has no points", f);
+    B2_REQUIRE(frames[f] != nullptr && (frames[f]->n == 0 || frames[f]->d_points), "error: frame %zu has no points", f);
     B2_REQUIRE(frames[f]->ctx->device == ctx->device, "b2_merge_frames: frame %zu lives on another device", f);
     total += frames[f]->n;
-    have_covs = have_covs && (frames[f]->n == 0 || frames[f]->d_covs != nullptr);
+    have_covs = have_covs && (frames[f]->n == 0 || frames[f]->d_covs);
   }
   B2_REQUIRE(total < (1ull << 31), "b2_merge_frames: too many points");
   *out_n = 0;
@@ -982,12 +924,12 @@ b2_status b2_merge_frames(b2_ctx* ctx, const double* poses, const b2_cloud* cons
   for (int r = 0; r < 3; r++) inv0[r * 4 + 3] = -(inv0[r * 4 + 0] * at(poses, 0, 3) + inv0[r * 4 + 1] * at(poses, 1, 3) + inv0[r * 4 + 2] * at(poses, 2, 3));
   inv0[15] = 1.0;
   std::vector<MergeFrame> h(num_frames);
-  std::vector<DevBuf> inv_perms(num_frames);
+  std::vector<DeviceBuffer> inv_perms(num_frames);
   uint32_t offset = 0;
   for (size_t f = 0; f < num_frames; f++) {
     const b2_cloud* c = frames[f];
     MergeFrame& m = h[f];
-    m.pts = c->d_points, m.covs = have_covs ? c->d_covs : nullptr, m.perm = c->d_perm, m.inv_perm = nullptr;
+    m.pts = c->d_points.get(), m.covs = have_covs ? c->d_covs.get() : nullptr, m.perm = c->d_perm.as<const uint32_t>(), m.inv_perm = nullptr;
     m.n = static_cast<uint32_t>(c->n), m.n_pad = static_cast<uint32_t>(c->n_pad), m.offset = offset;
     m.point_bytes = c->point_bytes, m.cov_bytes = c->cov_bytes;
     const double* P = poses + 16 * f;
@@ -999,49 +941,51 @@ b2_status b2_merge_frames(b2_ctx* ctx, const double* poses, const b2_cloud* cons
         m.pose[r * 4 + cc] = at(P, r, cc);
       }
     if (c->d_perm && c->n > 0) {
-      B2_CUDA(cudaMalloc(&inv_perms[f].p, c->n * sizeof(uint32_t)));
-      merge_invert_perm_kernel<<<static_cast<unsigned>((c->n + 255) / 256), 256, 0, st>>>(c->d_perm, m.n, inv_perms[f].as<uint32_t>());
+      B2_TRY(inv_perms[f].alloc(c->n * sizeof(uint32_t)));
+      merge_invert_perm_kernel<<<static_cast<unsigned>((c->n + 255) / 256), 256, 0, st>>>(c->d_perm.as<const uint32_t>(), m.n, inv_perms[f].as<uint32_t>());
       m.inv_perm = inv_perms[f].as<uint32_t>();
     }
     offset += m.n;
   }
-  DevBuf d_frames, keys, keys2, vals, vals2, flags, incl, starts, d_min, tmp, d_xyz, d_cov;
+  DeviceBuffer d_frames, keys, keys2, vals, vals2, flags, incl, starts, d_min, tmp, d_xyz, d_cov;
   const int ni = static_cast<int>(total);
-  B2_CUDA(cudaMalloc(&d_frames.p, num_frames * sizeof(MergeFrame)));
-  B2_CUDA(cudaMalloc(&keys.p, total * 8));
-  B2_CUDA(cudaMalloc(&keys2.p, total * 8));
-  B2_CUDA(cudaMalloc(&vals.p, total * 4));
-  B2_CUDA(cudaMalloc(&vals2.p, total * 4));
-  B2_CUDA(cudaMalloc(&flags.p, total * 4));
-  B2_CUDA(cudaMalloc(&incl.p, total * 4));
-  B2_CUDA(cudaMalloc(&starts.p, (total + 1) * 4));
-  B2_CUDA(cudaMalloc(&d_min.p, 8));
-  B2_CUDA(cudaMemcpyAsync(d_frames.p, h.data(), num_frames * sizeof(MergeFrame), cudaMemcpyHostToDevice, st));
+  B2_TRY(d_frames.alloc(num_frames * sizeof(MergeFrame)));
+  B2_TRY(keys.alloc(total * 8));
+  B2_TRY(keys2.alloc(total * 8));
+  B2_TRY(vals.alloc(total * 4));
+  B2_TRY(vals2.alloc(total * 4));
+  B2_TRY(flags.alloc(total * 4));
+  B2_TRY(incl.alloc(total * 4));
+  B2_TRY(starts.alloc((total + 1) * 4));
+  B2_TRY(d_min.alloc(8));
+  B2_CUDA(cudaMemcpyAsync(d_frames.get(), h.data(), num_frames * sizeof(MergeFrame), cudaMemcpyHostToDevice, st));
   for (size_t f = 0; f < num_frames; f++)
     if (h[f].n) merge_keys_kernel<<<(h[f].n + 255) / 256, 256, 0, st>>>(d_frames.as<MergeFrame>(), static_cast<int>(f), 1.0 / downsample_resolution, keys.as<unsigned long long>(), vals.as<uint32_t>());
-  size_t t1 = 0, t2 = 0, t3 = 0;
-  cub::DeviceReduce::Reduce(nullptr, t1, keys.as<unsigned long long>(), d_min.as<unsigned long long>(), ni, MinU64(), kMergeNoKey, st);
-  cub::DeviceRadixSort::SortPairs(nullptr, t2, keys.as<unsigned long long>(), keys2.as<unsigned long long>(), vals.as<uint32_t>(), vals2.as<uint32_t>(), ni, 0, 63, st);
-  cub::DeviceScan::InclusiveSum(nullptr, t3, flags.as<uint32_t>(), incl.as<uint32_t>(), ni, st);
-  size_t tb = std::max(t1, std::max(t2, t3));
-  B2_CUDA(cudaMalloc(&tmp.p, std::max<size_t>(tb, 16)));
+  auto min_key = [&](void* t, size_t& b) {
+    return cub::DeviceReduce::Reduce(t, b, keys.as<unsigned long long>(), d_min.as<unsigned long long>(), ni, MinU64(), kMergeNoKey, st);
+  };
+  auto sort_keys = [&](void* t, size_t& b) {
+    return cub::DeviceRadixSort::SortPairs(t, b, keys.as<unsigned long long>(), keys2.as<unsigned long long>(), vals.as<uint32_t>(), vals2.as<uint32_t>(), ni, 0, 63, st);
+  };
+  auto scan_heads = [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, flags.as<uint32_t>(), incl.as<uint32_t>(), ni, st); };
+  B2_TRY(cub_reserve(tmp, st, min_key, sort_keys, scan_heads));
   const unsigned grid = static_cast<unsigned>((total + 255) / 256);
-  B2_CUDA(cub::DeviceReduce::Reduce(tmp.p, tb, keys.as<unsigned long long>(), d_min.as<unsigned long long>(), ni, MinU64(), kMergeNoKey, st));
+  B2_TRY(cub_launch(tmp, min_key));
   merge_fix_keys_kernel<<<grid, 256, 0, st>>>(keys.as<unsigned long long>(), total, d_min.as<unsigned long long>());
-  B2_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, keys.as<unsigned long long>(), keys2.as<unsigned long long>(), vals.as<uint32_t>(), vals2.as<uint32_t>(), ni, 0, 63, st));
+  B2_TRY(cub_launch(tmp, sort_keys));
   merge_heads_kernel<<<grid, 256, 0, st>>>(keys2.as<unsigned long long>(), total, flags.as<uint32_t>());
-  B2_CUDA(cub::DeviceScan::InclusiveSum(tmp.p, tb, flags.as<uint32_t>(), incl.as<uint32_t>(), ni, st));
+  B2_TRY(cub_launch(tmp, scan_heads));
   merge_starts_kernel<<<grid, 256, 0, st>>>(flags.as<uint32_t>(), incl.as<uint32_t>(), total, starts.as<uint32_t>());
   uint32_t num_voxels = 0;
   B2_CUDA(cudaMemcpyAsync(&num_voxels, incl.as<uint32_t>() + (total - 1), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
-  B2_CUDA(cudaMalloc(&d_xyz.p, static_cast<size_t>(num_voxels) * 3 * sizeof(double)));
-  B2_CUDA(cudaMalloc(&d_cov.p, static_cast<size_t>(num_voxels) * 9 * sizeof(double)));
+  B2_TRY(d_xyz.alloc(static_cast<size_t>(num_voxels) * 3 * sizeof(double)));
+  B2_TRY(d_cov.alloc(static_cast<size_t>(num_voxels) * 9 * sizeof(double)));
   merge_sum_kernel<<<(num_voxels + 127) / 128, 128, 0, st>>>(d_frames.as<MergeFrame>(), static_cast<int>(num_frames), vals2.as<uint32_t>(), starts.as<uint32_t>(), num_voxels, d_xyz.as<double>(),
                                                              d_cov.as<double>());
   B2_CUDA(cudaGetLastError());
-  B2_CUDA(cudaMemcpyAsync(out_points, d_xyz.p, static_cast<size_t>(num_voxels) * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
-  if (out_covs) B2_CUDA(cudaMemcpyAsync(out_covs, d_cov.p, static_cast<size_t>(num_voxels) * 9 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(out_points, d_xyz.get(), static_cast<size_t>(num_voxels) * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (out_covs) B2_CUDA(cudaMemcpyAsync(out_covs, d_cov.get(), static_cast<size_t>(num_voxels) * 9 * sizeof(double), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
   *out_n = num_voxels;
   return B2_OK;
@@ -1053,14 +997,14 @@ b2_status b2_voxelmap_lookup(const b2_voxelmap* vm, const double* points, int po
   if (n == 0) return B2_OK;
   B2_CUDA(cudaSetDevice(vm->ctx->device));
   cudaStream_t st = vm->ctx->stream;
-  DevBuf dp, di;
-  B2_CUDA(cudaMalloc(&dp.p, n * point_stride * sizeof(double)));
-  B2_CUDA(cudaMalloc(&di.p, n * sizeof(int32_t)));
-  B2_CUDA(cudaMemcpyAsync(dp.p, points, n * point_stride * sizeof(double), cudaMemcpyHostToDevice, st));
-  lookup_points_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(dp.as<double>(), point_stride, n, vm->inv_resolution, vm->d_buckets,
+  DeviceBuffer dp, di;
+  B2_TRY(dp.alloc(n * point_stride * sizeof(double)));
+  B2_TRY(di.alloc(n * sizeof(int32_t)));
+  B2_CUDA(cudaMemcpyAsync(dp.get(), points, n * point_stride * sizeof(double), cudaMemcpyHostToDevice, st));
+  lookup_points_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(dp.as<double>(), point_stride, n, vm->inv_resolution, vm->d_buckets.as<VoxelBucket>(),
                                                                               static_cast<uint32_t>(vm->num_buckets / kGroup - 1), di.as<int32_t>());
   B2_CUDA(cudaGetLastError());
-  B2_CUDA(cudaMemcpyAsync(out_index, di.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(out_index, di.get(), n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
   return B2_OK;
 }
@@ -1074,23 +1018,17 @@ b2_status b2_ivox_create(b2_ctx* ctx, double resolution, b2_ivox** out) {
   B2_REQUIRE(ctx != nullptr, "b2_ivox_create: ctx is NULL");
   B2_REQUIRE(resolution > 0.0, "b2_ivox_create: resolution must be positive");
   B2_CUDA(cudaSetDevice(ctx->device));
-  b2_voxelmap* vm = nullptr;
-  B2_TRY(alloc_map(ctx, resolution, 0, &vm));  // empty table; the per-voxel arrays get their layout at the first insert
-  b2_ivox* iv = new b2_ivox;
-  iv->map = *vm;
-  delete vm;  // (ownership of the device arrays moved into iv->map)
-  const cudaError_t e = cudaMemsetAsync(iv->map.d_buckets, 0xFF, iv->map.num_buckets * sizeof(VoxelBucket), ctx->stream);
-  if (e != cudaSuccess || cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
-    b2_ivox_destroy(iv);
-    return fail(B2_ERR_CUDA, "b2_ivox_create: %s", cudaGetErrorString(e));
-  }
-  *out = iv;
+  auto iv = std::make_unique<b2_ivox>();
+  B2_TRY(init_map(iv->map, ctx, resolution, 0));  // empty table; the per-voxel arrays get their layout at the first insert
+  B2_CUDA(cudaMemsetAsync(iv->map.d_buckets.get(), 0xFF, iv->map.num_buckets * sizeof(VoxelBucket), ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  *out = iv.release();
   return B2_OK;
 }
 
 b2_status b2_ivox_destroy(b2_ivox* iv) {
   if (!iv) return B2_OK;
-  release_map(&iv->map);
+  cudaSetDevice(iv->map.ctx->device);
   delete iv;
   return B2_OK;
 }
@@ -1158,18 +1096,14 @@ b2_status b2_ivox_insert(b2_ivox* iv, const double* points, int point_stride, co
     if (iv->stride == 0) {
       // nothing is stored yet: make the per-voxel arrays in the slot layout, and commit the layout only once they exist
       const size_t cap = std::max<size_t>(V_new, 1), rd = static_cast<size_t>(stride) * kRecordDoubles;
-      DevBuf rec, coords, lru, counts;
-      B2_CUDA(cudaMalloc(&rec.p, cap * rd * sizeof(double)));
-      B2_CUDA(cudaMalloc(&coords.p, cap * 3 * sizeof(int32_t)));
-      B2_CUDA(cudaMalloc(&lru.p, cap * sizeof(uint32_t)));
-      B2_CUDA(cudaMalloc(&counts.p, cap * sizeof(uint32_t)));
-      cudaFree(vm->d_records), cudaFree(vm->d_coords), cudaFree(vm->d_lru);
-      vm->device_bytes -= vm->capacity * (vm->rec_doubles * sizeof(double) + 3 * sizeof(int32_t) + sizeof(uint32_t));
-      vm->d_records = rec.as<double>(), vm->d_coords = coords.as<int32_t>(), vm->d_lru = lru.as<uint32_t>(), vm->d_counts = counts.as<uint32_t>();
-      rec.p = coords.p = lru.p = counts.p = nullptr;  // owned by the map now
+      DeviceBuffer rec, coords, lru, counts;
+      B2_TRY(rec.alloc(cap * rd * sizeof(double)));
+      B2_TRY(coords.alloc(cap * 3 * sizeof(int32_t)));
+      B2_TRY(lru.alloc(cap * sizeof(uint32_t)));
+      B2_TRY(counts.alloc(cap * sizeof(uint32_t)));
+      vm->d_records = std::move(rec), vm->d_coords = std::move(coords), vm->d_lru = std::move(lru), vm->d_counts = std::move(counts);
       vm->capacity = cap;
       vm->rec_doubles = rd;
-      vm->device_bytes += cap * (rd * sizeof(double) + 3 * sizeof(int32_t) + 2 * sizeof(uint32_t));
       iv->stride = stride;
     } else {
       B2_TRY(reserve_voxels(vm, V_new));
@@ -1178,8 +1112,8 @@ b2_status b2_ivox_insert(b2_ivox* iv, const double* points, int point_stride, co
     const unsigned vgrid = static_cast<unsigned>((sg.B + 127) / 128);
     ivox_add_kernel<<<vgrid, 128, 0, st>>>(sg.raw_p.as<double>(), point_stride, sg.raw_c.as<double>(), cov_stride, n, sg.B, sg.idx(), sg.seg_start.as<uint32_t>(),
                                            sg.seg_of_rank.as<uint32_t>(), sg.batch_coords.as<int32_t>(), sg.existing_id.as<int32_t>(), sg.new_rank.as<uint32_t>(), V_old,
-                                           static_cast<uint32_t>(vm->lru_counter), iv->stride, iv->max_num_points_in_cell, iv->min_sq_dist_in_cell, vm->d_records, vm->d_counts,
-                                           vm->d_coords, vm->d_lru);
+                                           static_cast<uint32_t>(vm->lru_counter), iv->stride, iv->max_num_points_in_cell, iv->min_sq_dist_in_cell, vm->d_records.as<double>(),
+                                           vm->d_counts.as<uint32_t>(), vm->d_coords.as<int32_t>(), vm->d_lru.as<uint32_t>());
     B2_CUDA(cudaGetLastError());
     vm->num_voxels = V_new;
     B2_CUDA(cudaStreamSynchronize(st));
@@ -1193,11 +1127,11 @@ b2_status b2_ivox_get_info(const b2_ivox* iv, b2_ivox_info* info) {
   info->num_voxels = vm->num_voxels;
   info->num_points = 0;
   info->resolution = vm->resolution;
-  info->device_bytes = vm->device_bytes;
+  info->device_bytes = vm->device_bytes();
   if (vm->num_voxels > 0) {
     std::vector<uint32_t> cnt(vm->num_voxels);
     B2_CUDA(cudaSetDevice(vm->ctx->device));
-    B2_CUDA(cudaMemcpyAsync(cnt.data(), vm->d_counts, cnt.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, vm->ctx->stream));
+    B2_CUDA(cudaMemcpyAsync(cnt.data(), vm->d_counts.get(), cnt.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, vm->ctx->stream));
     B2_CUDA(cudaStreamSynchronize(vm->ctx->stream));
     for (uint32_t c : cnt) info->num_points += c;
   }
@@ -1213,9 +1147,9 @@ b2_status b2_ivox_download(const b2_ivox* iv, int32_t* coords, int32_t* counts, 
   cudaStream_t st = vm->ctx->stream;
   std::vector<uint32_t> cnt(V);
   std::vector<double> rec(V * vm->rec_doubles);
-  B2_CUDA(cudaMemcpyAsync(cnt.data(), vm->d_counts, V * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-  B2_CUDA(cudaMemcpyAsync(rec.data(), vm->d_records, rec.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
-  if (coords) B2_CUDA(cudaMemcpyAsync(coords, vm->d_coords, V * 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(cnt.data(), vm->d_counts.get(), V * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(rec.data(), vm->d_records.get(), rec.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (coords) B2_CUDA(cudaMemcpyAsync(coords, vm->d_coords.get(), V * 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
   size_t o = 0;
   for (size_t v = 0; v < V; v++) {
@@ -1247,17 +1181,18 @@ b2_status b2_ivox_knn(const b2_ivox* iv, const double* queries, int query_stride
   const b2_voxelmap* vm = &iv->map;
   B2_CUDA(cudaSetDevice(vm->ctx->device));
   cudaStream_t st = vm->ctx->stream;
-  DevBuf dq, di, ds;
-  B2_CUDA(cudaMalloc(&dq.p, nq * query_stride * sizeof(double)));
-  B2_CUDA(cudaMalloc(&di.p, nq * k * sizeof(long long)));
-  B2_CUDA(cudaMalloc(&ds.p, nq * k * sizeof(double)));
-  B2_CUDA(cudaMemcpyAsync(dq.p, queries, nq * query_stride * sizeof(double), cudaMemcpyHostToDevice, st));
-  ivox_knn_kernel<<<static_cast<unsigned>((nq + 127) / 128), 128, 0, st>>>(dq.as<double>(), query_stride, nq, k, max_sq_dist, vm->d_buckets, static_cast<uint32_t>(vm->num_buckets / kGroup - 1),
-                                                                           vm->inv_resolution, vm->d_records, vm->d_counts, iv->stride, iv->neighbor_mode, vm->num_voxels,
+  DeviceBuffer dq, di, ds;
+  B2_TRY(dq.alloc(nq * query_stride * sizeof(double)));
+  B2_TRY(di.alloc(nq * k * sizeof(long long)));
+  B2_TRY(ds.alloc(nq * k * sizeof(double)));
+  B2_CUDA(cudaMemcpyAsync(dq.get(), queries, nq * query_stride * sizeof(double), cudaMemcpyHostToDevice, st));
+  ivox_knn_kernel<<<static_cast<unsigned>((nq + 127) / 128), 128, 0, st>>>(dq.as<double>(), query_stride, nq, k, max_sq_dist, vm->d_buckets.as<VoxelBucket>(),
+                                                                           static_cast<uint32_t>(vm->num_buckets / kGroup - 1), vm->inv_resolution, vm->d_records.as<double>(),
+                                                                           vm->d_counts.as<uint32_t>(), iv->stride, iv->neighbor_mode, vm->num_voxels,
                                                                            di.as<long long>(), ds.as<double>());
   B2_CUDA(cudaGetLastError());
-  B2_CUDA(cudaMemcpyAsync(out_index, di.p, nq * k * sizeof(long long), cudaMemcpyDeviceToHost, st));
-  B2_CUDA(cudaMemcpyAsync(out_sq_dist, ds.p, nq * k * sizeof(double), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(out_index, di.get(), nq * k * sizeof(long long), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(out_sq_dist, ds.get(), nq * k * sizeof(double), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
   return B2_OK;
 }

@@ -34,12 +34,12 @@ def _mtime(p):
     return os.path.getmtime(p) if os.path.exists(p) else 0.0
 
 
-def _compile(src, verbose, defines=(), tag=""):
-    obj = os.path.join(OBJDIR, src.replace(".cu", tag + ".o"))
+def _compile(src, verbose):
+    obj = os.path.join(OBJDIR, src.replace(".cu", ".o"))
     deps = [os.path.join(CSRC, src)] + [os.path.join(CSRC, h) for h in HEADERS]
     if _mtime(obj) > max(_mtime(d) for d in deps):
         return obj, False
-    cmd = [NVCC] + NVCC_FLAGS + [f"-D{d}" for d in defines] + (["-Xptxas", "-v"] if verbose else []) + ["-c", os.path.join(CSRC, src), "-o", obj]
+    cmd = [NVCC] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-c", os.path.join(CSRC, src), "-o", obj]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"nvcc failed for {src}:\n{r.stdout}\n{r.stderr}")
@@ -48,23 +48,21 @@ def _compile(src, verbose, defines=(), tag=""):
     return obj, True
 
 
-def build(force: bool = False, verbose: bool = False, defines=(), tag: str = "") -> str:
-    """`defines` / `tag` build an experimental variant (e.g. defines=["B2_WS_RING=512"], tag="_r512") next to the default library."""
+def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(LIBDIR, exist_ok=True)
     os.makedirs(OBJDIR, exist_ok=True)
-    lib = LIB if not tag else LIB.replace(".so", tag + ".so")
     if force:
         for f in os.listdir(OBJDIR):
             os.remove(os.path.join(OBJDIR, f))
     with ThreadPoolExecutor(max_workers=len(SOURCES)) as ex:
-        results = list(ex.map(lambda s: _compile(s, verbose, defines, tag), SOURCES))
+        results = list(ex.map(lambda s: _compile(s, verbose), SOURCES))
     objs = [o for o, _ in results]
-    if any(changed for _, changed in results) or not os.path.exists(lib):
-        cmd = [NVCC, "-shared", "-ccbin", HOST_CXX, "-gencode", "arch=compute_90a,code=sm_90a", "-o", lib] + objs
+    if any(changed for _, changed in results) or not os.path.exists(LIB):
+        cmd = [NVCC, "-shared", "-ccbin", HOST_CXX, "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB] + objs
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")
-    return lib
+    return LIB
 
 
 if __name__ == "__main__":

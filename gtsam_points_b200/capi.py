@@ -11,7 +11,7 @@ import os
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("B2POINTS_LIB") or os.path.join(HERE, "lib", "libb2points.so")  # env override: experimental variants only
+LIB_PATH = os.path.join(HERE, "lib", "libb2points.so")
 
 B2_LINEARIZED_DOUBLES = 128
 B2_CLOUD_DEFAULT = 0

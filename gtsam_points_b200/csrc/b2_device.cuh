@@ -39,10 +39,7 @@ __device__ __forceinline__ VoxelBucket load_bucket(const VoxelBucket* p) {
 // the GPU the probe chain is pure latency, so its length is what counts -- and the factor kernel can stage the home group of
 // every point asynchronously (32 bytes per point in flight); the few keys whose home group is full continue with ordinary
 // loads.  (Round 1 used 64-byte groups of 4: 98 % one-access lookups, but twice the bytes per probe in flight.)
-#ifndef B2_BUCKET_GROUP
-#define B2_BUCKET_GROUP 2
-#endif
-constexpr int kGroup = B2_BUCKET_GROUP;
+constexpr int kGroup = 2;
 
 struct BucketGroup {
   int4 b[kGroup];

@@ -23,29 +23,68 @@
 // reaches that ring) or at the end of a factor run until the consumer acknowledges; an accumulate warp waits on a ring
 // only while it holds less than a batch and is not finished, in which case its producer is not blocked.  Waits sleep
 // between polls and are bounded (trap instead of hanging the GPU).
-// Measurement aids (never defined in the production build): B2_WS_TIMING (per-CTA timestamps), B2_WS_DEBUG_NO_PROBE /
-// B2_WS_DEBUG_NO_ACCUM (role isolation: results are garbage, timing only).
-// This file is included once per kernel configuration (no include guard): the includer defines B2_WS_NAMESPACE and the
-// B2_WS_* parameters (see b2_factors.cu), e.g. few fat accumulate warps + many thin probe warps for the kd-tree path.
+// What differs between factor kinds -- warp shape, source covariance, weight metric -- is KindTraits<KIND> below; DESIGN.md
+// section 4.1 gives the measurements behind the warp shapes.
+#pragma once
 
 namespace b2 {
-namespace B2_WS_NAMESPACE {
+namespace ws {
 
-constexpr int kP = B2_WS_PRODUCERS;
-constexpr int kC = B2_WS_CONSUMERS;
-constexpr int kThreads = (kP + kC) * 32;
-constexpr int kPPL = B2_WS_PPL;             // points per probe lane and tile (independent chains interleaved for ILP)
-constexpr int kWarpPoints = 32 * kPPL;      // contiguous source points per probe warp and tile
-constexpr int kTile = kP * kWarpPoints;     // source points per CTA tile
-constexpr uint32_t kPrefetchAhead = 3;      // tiles between the L2 prefetch of a tile's coordinates and their use
-constexpr int kRing = B2_WS_RING;           // items per ring (power of two, >= 64)
-constexpr int kRingsPerConsumer = kP / kC;
-constexpr int kIPL = B2_WS_IPL;             // correspondences per accumulate lane and batch (independent chains interleaved)
-static_assert(kP % 4 == 0 && kC % 4 == 0, "setmaxnreg works on warpgroups of 4 warps");
-static_assert(kP % kC == 0, "every accumulate warp drains the same number of rings");
-static_assert((kRing & (kRing - 1)) == 0 && kRing >= 2 * 32 * kIPL + kWarpPoints, "ring capacity: a tile's hits + one batch of publication lag + one batch");
-static_assert(kWarpPoints * 4 % 128 == 0 || kPPL == 1, "coordinate prefetch works on whole lines");
-constexpr size_t kRingBytes = static_cast<size_t>(kP) * 2 * kRing * sizeof(double2);  // dynamic shared memory of a launch
+// Warp shapes.  VGICP: voxel hash probe.
+struct VoxelProbeWarps {
+  static constexpr int kP = 8;        // probe warps
+  static constexpr int kC = 8;        // accumulate warps
+  static constexpr int kRegsP = 88;   // setmaxnreg of a probe warp
+  static constexpr int kRegsC = 168;  // setmaxnreg of an accumulate warp
+  static constexpr int kRing = 256;   // items per ring (power of two, >= 64)
+  static constexpr int kPPL = 2;      // points per probe lane and tile (independent chains interleaved for ILP)
+  static constexpr int kIPL = 2;      // correspondences per accumulate lane and batch (independent chains interleaved)
+};
+// kd-tree 1-NN / iVox neighbour search: the tree walk is ~100 dependent loads per point, the accumulate work is unchanged ->
+// many thin probe warps (the walk keeps its stack in local memory and needs few registers) feeding 4 fat accumulate warps.
+struct TreeProbeWarps {
+  static constexpr int kP = 28;
+  static constexpr int kC = 4;
+  static constexpr int kRegsP = 48;
+  static constexpr int kRegsC = 168;
+  static constexpr int kRing = 128;
+  static constexpr int kPPL = 1;
+  static constexpr int kIPL = 1;
+};
+
+// SOURCE_COV: the kind reads the source cloud's covariances (ICP kinds do not; their CT is a dummy).
+// METRIC: the weight matrix of accumulate_point_f (0 GICP / VGICP, 1 point-to-point ICP, 2 point-to-plane ICP).
+template <class Warps, bool SOURCE_COV, int METRIC>
+struct Traits : Warps {
+  static constexpr bool kSourceCov = SOURCE_COV;
+  static constexpr int kMetric = METRIC;
+  static constexpr int kThreads = (Warps::kP + Warps::kC) * 32;
+  static constexpr int kWarpPoints = 32 * Warps::kPPL;       // contiguous source points per probe warp and tile
+  static constexpr int kTile = Warps::kP * kWarpPoints;      // source points per CTA tile
+  static constexpr int kRingsPerConsumer = Warps::kP / Warps::kC;
+  static constexpr size_t kRingBytes = static_cast<size_t>(Warps::kP) * 2 * Warps::kRing * sizeof(double2);  // dynamic shared memory of a launch
+  static_assert(Warps::kP % 4 == 0 && Warps::kC % 4 == 0, "setmaxnreg works on warpgroups of 4 warps");
+  static_assert(Warps::kP % Warps::kC == 0, "every accumulate warp drains the same number of rings");
+  static_assert((Warps::kRing & (Warps::kRing - 1)) == 0 && Warps::kRing >= 2 * 32 * Warps::kIPL + kWarpPoints,
+                "ring capacity: a tile's hits + one batch of publication lag + one batch");
+  static_assert(kWarpPoints * 4 % 128 == 0 || Warps::kPPL == 1, "coordinate prefetch works on whole lines");
+};
+
+// One entry per b2_factor_kind.  Every kind but VGICP searches a kd-tree or an iVox.
+template <int KIND>
+struct KindTraits;
+template <>
+struct KindTraits<B2_FACTOR_VGICP> : Traits<VoxelProbeWarps, true, 0> {};
+template <>
+struct KindTraits<B2_FACTOR_GICP> : Traits<TreeProbeWarps, true, 0> {};
+template <>
+struct KindTraits<B2_FACTOR_ICP> : Traits<TreeProbeWarps, false, 1> {};
+template <>
+struct KindTraits<B2_FACTOR_ICP_PLANE> : Traits<TreeProbeWarps, false, 2> {};
+template <>
+struct KindTraits<B2_FACTOR_GICP_IVOX> : Traits<TreeProbeWarps, true, 0> {};
+
+constexpr uint32_t kPrefetchAhead = 3;  // tiles between the L2 prefetch of a tile's coordinates and their use
 
 constexpr unsigned kSpinLimit = 1u << 25;  // polls (with sleeps: >= 2 s, typically tens of seconds) before a wait traps: a protocol bug must not hang the GPU
 
@@ -71,32 +110,25 @@ struct Backoff {
   }
 };
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
+// barrier of the kC accumulate warps
+template <int kC>
 __device__ __forceinline__ void consumer_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(kC * 32) : "memory"); }
 
-#ifdef B2_WS_TIMING
-// development aid: per-CTA {start, probe warps done, accumulate warps done} timestamps of the last launch (ns)
-__device__ unsigned long long g_cta_times[1024 * 4];
-__device__ __forceinline__ unsigned long long globaltimer() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-#endif
-
+template <class K>
 struct Shared {
   FactorDesc desc;  // accumulate-side copy of the current factor's descriptor (flush / epilogue)
-  double red[kC][kAcc];
+  double red[K::kC][kAcc];
   double tot[kAcc];
   double A[36], X[36], D[36];
   double R[9], t[3];  // pose the residuals of the current factor run are evaluated at (accumulate side)
   double RL[9];       // rotation of its linearization point (== R when linearizing)
   int flag;
   // ring control words, one set per probe warp (all monotonic counters)
-  uint32_t tail[kP];  // items published by the probe warp
-  uint32_t head[kP];  // items taken by the accumulate warp
-  uint32_t done[kP];  // factor runs completed by the probe warp (tail is final for run e once done == e + 1)
-  uint32_t ack[kP];   // factor runs the accumulate warp has finished draining
-  double probe_pose[kP][12];  // per probe warp: R (9, row-major) | t (3) of the factor run it is working on
+  uint32_t tail[K::kP];  // items published by the probe warp
+  uint32_t head[K::kP];  // items taken by the accumulate warp
+  uint32_t done[K::kP];  // factor runs completed by the probe warp (tail is final for run e once done == e + 1)
+  uint32_t ack[K::kP];   // factor runs the accumulate warp has finished draining
+  double probe_pose[K::kP][12];  // per probe warp: R (9, row-major) | t (3) of the factor run it is working on
 };
 
 // tiles of CTA c: [c * T / G, (c + 1) * T / G) -- contiguous and balanced; the host uses the same formula for the slots
@@ -108,14 +140,15 @@ __host__ __device__ __forceinline__ uint32_t cta_tile_begin(uint32_t c, uint32_t
 // Per-factor flush by the accumulate warpgroup(s): warp butterfly -> cross-warp sum -> fixed slot; the last CTA of the
 // factor sums the slots in slot order and runs the epilogue (H_t = X^T A' X, ...).
 // ---------------------------------------------------------------------------------------------------------------
-template <int MODE>
-__device__ __forceinline__ void flush_factor(Shared& sh, double (&v)[kAcc], int ctid, double* __restrict__ partials, unsigned int* __restrict__ counters, double* __restrict__ out,
+template <int MODE, class K>
+__device__ __forceinline__ void flush_factor(Shared<K>& sh, double (&v)[kAcc], int ctid, double* __restrict__ partials, unsigned int* __restrict__ counters, double* __restrict__ out,
                                              const double* __restrict__ pose_lin /* this factor's linearization pose (16 doubles) */, const DoneSignal& sig) {
+  constexpr int kC = K::kC;
   constexpr int kCT = kC * 32;
   const int lane = ctid & 31, warp = ctid >> 5;
   const double w = warp_reduce32(v, lane);
   sh.red[warp][lane] = w;
-  consumer_barrier();
+  consumer_barrier<kC>();
   const FactorDesc& d = sh.desc;
   const uint32_t slot = blockIdx.x - d.cta_first[MODE];
   if (warp == 0) {
@@ -125,12 +158,12 @@ __device__ __forceinline__ void flush_factor(Shared& sh, double (&v)[kAcc], int 
     partials[(static_cast<size_t>(d.slot_begin[MODE]) + slot) * kAcc + lane] = s;
     __threadfence();  // only the writing warp pays for the fence
   }
-  consumer_barrier();
+  consumer_barrier<kC>();
   if (ctid == 0) {
     const unsigned int prev = atomicAdd(&counters[d.out_index], 1u);
     sh.flag = (prev == d.num_slots[MODE] - 1u) ? 1 : 0;
   }
-  consumer_barrier();
+  consumer_barrier<kC>();
   if (!sh.flag) return;
 
   // ---- last CTA of this factor ----
@@ -153,7 +186,7 @@ __device__ __forceinline__ void flush_factor(Shared& sh, double (&v)[kAcc], int 
     }
     sh.red[warp][lane] = s;
   }
-  consumer_barrier();
+  consumer_barrier<kC>();
   if (ctid < kAcc) {
     double s = sh.red[0][ctid];
 #pragma unroll
@@ -161,7 +194,7 @@ __device__ __forceinline__ void flush_factor(Shared& sh, double (&v)[kAcc], int 
     sh.tot[ctid] = s;
   }
   if (ctid == 0) counters[d.out_index] = 0u;  // re-arm for the next launch
-  consumer_barrier();
+  consumer_barrier<kC>();
 
   // results in mapped host memory / peer memory always come with a completion signal: only then the fence must be system-wide
   const bool system_scope = sig.flag != nullptr || sig.n_peers > 0;
@@ -173,11 +206,11 @@ __device__ __forceinline__ void flush_factor(Shared& sh, double (&v)[kAcc], int 
         signal_done(sig);
       }
     }
-    consumer_barrier();
+    consumer_barrier<kC>();
     return;
   }
   epilogue_build(sh.A, sh.X, sh.D, sh.tot, sh.R, sh.t, ctid);
-  consumer_barrier();
+  consumer_barrier<kC>();
   double* rec = out + static_cast<size_t>(d.out_index) * B2_LINEARIZED_DOUBLES;
   epilogue_store(rec, sh.A, sh.X, sh.D, sh.tot, ctid);
   if (ctid >= 100 && ctid < 116) {
@@ -187,7 +220,7 @@ __device__ __forceinline__ void flush_factor(Shared& sh, double (&v)[kAcc], int 
   // `out` may be mapped host memory (zero-copy host API): fence at system scope before the completion signal.  With peers, `out`
   // is this GPU's own device block and ONE system fence after the peer copies below covers everything that leaves the GPU
   if (system_scope && sig.n_peers <= 1) __threadfence_system();
-  consumer_barrier();
+  consumer_barrier<kC>();
   if (sig.n_peers > 1) {
     // multi-GPU exchange fused into the epilogue: copy the finished record into the same slot of every peer's buffer
     // (plain stores to peer memory over NVLink), fence at system scope, then signal
@@ -197,7 +230,7 @@ __device__ __forceinline__ void flush_factor(Shared& sh, double (&v)[kAcc], int 
       for (int i = ctid; i < B2_LINEARIZED_DOUBLES; i += kCT) dst[i] = __ldcg(rec + i);
     }
     __threadfence_system();
-    consumer_barrier();
+    consumer_barrier<kC>();
   }
   if (sig.mirror == nullptr) {
     if (ctid == 0) signal_done(sig);  // every writer of this record fenced before the barrier
@@ -205,10 +238,10 @@ __device__ __forceinline__ void flush_factor(Shared& sh, double (&v)[kAcc], int 
     // exchange step with host delivery: the CTA that completes the call (and waited for the peers) copies every rank's records
     // from this GPU's block to mapped host memory, then raises the host's completion word
     if (ctid == 0) sh.flag = signal_done(sig) ? 1 : 0;
-    consumer_barrier();
+    consumer_barrier<kC>();
     if (sh.flag) {
       mirror_to_host(sig, ctid, kCT);
-      consumer_barrier();
+      consumer_barrier<kC>();
       if (ctid == 0) *sig.mirror_flag = sig.mirror_seq;
     }
   }
@@ -225,6 +258,7 @@ struct Batch {
   SourceCov A;
 };
 
+template <int kRing>
 __device__ __forceinline__ void load_meta(Batch& b, const double2* __restrict__ ring, uint32_t head, uint32_t n, int lane) {
   b.valid = static_cast<uint32_t>(lane) < n;
   const uint32_t slot = (head + lane) & (kRing - 1);
@@ -239,36 +273,30 @@ __device__ __forceinline__ void load_meta(Batch& b, const double2* __restrict__ 
   b.id = b.valid ? static_cast<int>(bits >> 32) : 0;
 }
 
-// KIND: 0 VGICP, 1 GICP, 2 point-to-point ICP, 3 point-to-plane ICP (kd-tree search for 1..3; ICP factors carry no source covariance),
-// 4 GICP on an iVox (neighbour-voxel search over its point slots)
-template <int KIND>
-struct HasSourceCov {
-  static constexpr bool value = KIND <= 1 || KIND == 4;
-};
 template <typename CT, int KIND>
 __device__ __forceinline__ void load_operands(Batch& b, const double* __restrict__ records, const CT* __restrict__ cv, size_t n_pad) {
   b.T = load_record(records, b.id);
-  if (HasSourceCov<KIND>::value)
+  if (KindTraits<KIND>::kSourceCov)
     b.A = load_cov(cv, n_pad, b.i);
   else
     b.A = SourceCov{0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
 }
-template <int KIND>
-struct MetricOf {
-  static constexpr int value = HasSourceCov<KIND>::value ? 0 : KIND - 1;
-};
 
 // ---------------------------------------------------------------------------------------------------------------
-// The kernel.  KIND: 0 = VGICP (voxel hash probe), 1..3 = GICP / ICP (kd-tree 1-NN), 4 = GICP on an iVox.  MODE: linearize / error-only.
+// The kernel.  KIND: a b2_factor_kind; it selects the search (voxel hash probe, kd-tree 1-NN or iVox neighbour voxels) and
+// KindTraits<KIND>.  MODE: linearize / error-only.
 // ---------------------------------------------------------------------------------------------------------------
 // SINGLE: the launch covers exactly one factor and its pose is the by-value parameter `pose` (linearize: the linearization
 // point; error: the evaluation point) -- DMUL / DFMA take it from uniform registers, nothing is read from host memory.
 template <typename PT, typename CT, int KIND, int MODE, bool SINGLE = false>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(KindTraits<KIND>::kThreads, 1)
 factor_kernel(const FactorDesc* __restrict__ descs, const uint32_t* __restrict__ tile_factor, uint32_t num_tiles, const double* __restrict__ poses_lin,
               const double* __restrict__ poses_eval, double* __restrict__ partials, unsigned int* __restrict__ counters, double* __restrict__ out,
               const __grid_constant__ DoneSignal sig, const __grid_constant__ PoseArg pose, const uint32_t* __restrict__ frozen_flags) {
-  __shared__ Shared sh;
+  using K = KindTraits<KIND>;
+  constexpr int kP = K::kP, kC = K::kC, kPPL = K::kPPL, kWarpPoints = K::kWarpPoints, kTile = K::kTile, kRing = K::kRing;
+  constexpr int kRingsPerConsumer = K::kRingsPerConsumer, kIPL = K::kIPL;
+  __shared__ Shared<K> sh;
   extern __shared__ __align__(16) unsigned char dyn_smem[];
   double2* const rings = reinterpret_cast<double2*>(dyn_smem);
 
@@ -281,16 +309,13 @@ factor_kernel(const FactorDesc* __restrict__ descs, const uint32_t* __restrict__
   }
   __syncthreads();
 
-#ifdef B2_WS_TIMING
-  if (tid == 0) g_cta_times[blockIdx.x * 4 + 0] = globaltimer();
-#endif
   const uint32_t G = gridDim.x;
   const uint32_t tile_lo = cta_tile_begin(blockIdx.x, num_tiles, G);
   const uint32_t tile_hi = cta_tile_begin(blockIdx.x + 1, num_tiles, G);
 
   if (warp < kP) {
     // ================================================= PROBE warps =================================================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(B2_WS_REGS_PRODUCER));
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(K::kRegsP));
     const int p = warp;
     double2* const ring = rings + static_cast<size_t>(p) * 2 * kRing;
     uint32_t tail = 0u, run = 0u;
@@ -304,9 +329,9 @@ factor_kernel(const FactorDesc* __restrict__ descs, const uint32_t* __restrict__
       const uint32_t out_index = dg->out_index;
       // correspondence-update tolerance (integrated_gicp_factor_impl.hpp:135-147): the host decided that this factor's pose moved
       // less than its tolerances since the last association -> keep the stored correspondences, linearize them at the new pose
-      // (the voxel path always re-associates -- integrated_vgicp_factor_impl.hpp:99 has no tolerance test -- so for KIND 0 this is a
+      // (the voxel path always re-associates -- integrated_vgicp_factor_impl.hpp:99 has no tolerance test -- so for VGICP this is a
       // compile-time constant and costs the probe warps neither registers nor branches)
-      const bool frozen = MODE == MODE_ERROR || (KIND != 0 && frozen_flags != nullptr && __ldg(frozen_flags + out_index) != 0u);
+      const bool frozen = MODE == MODE_ERROR || (KIND != B2_FACTOR_VGICP && frozen_flags != nullptr && __ldg(frozen_flags + out_index) != 0u);
       const PT* __restrict__ px = static_cast<const PT*>(dg->pts);
       const CT* __restrict__ cv = static_cast<const CT*>(dg->covs);
       const double* __restrict__ records = dg->records;
@@ -397,32 +422,26 @@ factor_kernel(const FactorDesc* __restrict__ descs, const uint32_t* __restrict__
             u[k][1] = __dadd_rn(__dadd_rn(__dmul_rn(Rm(3), x), __dmul_rn(Rm(4), y)), __dmul_rn(Rm(5), z));
             u[k][2] = __dadd_rn(__dadd_rn(__dmul_rn(Rm(6), x), __dmul_rn(Rm(7), y)), __dmul_rn(Rm(8), z));
           }
-          if (MODE == MODE_LINEARIZE && KIND == 0 && !frozen) {
+          if (MODE == MODE_LINEARIZE && KIND == B2_FACTOR_VGICP && !frozen) {
             cx[k] = voxel_coord1(__dadd_rn(u[k][0], tvec(0)), inv_leaf);
             cy[k] = voxel_coord1(__dadd_rn(u[k][1], tvec(1)), inv_leaf);
             cz[k] = voxel_coord1(__dadd_rn(u[k][2], tvec(2)), inv_leaf);
             grp_idx[k] = voxel_hash(cx[k], cy[k], cz[k]) & bucket_mask;
-#ifndef B2_WS_DEBUG_NO_PROBE
             grp[k] = load_group(buckets, grp_idx[k]);
-#endif
           }
         }
         uint32_t mask[kPPL], cnt = 0u;
 #pragma unroll
         for (int k = 0; k < kPPL; k++) {
           if (MODE == MODE_LINEARIZE && !frozen) {
-            if (KIND == 0) {
-#ifdef B2_WS_DEBUG_NO_PROBE
-              id[k] = static_cast<int>(grp_idx[k] & 0xffffu);  // measurement aid: no table access, every point "hits" some record
-#else
+            if (KIND == B2_FACTOR_VGICP) {
               id[k] = match_group(grp[k], cx[k], cy[k], cz[k]);
-#endif
               uint32_t g = grp_idx[k];
               while (id[k] == -2) {  // rare (<2% at load <= 0.25): the home group is full, walk on
                 g = (g + 1) & bucket_mask;
                 id[k] = match_group(load_group(buckets, g), cx[k], cy[k], cz[k]);
               }
-            } else if (KIND == 4) {
+            } else if (KIND == B2_FACTOR_GICP_IVOX) {
               // iVox: the neighbour voxels of the transformed point (offset order) through the bucket table, their point slots in
               // order; the ivox's point counts travel in leaf_pts, slots per voxel | neighbour mode << 8 in ivox_slots_mode
               id[k] = ok[k] ? ivox_nn1(buckets, bucket_mask, inv_leaf, records, static_cast<const uint32_t*>(dg->leaf_pts), static_cast<int>(dg->ivox_slots_mode & 0xffu),
@@ -456,7 +475,7 @@ factor_kernel(const FactorDesc* __restrict__ descs, const uint32_t* __restrict__
             prefetch_l2(rec);
             prefetch_l2(rec + 72);
           }
-          if (HasSourceCov<KIND>::value && lane < 12) {
+          if (K::kSourceCov && lane < 12) {
             // covariance lines of this 32-point group: 6 planes x 2 halves of 16 points
             const uint32_t half = lane & 1, plane = lane >> 1;
             if ((mask[k] >> (16 * half)) & 0xffffu) prefetch_l2(cv + plane * n_pad + (base - lane) + k * 32 + 16 * half);
@@ -475,12 +494,9 @@ factor_kernel(const FactorDesc* __restrict__ descs, const uint32_t* __restrict__
         while (ld_acquire(&sh.ack[p]) != run) bo.wait();
       }
     }
-#ifdef B2_WS_TIMING
-    if (lane == 0) atomicMax(&g_cta_times[blockIdx.x * 4 + 1], globaltimer());
-#endif
   } else {
     // =============================================== ACCUMULATE warps ===============================================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(B2_WS_REGS_CONSUMER));
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(K::kRegsC));
     const int cw = warp - kP;          // accumulate warp index
     const int ctid = tid - kP * 32;    // thread index within the accumulate group
     uint32_t head[kRingsPerConsumer];  // items taken from each of this warp's rings
@@ -491,10 +507,10 @@ factor_kernel(const FactorDesc* __restrict__ descs, const uint32_t* __restrict__
     double acc[kAcc];
     while (tile < tile_hi) {
       const uint32_t f = SINGLE ? 0u : __ldg(tile_factor + tile);
-      consumer_barrier();  // previous flush is done with sh.desc
+      consumer_barrier<kC>();  // previous flush is done with sh.desc
       if (ctid < static_cast<int>(sizeof(FactorDesc) / 4))
         reinterpret_cast<uint32_t*>(&sh.desc)[ctid] = SINGLE ? reinterpret_cast<const uint32_t*>(&pose.desc)[ctid] : __ldg(reinterpret_cast<const uint32_t*>(descs + f) + ctid);
-      consumer_barrier();
+      consumer_barrier<kC>();
       const FactorDesc& d = sh.desc;
       if (ctid < 21) {
         const double* pe = SINGLE ? pose.m : ((MODE == MODE_ERROR ? poses_eval : poses_lin) + static_cast<size_t>(d.out_index) * 16);
@@ -506,7 +522,7 @@ factor_kernel(const FactorDesc* __restrict__ descs, const uint32_t* __restrict__
         else
           sh.RL[ctid - 12] = pl[((ctid - 12) / 3) * 4 + (ctid - 12) % 3];
       }
-      consumer_barrier();
+      consumer_barrier<kC>();
       constexpr bool kConstRL = SINGLE && MODE == MODE_LINEARIZE;
       double RLr[kConstRL ? 1 : 9], tr[SINGLE ? 1 : 3];
       if (!kConstRL) {
@@ -571,29 +587,21 @@ factor_kernel(const FactorDesc* __restrict__ descs, const uint32_t* __restrict__
 #pragma unroll
           for (int j = 0; j < kIPL; j++) {
             const uint32_t nj = nb > 32u * j ? min(32u, nb - 32u * j) : 0u;
-            load_meta(b[j], rings + static_cast<size_t>(p) * 2 * kRing, hd + 32u * j, nj, lane);
-#ifndef B2_WS_DEBUG_NO_ACCUM
+            load_meta<kRing>(b[j], rings + static_cast<size_t>(p) * 2 * kRing, hd + 32u * j, nj, lane);
             load_operands<CT, KIND>(b[j], records, cv, n_pad);  // lanes beyond nj gather element 0 (valid memory), masked below
-#endif
           }
 #pragma unroll
           for (int k = 0; k < kRingsPerConsumer; k++)
             if (k == r) head[k] = hd + nb;
-#ifdef B2_WS_DEBUG_NO_ACCUM
-#pragma unroll
-          for (int j = 0; j < kIPL; j++)
-            if (b[j].valid) acc[28] += b[j].u0 * 0.0 + 1.0;  // measurement aid: probe-side throughput only
-#else
           if (nb == kBatch) {
             // full batch (uniform branch): no per-lane predicates, the kIPL bodies sit in one basic block and interleave
 #pragma unroll
-            for (int j = 0; j < kIPL; j++) accumulate_point_f<MODE, MetricOf<KIND>::value>(acc, rl, tt, b[j].u0, b[j].u1, b[j].u2, b[j].T, b[j].A);
+            for (int j = 0; j < kIPL; j++) accumulate_point_f<MODE, K::kMetric>(acc, rl, tt, b[j].u0, b[j].u1, b[j].u2, b[j].T, b[j].A);
           } else {
 #pragma unroll
             for (int j = 0; j < kIPL; j++)
-              if (b[j].valid) accumulate_point_f<MODE, MetricOf<KIND>::value>(acc, rl, tt, b[j].u0, b[j].u1, b[j].u2, b[j].T, b[j].A);
+              if (b[j].valid) accumulate_point_f<MODE, K::kMetric>(acc, rl, tt, b[j].u0, b[j].u1, b[j].u2, b[j].T, b[j].A);
           }
-#endif
         }
         if (fin) {
           finished |= 1u << r;
@@ -606,17 +614,11 @@ factor_kernel(const FactorDesc* __restrict__ descs, const uint32_t* __restrict__
         }
         r = (r + 1 == kRingsPerConsumer) ? 0 : r + 1;
       }
-#ifdef B2_WS_TIMING
-      if (lane == 0) atomicMax(&g_cta_times[blockIdx.x * 4 + 2], globaltimer());
-#endif
       flush_factor<MODE>(sh, acc, ctid, partials, counters, out, SINGLE ? pose.m : (poses_lin + static_cast<size_t>(sh.desc.out_index) * 16), sig);
-#ifdef B2_WS_TIMING
-      if (lane == 0) atomicMax(&g_cta_times[blockIdx.x * 4 + 3], globaltimer());  // flush (and, in the factor's last CTA, the epilogue) done
-#endif
       tile = run_end;
     }
   }
 }
 
-}  // namespace B2_WS_NAMESPACE
+}  // namespace ws
 }  // namespace b2

@@ -28,10 +28,7 @@
 namespace b2 {
 namespace {
 
-#ifndef B2_KD_LEAF
-#define B2_KD_LEAF 16
-#endif
-constexpr int kMaxLeaf = B2_KD_LEAF;
+constexpr int kMaxLeaf = 16;
 
 // order-preserving map double -> uint64 (sort keys, atomicMin / atomicMax on coordinates)
 __host__ __device__ __forceinline__ unsigned long long ordered_bits(double v) {

@@ -48,7 +48,6 @@ __global__ void scan_raw_kernel(const double* __restrict__ pts, int pstride, con
                                 ScanResult* __restrict__ res) {
   double mn[3] = {1e300, 1e300, 1e300}, mx[3] = {-1e300, -1e300, -1e300};
   unsigned int flags = 0;
-  const int ld = cstride == 16 ? 4 : 3;
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
 #pragma unroll
     for (int k = 0; k < 3; k++) {
@@ -59,15 +58,12 @@ __global__ void scan_raw_kernel(const double* __restrict__ pts, int pstride, con
       mx[k] = fmax(mx[k], v);
     }
     if (covs) {
-      const double* c = covs + i * cstride;
+      double u[6];
+      cov_upper(covs + i * cstride, cstride, u);
 #pragma unroll
-      for (int r = 0; r < 3; r++) {
-#pragma unroll
-        for (int k = r; k < 3; k++) {
-          const double v = c[r * ld + k];
-          if (!isfinite(v)) flags |= 4u;
-          if (!f32_exact(v)) flags |= 2u;
-        }
+      for (int k = 0; k < 6; k++) {
+        if (!isfinite(u[k])) flags |= 4u;
+        if (!f32_exact(u[k])) flags |= 2u;
       }
     }
   }
@@ -136,14 +132,10 @@ __global__ void gather_planes_kernel(const double* __restrict__ pts, int pstride
 #pragma unroll
   for (int k = 0; k < 3; k++) out_p[k * n_pad + i] = static_cast<PT>(pts[s * pstride + k]);
   if (out_c) {
-    const int ld = cstride == 16 ? 4 : 3;
-    const double* c = covs + s * cstride;
-    out_c[0 * n_pad + i] = static_cast<CT>(c[0 * ld + 0]);
-    out_c[1 * n_pad + i] = static_cast<CT>(c[0 * ld + 1]);
-    out_c[2 * n_pad + i] = static_cast<CT>(c[0 * ld + 2]);
-    out_c[3 * n_pad + i] = static_cast<CT>(c[1 * ld + 1]);
-    out_c[4 * n_pad + i] = static_cast<CT>(c[1 * ld + 2]);
-    out_c[5 * n_pad + i] = static_cast<CT>(c[2 * ld + 2]);
+    CT u[6];
+    cov_upper(covs + s * cstride, cstride, u);
+#pragma unroll
+    for (int k = 0; k < 6; k++) out_c[k * n_pad + i] = u[k];
   }
 }
 

@@ -38,9 +38,8 @@ __device__ __forceinline__ VoxelBucket load_bucket(const VoxelBucket* p) {
 // for a load factor <= 0.25: ~95 % of all lookups (hits AND misses) resolve inside the home group, i.e. with ONE access -- on
 // the GPU the probe chain is pure latency, so its length is what counts -- and the factor kernel can stage the home group of
 // every point asynchronously (32 bytes per point in flight); the few keys whose home group is full continue with ordinary
-// loads.  (Round 1 used 64-byte groups of 4: 98 % one-access lookups, but twice the bytes per probe in flight.)
-constexpr int kGroup = 2;
-
+// loads.  (Round 1 used 64-byte groups of 4: 98 % one-access lookups, but twice the bytes per probe in flight.)  kGroup is
+// defined beside VoxelBucket (b2_internal.hpp).
 struct BucketGroup {
   int4 b[kGroup];
 };

@@ -143,9 +143,39 @@ struct alignas(16) VoxelBucket {
   int32_t id;  // -1 = empty
 };
 
+// Buckets per group of a voxel table (b2_device.cuh: bucket groups); the number of groups is a power of two.
+constexpr int kGroup = 2;
+
 // One target record: mean (3), upper-triangular covariance (6), number of points (1).  80 bytes = 5 x LDG.128.
 // Used for voxels (VGICP) and for target points (GICP, count = 1).
 constexpr int kRecordDoubles = 10;
+
+// Payload doubles per voxel of a voxel map with `slots` point slots per voxel (b2_voxelmap::slots): one Gaussian voxel record
+// for slots = 0, else one point record per slot.
+inline size_t voxel_payload_doubles(int slots) { return static_cast<size_t>(slots > 0 ? slots : 1) * kRecordDoubles; }
+
+// Covariance records hold the upper triangle (00, 01, 02, 11, 12, 22) of a symmetric 3x3.
+// cov_upper: the six entries of a row-major 3x3 (stride 9) or 4x4 (stride 16) input.
+template <typename T>
+__host__ __device__ __forceinline__ void cov_upper(const double* c, int stride, T* u) {
+  const int ld = stride == 16 ? 4 : 3;
+  u[0] = static_cast<T>(c[0 * ld + 0]);
+  u[1] = static_cast<T>(c[0 * ld + 1]);
+  u[2] = static_cast<T>(c[0 * ld + 2]);
+  u[3] = static_cast<T>(c[1 * ld + 1]);
+  u[4] = static_cast<T>(c[1 * ld + 2]);
+  u[5] = static_cast<T>(c[2 * ld + 2]);
+}
+// cov_full: the row-major symmetric 3x3 of the six entries.
+template <typename T>
+__host__ __device__ __forceinline__ void cov_full(const T* u, double* c) {
+  c[0] = u[0];
+  c[1] = c[3] = u[1];
+  c[2] = c[6] = u[2];
+  c[4] = u[3];
+  c[5] = c[7] = u[4];
+  c[8] = u[5];
+}
 
 // kd-tree node, 16 bytes = one LDG.128.
 //   internal: thresh = split value, a = index of the left child (right child = a + 1), b = axis (0..2)
@@ -191,6 +221,9 @@ struct b2_cloud {
   size_t device_bytes() const { return d_points.bytes() + d_covs.bytes() + d_perm.bytes(); }
 };
 
+// A voxel-keyed map: a bucket table (integer voxel coordinate -> voxel id) over per-voxel arrays in id order.  `slots` is the
+// per-voxel layout: 0 = one Gaussian voxel record per voxel (the Gaussian voxel map); k > 0 = k point-record slots per voxel plus
+// a per-voxel point count (the iVox).
 struct b2_voxelmap {
   b2_ctx* ctx = nullptr;
   double resolution = 0.0;
@@ -198,27 +231,27 @@ struct b2_voxelmap {
   size_t num_voxels = 0;
   size_t num_buckets = 0;  // power of two
   b2::DeviceBuffer d_buckets;  // num_buckets VoxelBucket
-  b2::DeviceBuffer d_records;  // double: capacity x rec_doubles
+  b2::DeviceBuffer d_records;  // double: capacity x voxel_payload_doubles(slots)
   b2::DeviceBuffer d_coords;   // int32: capacity x 3 (id order), kept for download
   // incremental insertion state (ann/incremental_voxelmap.hpp:13-28): LRU bookkeeping as in the CPU map
   b2::DeviceBuffer d_lru;        // uint32 per voxel: lru_counter value of the last insert() that touched it
-  size_t capacity = 0;           // voxels the record / coord / lru arrays can hold
+  size_t capacity = 0;           // voxels the per-voxel arrays can hold
   size_t lru_horizon = 10, lru_clear_cycle = 10, lru_counter = 0;
   uint64_t generation = 0;       // bumped whenever the device pointers / voxel ids change: factor sets refresh their descriptors
-  // per-voxel payload: kRecordDoubles for a Gaussian voxel map; an iVox keeps `stride` point records per voxel plus a point count
-  size_t rec_doubles = b2::kRecordDoubles;
-  b2::DeviceBuffer d_counts;     // iVox only, uint32: points stored per voxel (slots 0..count-1 of its records are occupied)
+  int slots = 0;                 // point slots per voxel (0: Gaussian voxel records)
+  b2::DeviceBuffer d_counts;     // slots > 0 only, uint32: points stored per voxel (slots 0..count-1 of its records are occupied)
+  uint32_t group_mask() const { return static_cast<uint32_t>(num_buckets / b2::kGroup - 1); }  // bucket groups - 1
   size_t device_bytes() const { return d_buckets.bytes() + d_records.bytes() + d_coords.bytes() + d_lru.bytes() + d_counts.bytes(); }
 };
 
-// IncrementalVoxelMap<FlatContainer> / iVox (ann/incremental_voxelmap.hpp, ann/flat_container.hpp, ann/ivox.hpp): the voxel-keyed
-// machinery of the Gaussian voxel map, with up to `stride` point records (mean = the point, covariance, count = 1) per voxel.
+// IncrementalVoxelMap<FlatContainer> / iVox (ann/incremental_voxelmap.hpp, ann/flat_container.hpp, ann/ivox.hpp): a voxel map with
+// point slots (mean = the point, covariance, count = 1).  Until the first insert fixes map.slots (to max_num_points_in_cell), the
+// map keeps the Gaussian layout of an empty map.
 struct b2_ivox {
-  b2_voxelmap map;                  // map.rec_doubles = stride * kRecordDoubles, map.d_counts = per-voxel point counts
+  b2_voxelmap map;
   int neighbor_mode = 7;            // 1, 7, 19 or 27 (incremental_voxelmap_impl.hpp:95-140)
   double min_sq_dist_in_cell = 0.1 * 0.1;  // FlatContainer::Setting (flat_container.hpp:19-23)
   int max_num_points_in_cell = 20;
-  int stride = 0;                   // point slots per voxel, fixed by the first insert (0: not fixed yet)
   int has_covs = -1;                // -1 unknown (nothing inserted yet), 0 / 1: whether inserted points carry covariances
 };
 

@@ -12,9 +12,10 @@
 // order), a scan over segment heads, one more sort of the segments by first-touch index, then one thread per voxel
 // accumulates its points sequentially.  Everything is deterministic.
 //
-// The same voxel-keyed machinery (segmentation, first-touch ids, lookups of existing voxels, LRU sweep, table rebuild) also
-// carries the iVox (IncrementalVoxelMap<FlatContainer>, ann/incremental_voxelmap.hpp, ann/flat_container.hpp): only the per-voxel
-// step differs -- FlatContainer::add gates each point into one of `stride` fixed point slots of its voxel.
+// The same voxel-keyed machinery (segmentation, first-touch ids, lookups of existing voxels, per-voxel arrays, LRU sweep, table
+// rebuild) also carries the iVox (IncrementalVoxelMap<FlatContainer>, ann/incremental_voxelmap.hpp, ann/flat_container.hpp): one
+// insert routine and one insert kernel serve both, and only the kernel's per-voxel step differs -- FlatContainer::add gates each
+// point into one of the map's `slots` fixed point slots of its voxel.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_reduce.cuh>
 #include <cub/device/device_scan.cuh>
@@ -93,56 +94,98 @@ __global__ void batch_voxels_kernel(const double* __restrict__ pts, int pstride,
   is_new[r] = e < 0 ? 1u : 0u;
 }
 
-// One thread per voxel of the batch: GaussianVoxel::add for each of its points in insertion order, then finalize
-// (src/gtsam_points/types/gaussian_voxelmap_cpu.cpp:23-47).  A voxel that already exists is finalized, so add() first
-// re-opens it (mean *= n, cov *= n); the sums then continue from there one point at a time -- exactly the CPU's float64
-// operation sequence, so means / covariances stay bit-identical over any number of insert() calls.
-__global__ void accumulate_voxels_kernel(const double* __restrict__ pts, int pstride, const double* __restrict__ covs, int cstride, size_t n, size_t num_batch,
-                                         const uint32_t* __restrict__ idx, const uint32_t* __restrict__ seg_start, const uint32_t* __restrict__ seg_of_rank,
-                                         const int32_t* __restrict__ batch_coords, const int32_t* __restrict__ existing_id, const uint32_t* __restrict__ new_rank,
-                                         size_t num_existing, uint32_t lru_counter, double* __restrict__ records, int32_t* __restrict__ coords, uint32_t* __restrict__ lru) {
+// The points of one voxel of an inserted batch: pts / covs rows idx[begin..end), in insertion order (covs may be NULL for the iVox).
+struct CellPoints {
+  const double *pts, *covs;
+  int pstride, cstride;
+  const uint32_t* idx;
+  size_t begin, end;
+};
+
+// Per-voxel step of the Gaussian voxel map (slots = 0): GaussianVoxel::add for each point in insertion order, then finalize
+// (src/gtsam_points/types/gaussian_voxelmap_cpu.cpp:23-47).  A voxel that already exists is finalized, so add() first re-opens it
+// (mean *= n, cov *= n); the sums then continue from there one point at a time -- exactly the CPU's float64 operation sequence, so
+// means / covariances stay bit-identical over any number of insert() calls.
+struct GaussianCell {
+  __device__ __forceinline__ void add(const CellPoints& b, bool existing, double* __restrict__ records, uint32_t* __restrict__, size_t dest) const {
+    double* rec = records + dest * kRecordDoubles;
+    double m[3] = {0, 0, 0}, c[6] = {0, 0, 0, 0, 0, 0}, cnt0 = 0.0;
+    if (existing) {
+      cnt0 = rec[9];
+#pragma unroll
+      for (int k = 0; k < 3; k++) m[k] = __dmul_rn(rec[k], cnt0);
+#pragma unroll
+      for (int k = 0; k < 6; k++) c[k] = __dmul_rn(rec[3 + k], cnt0);
+    }
+    for (size_t j = b.begin; j < b.end; j++) {
+      const size_t i = b.idx[j];
+      const double* p = b.pts + i * b.pstride;
+      double u[6];
+      cov_upper(b.covs + i * b.cstride, b.cstride, u);
+#pragma unroll
+      for (int k = 0; k < 3; k++) m[k] = __dadd_rn(m[k], p[k]);
+#pragma unroll
+      for (int k = 0; k < 6; k++) c[k] = __dadd_rn(c[k], u[k]);
+    }
+    const double cnt = cnt0 + static_cast<double>(b.end - b.begin);
+#pragma unroll
+    for (int k = 0; k < 3; k++) rec[k] = __ddiv_rn(m[k], cnt);
+#pragma unroll
+    for (int k = 0; k < 6; k++) rec[3 + k] = __ddiv_rn(c[k], cnt);
+    rec[9] = cnt;
+  }
+};
+
+// Per-voxel step of the iVox (slots > 0): FlatContainer::add (flat_container.hpp:33-50) for each point in insertion order -- rejected
+// if the voxel already holds max_points points or a stored point lies closer than min_sq -- appending the rest to the voxel's slots
+// as records (point | covariance upper | 1).
+struct FlatCell {
+  int slots, max_points;
+  double min_sq;
+  __device__ __forceinline__ void add(const CellPoints& b, bool existing, double* __restrict__ records, uint32_t* __restrict__ counts, size_t dest) const {
+    double* rec = records + dest * static_cast<size_t>(slots) * kRecordDoubles;
+    int cnt = existing ? static_cast<int>(counts[dest]) : 0;
+    for (size_t j = b.begin; j < b.end && cnt < max_points; j++) {
+      const size_t i = b.idx[j];
+      const double* p = b.pts + i * b.pstride;
+      bool reject = false;
+      for (int q = 0; q < cnt && !reject; q++) reject = ivox_sq_dist(rec[q * kRecordDoubles + 0], rec[q * kRecordDoubles + 1], rec[q * kRecordDoubles + 2], p[0], p[1], p[2]) < min_sq;
+      if (reject) continue;
+      double* o = rec + static_cast<size_t>(cnt) * kRecordDoubles;
+      o[0] = p[0], o[1] = p[1], o[2] = p[2];
+      if (b.covs) {
+        cov_upper(b.covs + i * b.cstride, b.cstride, o + 3);
+      } else {
+        o[3] = o[4] = o[5] = o[6] = o[7] = o[8] = 0.0;
+      }
+      o[9] = 1.0;
+      cnt++;
+    }
+    counts[dest] = static_cast<uint32_t>(cnt);
+  }
+};
+
+// Insert (IncrementalVoxelMap::insert, incremental_voxelmap_impl.hpp:31-50): one thread per voxel of the batch runs the cell's
+// per-voxel step over its points, gives a new voxel its coordinate and stamps the voxel's lru -- also when the step took no point.
+template <typename Cell>
+__global__ void insert_voxels_kernel(Cell cell, const double* __restrict__ pts, int pstride, const double* __restrict__ covs, int cstride, size_t n, size_t num_batch,
+                                     const uint32_t* __restrict__ idx, const uint32_t* __restrict__ seg_start, const uint32_t* __restrict__ seg_of_rank,
+                                     const int32_t* __restrict__ batch_coords, const int32_t* __restrict__ existing_id, const uint32_t* __restrict__ new_rank,
+                                     size_t num_existing, uint32_t lru_counter, double* __restrict__ records, uint32_t* __restrict__ counts, int32_t* __restrict__ coords,
+                                     uint32_t* __restrict__ lru) {
   const size_t r = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
   if (r >= num_batch) return;
   const uint32_t s = seg_of_rank[r];
   const size_t begin = seg_start[s];
   const size_t end = (s + 1 < num_batch) ? seg_start[s + 1] : n;
-  const int ld = cstride == 16 ? 4 : 3;
   const int e = existing_id[r];
   const size_t dest = e >= 0 ? static_cast<size_t>(e) : num_existing + new_rank[r];  // new voxels: first-touch order after the existing ones
-  double* rec = records + dest * kRecordDoubles;
-  double m[3] = {0, 0, 0}, c[6] = {0, 0, 0, 0, 0, 0}, cnt0 = 0.0;
-  if (e >= 0) {
-    cnt0 = rec[9];
-#pragma unroll
-    for (int k = 0; k < 3; k++) m[k] = __dmul_rn(rec[k], cnt0);
-#pragma unroll
-    for (int k = 0; k < 6; k++) c[k] = __dmul_rn(rec[3 + k], cnt0);
-  }
-  for (size_t j = begin; j < end; j++) {
-    const size_t i = idx[j];
-    const double* p = pts + i * pstride;
-    const double* cv = covs + i * cstride;
-    m[0] = __dadd_rn(m[0], p[0]);
-    m[1] = __dadd_rn(m[1], p[1]);
-    m[2] = __dadd_rn(m[2], p[2]);
-    c[0] = __dadd_rn(c[0], cv[0 * ld + 0]);
-    c[1] = __dadd_rn(c[1], cv[0 * ld + 1]);
-    c[2] = __dadd_rn(c[2], cv[0 * ld + 2]);
-    c[3] = __dadd_rn(c[3], cv[1 * ld + 1]);
-    c[4] = __dadd_rn(c[4], cv[1 * ld + 2]);
-    c[5] = __dadd_rn(c[5], cv[2 * ld + 2]);
-  }
-  const double cnt = cnt0 + static_cast<double>(end - begin);
-#pragma unroll
-  for (int k = 0; k < 3; k++) rec[k] = __ddiv_rn(m[k], cnt);
-#pragma unroll
-  for (int k = 0; k < 6; k++) rec[3 + k] = __ddiv_rn(c[k], cnt);
-  rec[9] = cnt;
+  cell.add(CellPoints{pts, covs, pstride, cstride, idx, begin, end}, e >= 0, records, counts, dest);
   if (e < 0) {
 #pragma unroll
     for (int k = 0; k < 3; k++) coords[dest * 3 + k] = batch_coords[r * 3 + k];
   }
-  lru[dest] = lru_counter;  // incremental_voxelmap_impl.hpp:49
+  lru[dest] = lru_counter;  // incremental_voxelmap_impl.hpp:45,49
 }
 
 // LRU eviction (incremental_voxelmap_impl.hpp:55-66): voxels untouched for more than `horizon` inserts are removed, the
@@ -151,62 +194,18 @@ __global__ void lru_keep_flags_kernel(const uint32_t* __restrict__ lru, size_t V
   const size_t r = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
   if (r < V) keep[r] = (static_cast<unsigned long long>(lru[r]) + horizon < counter) ? 0u : 1u;
 }
-// rec_doubles: payload doubles per voxel (kRecordDoubles, or stride point records of an iVox); counts: iVox point counts or nullptr
-__global__ void lru_compact_kernel(const uint32_t* __restrict__ keep, const uint32_t* __restrict__ pos, size_t V, size_t rec_doubles, const double* __restrict__ rec_in,
+// payload: voxel_payload_doubles(slots); counts: the point counts of a map with slots, or nullptr
+__global__ void lru_compact_kernel(const uint32_t* __restrict__ keep, const uint32_t* __restrict__ pos, size_t V, size_t payload, const double* __restrict__ rec_in,
                                    const int32_t* __restrict__ coords_in, const uint32_t* __restrict__ lru_in, const uint32_t* __restrict__ counts_in, double* __restrict__ rec_out,
                                    int32_t* __restrict__ coords_out, uint32_t* __restrict__ lru_out, uint32_t* __restrict__ counts_out) {
   const size_t r = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
   if (r >= V || !keep[r]) return;
   const size_t d = pos[r];
-  for (size_t k = 0; k < rec_doubles; k++) rec_out[d * rec_doubles + k] = rec_in[r * rec_doubles + k];
+  for (size_t k = 0; k < payload; k++) rec_out[d * payload + k] = rec_in[r * payload + k];
 #pragma unroll
   for (int k = 0; k < 3; k++) coords_out[d * 3 + k] = coords_in[r * 3 + k];
   lru_out[d] = lru_in[r];
   if (counts_in) counts_out[d] = counts_in[r];
-}
-
-// iVox insert (IncrementalVoxelMap<FlatContainer>::insert, incremental_voxelmap_impl.hpp:31-50): one thread per voxel of the batch
-// walks its points in insertion order through FlatContainer::add (flat_container.hpp:33-50) -- rejected if the voxel already holds
-// max_points points or a stored point lies closer than min_sq -- and appends the rest to the voxel's slots as records
-// (point | covariance upper | 1).  The voxel's lru is set whether or not any point was taken.
-__global__ void ivox_add_kernel(const double* __restrict__ pts, int pstride, const double* __restrict__ covs, int cstride, size_t n, size_t num_batch,
-                                const uint32_t* __restrict__ idx, const uint32_t* __restrict__ seg_start, const uint32_t* __restrict__ seg_of_rank,
-                                const int32_t* __restrict__ batch_coords, const int32_t* __restrict__ existing_id, const uint32_t* __restrict__ new_rank, size_t num_existing,
-                                uint32_t lru_counter, int stride, int max_points, double min_sq, double* __restrict__ records, uint32_t* __restrict__ counts,
-                                int32_t* __restrict__ coords, uint32_t* __restrict__ lru) {
-  const size_t r = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
-  if (r >= num_batch) return;
-  const uint32_t s = seg_of_rank[r];
-  const size_t begin = seg_start[s];
-  const size_t end = (s + 1 < num_batch) ? seg_start[s + 1] : n;
-  const int ld = cstride == 16 ? 4 : 3;
-  const int e = existing_id[r];
-  const size_t dest = e >= 0 ? static_cast<size_t>(e) : num_existing + new_rank[r];
-  double* rec = records + dest * static_cast<size_t>(stride) * kRecordDoubles;
-  int cnt = e >= 0 ? static_cast<int>(counts[dest]) : 0;
-  for (size_t j = begin; j < end && cnt < max_points; j++) {
-    const size_t i = idx[j];
-    const double* p = pts + i * pstride;
-    bool reject = false;
-    for (int q = 0; q < cnt && !reject; q++) reject = ivox_sq_dist(rec[q * kRecordDoubles + 0], rec[q * kRecordDoubles + 1], rec[q * kRecordDoubles + 2], p[0], p[1], p[2]) < min_sq;
-    if (reject) continue;
-    double* o = rec + static_cast<size_t>(cnt) * kRecordDoubles;
-    o[0] = p[0], o[1] = p[1], o[2] = p[2];
-    if (covs) {
-      const double* cv = covs + i * cstride;
-      o[3] = cv[0 * ld + 0], o[4] = cv[0 * ld + 1], o[5] = cv[0 * ld + 2], o[6] = cv[1 * ld + 1], o[7] = cv[1 * ld + 2], o[8] = cv[2 * ld + 2];
-    } else {
-      o[3] = o[4] = o[5] = o[6] = o[7] = o[8] = 0.0;
-    }
-    o[9] = 1.0;
-    cnt++;
-  }
-  counts[dest] = static_cast<uint32_t>(cnt);
-  if (e < 0) {
-#pragma unroll
-    for (int k = 0; k < 3; k++) coords[dest * 3 + k] = batch_coords[r * 3 + k];
-  }
-  lru[dest] = lru_counter;  // incremental_voxelmap_impl.hpp:45: also when every point was rejected
 }
 
 // IncrementalVoxelMap::knn_search (incremental_voxelmap_impl.hpp:71-92) with KnnResult<-1> (knn_result.hpp:84-109): one thread per
@@ -419,46 +418,59 @@ struct MinU64 {
 // load factor <= 0.25 (see b2_device.cuh: one-round-trip lookups)
 size_t bucket_count_for(size_t num_voxels) { return static_cast<size_t>(next_pow2(std::max<uint64_t>(64, 4 * static_cast<uint64_t>(num_voxels)))); }
 
-// An empty Gaussian voxel map laid out for V voxels: a bucket table for V (contents left to the caller) and per-voxel arrays
-// for max(V, 1) voxels, LRU zeroed
+// The per-voxel arrays of a voxel map: payload records, coordinates, LRU stamps and, iff slots > 0, point counts.
+struct VoxelArrays {
+  DeviceBuffer records, coords, lru, counts;
+};
+
+// Gives the map new per-voxel arrays for `cap` voxels in the layout `slots`.  `fill` runs on them once all are allocated, while the
+// map still holds its current arrays (growth copies from them, the LRU sweep compacts them); the map takes the new arrays only after
+// every allocation and `fill` have succeeded.
+template <typename Fill>
+b2_status set_voxel_arrays(b2_voxelmap* vm, size_t cap, int slots, Fill&& fill) {
+  VoxelArrays a;
+  B2_TRY(a.records.alloc(cap * voxel_payload_doubles(slots) * sizeof(double)));
+  B2_TRY(a.coords.alloc(cap * 3 * sizeof(int32_t)));
+  B2_TRY(a.lru.alloc(cap * sizeof(uint32_t)));
+  if (slots > 0) B2_TRY(a.counts.alloc(cap * sizeof(uint32_t)));
+  B2_TRY(fill(a));
+  vm->d_records = std::move(a.records), vm->d_coords = std::move(a.coords), vm->d_lru = std::move(a.lru), vm->d_counts = std::move(a.counts);
+  vm->capacity = cap;
+  vm->slots = slots;
+  return B2_OK;
+}
+
+// An empty map sized for V voxels, the one constructor of every voxel map and iVox: an empty bucket table for V voxels and
+// Gaussian-layout per-voxel arrays for max(V, 1) voxels, LRU zeroed.  The caller synchronizes.
 b2_status init_map(b2_voxelmap& vm, b2_ctx* ctx, double resolution, size_t V) {
   vm.ctx = ctx;
   vm.resolution = resolution;
   vm.inv_resolution = 1.0 / resolution;  // ann/impl/incremental_voxelmap_impl.hpp:14
-  vm.num_voxels = V;
   vm.num_buckets = bucket_count_for(V);
-  vm.capacity = std::max<size_t>(V, 1);
   B2_TRY(vm.d_buckets.alloc(vm.num_buckets * sizeof(VoxelBucket)));
-  B2_TRY(vm.d_records.alloc(vm.capacity * kRecordDoubles * sizeof(double)));
-  B2_TRY(vm.d_coords.alloc(vm.capacity * 3 * sizeof(int32_t)));
-  B2_TRY(vm.d_lru.alloc(vm.capacity * sizeof(uint32_t)));
-  B2_CUDA(cudaMemsetAsync(vm.d_lru.get(), 0, vm.capacity * sizeof(uint32_t), ctx->stream));
-  return B2_OK;
+  B2_CUDA(cudaMemsetAsync(vm.d_buckets.get(), 0xFF, vm.num_buckets * sizeof(VoxelBucket), ctx->stream));
+  const size_t cap = std::max<size_t>(V, 1);
+  return set_voxel_arrays(&vm, cap, 0, [&](VoxelArrays& a) -> b2_status {
+    B2_CUDA(cudaMemsetAsync(a.lru.get(), 0, cap * sizeof(uint32_t), ctx->stream));
+    return B2_OK;
+  });
 }
 
 // grow the per-voxel arrays to hold `want` voxels (contents up to num_voxels are kept)
 b2_status reserve_voxels(b2_voxelmap* vm, size_t want) {
   if (want <= vm->capacity) return B2_OK;
-  const size_t cap = std::max(want, vm->capacity * 2);
-  const size_t rd = vm->rec_doubles;
   cudaStream_t st = vm->ctx->stream;
-  DeviceBuffer rec, coords, lru, counts;
-  B2_TRY(rec.alloc(cap * rd * sizeof(double)));
-  B2_TRY(coords.alloc(cap * 3 * sizeof(int32_t)));
-  B2_TRY(lru.alloc(cap * sizeof(uint32_t)));
-  if (vm->d_counts) B2_TRY(counts.alloc(cap * sizeof(uint32_t)));
-  const size_t V = vm->num_voxels;
-  if (V) {
-    B2_CUDA(cudaMemcpyAsync(rec.get(), vm->d_records.get(), V * rd * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    B2_CUDA(cudaMemcpyAsync(coords.get(), vm->d_coords.get(), V * 3 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
-    B2_CUDA(cudaMemcpyAsync(lru.get(), vm->d_lru.get(), V * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
-    if (counts) B2_CUDA(cudaMemcpyAsync(counts.get(), vm->d_counts.get(), V * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
-  }
-  B2_CUDA(cudaStreamSynchronize(st));
-  vm->d_records = std::move(rec), vm->d_coords = std::move(coords), vm->d_lru = std::move(lru);
-  if (counts) vm->d_counts = std::move(counts);
-  vm->capacity = cap;
-  return B2_OK;
+  const size_t V = vm->num_voxels, payload = voxel_payload_doubles(vm->slots);
+  return set_voxel_arrays(vm, std::max(want, vm->capacity * 2), vm->slots, [&](VoxelArrays& a) -> b2_status {
+    if (V) {
+      B2_CUDA(cudaMemcpyAsync(a.records.get(), vm->d_records.get(), V * payload * sizeof(double), cudaMemcpyDeviceToDevice, st));
+      B2_CUDA(cudaMemcpyAsync(a.coords.get(), vm->d_coords.get(), V * 3 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+      B2_CUDA(cudaMemcpyAsync(a.lru.get(), vm->d_lru.get(), V * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
+      if (a.counts) B2_CUDA(cudaMemcpyAsync(a.counts.get(), vm->d_counts.get(), V * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
+    }
+    B2_CUDA(cudaStreamSynchronize(st));
+    return B2_OK;
+  });
 }
 
 // (re)build the bucket table over the current voxels; resized when the load factor bound asks for it
@@ -468,14 +480,14 @@ b2_status rebuild_table(b2_voxelmap* vm) {
   if (nb != vm->num_buckets) {
     DeviceBuffer fresh;
     B2_TRY(fresh.alloc(nb * sizeof(VoxelBucket)));
-    cudaStreamSynchronize(st);
+    B2_CUDA(cudaStreamSynchronize(st));
     vm->d_buckets = std::move(fresh);
     vm->num_buckets = nb;
   }
   B2_CUDA(cudaMemsetAsync(vm->d_buckets.get(), 0xFF, vm->num_buckets * sizeof(VoxelBucket), st));
   if (vm->num_voxels) {
     insert_buckets_kernel<<<static_cast<unsigned>((vm->num_voxels + 127) / 128), 128, 0, st>>>(vm->d_coords.as<int32_t>(), vm->num_voxels, vm->d_buckets.as<VoxelBucket>(),
-                                                                                               static_cast<uint32_t>(vm->num_buckets / kGroup - 1));
+                                                                                               vm->group_mask());
     B2_CUDA(cudaGetLastError());
   }
   vm->generation++;
@@ -501,74 +513,70 @@ b2_status segment_batch(b2_voxelmap* vm, const double* points, int point_stride,
   cudaStream_t st = vm->ctx->stream;
   const double inv_leaf = vm->inv_resolution;
   const size_t V_old = vm->num_voxels;
-  DeviceBuffer &raw_p = s.raw_p, &raw_c = s.raw_c, &key_z = s.key_z, &key_z2 = s.key_z2, &idx_a = s.idx_a, &idx_b = s.idx_b, &key_xy = s.key_xy, &key_xy2 = s.key_xy2,
-               &flags = s.flags, &seg_incl = s.seg_incl, &tmp = s.tmp;
-  DeviceBuffer &seg_start = s.seg_start, &seg_first = s.seg_first, &seg_first2 = s.seg_first2, &seg_iota = s.seg_iota, &seg_of_rank = s.seg_of_rank, &tmp2 = s.tmp2,
-               &batch_coords = s.batch_coords, &existing_id = s.existing_id, &is_new = s.is_new, &new_rank = s.new_rank;
-  B2_TRY(raw_p.alloc(n * point_stride * sizeof(double)));
-  if (covs) B2_TRY(raw_c.alloc(n * cov_stride * sizeof(double)));
-  B2_CUDA(cudaMemcpyAsync(raw_p.get(), points, n * point_stride * sizeof(double), cudaMemcpyHostToDevice, st));
-  if (covs) B2_CUDA(cudaMemcpyAsync(raw_c.get(), covs, n * cov_stride * sizeof(double), cudaMemcpyHostToDevice, st));
-  B2_TRY(key_z.alloc(n * 4));
-  B2_TRY(key_z2.alloc(n * 4));
-  B2_TRY(idx_a.alloc(n * 4));
-  B2_TRY(idx_b.alloc(n * 4));
-  B2_TRY(key_xy.alloc(n * 8));
-  B2_TRY(key_xy2.alloc(n * 8));
-  B2_TRY(flags.alloc(n * 4));
-  B2_TRY(seg_incl.alloc(n * 4));
+  B2_TRY(s.raw_p.alloc(n * point_stride * sizeof(double)));
+  if (covs) B2_TRY(s.raw_c.alloc(n * cov_stride * sizeof(double)));
+  B2_CUDA(cudaMemcpyAsync(s.raw_p.get(), points, n * point_stride * sizeof(double), cudaMemcpyHostToDevice, st));
+  if (covs) B2_CUDA(cudaMemcpyAsync(s.raw_c.get(), covs, n * cov_stride * sizeof(double), cudaMemcpyHostToDevice, st));
+  B2_TRY(s.key_z.alloc(n * 4));
+  B2_TRY(s.key_z2.alloc(n * 4));
+  B2_TRY(s.idx_a.alloc(n * 4));
+  B2_TRY(s.idx_b.alloc(n * 4));
+  B2_TRY(s.key_xy.alloc(n * 8));
+  B2_TRY(s.key_xy2.alloc(n * 8));
+  B2_TRY(s.flags.alloc(n * 4));
+  B2_TRY(s.seg_incl.alloc(n * 4));
 
   const unsigned grid = static_cast<unsigned>((n + 255) / 256);
-  const double* rp = raw_p.as<double>();
+  const double* rp = s.raw_p.as<double>();
   const int ni = static_cast<int>(n);
 
   // pass 1: stable sort by z; pass 2: stable sort by (x, y)  => lexicographic (x, y, z), insertion order inside a voxel
   auto sort_z = [&](void* t, size_t& b) {
-    return cub::DeviceRadixSort::SortPairs(t, b, key_z.as<uint32_t>(), key_z2.as<uint32_t>(), idx_a.as<uint32_t>(), idx_b.as<uint32_t>(), ni, 0, 32, st);
+    return cub::DeviceRadixSort::SortPairs(t, b, s.key_z.as<uint32_t>(), s.key_z2.as<uint32_t>(), s.idx_a.as<uint32_t>(), s.idx_b.as<uint32_t>(), ni, 0, 32, st);
   };
   auto sort_xy = [&](void* t, size_t& b) {
-    return cub::DeviceRadixSort::SortPairs(t, b, key_xy.as<unsigned long long>(), key_xy2.as<unsigned long long>(), idx_b.as<uint32_t>(), idx_a.as<uint32_t>(), ni, 0, 64, st);
+    return cub::DeviceRadixSort::SortPairs(t, b, s.key_xy.as<unsigned long long>(), s.key_xy2.as<unsigned long long>(), s.idx_b.as<uint32_t>(), s.idx_a.as<uint32_t>(), ni, 0, 64, st);
   };
-  auto scan_heads = [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, flags.as<uint32_t>(), seg_incl.as<uint32_t>(), ni, st); };
-  B2_TRY(cub_reserve(tmp, st, sort_z, sort_xy, scan_heads));
+  auto scan_heads = [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, s.flags.as<uint32_t>(), s.seg_incl.as<uint32_t>(), ni, st); };
+  B2_TRY(cub_reserve(s.tmp, st, sort_z, sort_xy, scan_heads));
 
-  point_coord_keys_kernel<<<grid, 256, 0, st>>>(rp, point_stride, n, inv_leaf, key_z.as<uint32_t>(), idx_a.as<uint32_t>());
-  B2_TRY(cub_launch(tmp, sort_z));
-  gather_xy_keys_kernel<<<grid, 256, 0, st>>>(rp, point_stride, n, inv_leaf, idx_b.as<uint32_t>(), key_xy.as<unsigned long long>());
-  B2_TRY(cub_launch(tmp, sort_xy));
-  const uint32_t* idx = idx_a.as<uint32_t>();
+  point_coord_keys_kernel<<<grid, 256, 0, st>>>(rp, point_stride, n, inv_leaf, s.key_z.as<uint32_t>(), s.idx_a.as<uint32_t>());
+  B2_TRY(cub_launch(s.tmp, sort_z));
+  gather_xy_keys_kernel<<<grid, 256, 0, st>>>(rp, point_stride, n, inv_leaf, s.idx_b.as<uint32_t>(), s.key_xy.as<unsigned long long>());
+  B2_TRY(cub_launch(s.tmp, sort_xy));
+  const uint32_t* idx = s.idx_a.as<uint32_t>();
 
-  head_flags_kernel<<<grid, 256, 0, st>>>(rp, point_stride, n, inv_leaf, idx, flags.as<uint32_t>());
-  B2_TRY(cub_launch(tmp, scan_heads));
+  head_flags_kernel<<<grid, 256, 0, st>>>(rp, point_stride, n, inv_leaf, idx, s.flags.as<uint32_t>());
+  B2_TRY(cub_launch(s.tmp, scan_heads));
   uint32_t B32 = 0;
-  B2_CUDA(cudaMemcpyAsync(&B32, seg_incl.as<uint32_t>() + (n - 1), 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(&B32, s.seg_incl.as<uint32_t>() + (n - 1), 4, cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
   const size_t B = B32;  // voxels touched by this batch
 
-  B2_TRY(seg_start.alloc(B * 4));
-  B2_TRY(seg_first.alloc(B * 4));
-  B2_TRY(seg_first2.alloc(B * 4));
-  B2_TRY(seg_iota.alloc(B * 4));
-  B2_TRY(seg_of_rank.alloc(B * 4));
-  B2_TRY(batch_coords.alloc(B * 12));
-  B2_TRY(existing_id.alloc(B * 4));
-  B2_TRY(is_new.alloc(B * 4));
-  B2_TRY(new_rank.alloc(B * 4));
-  segment_heads_kernel<<<grid, 256, 0, st>>>(n, flags.as<uint32_t>(), seg_incl.as<uint32_t>(), idx, seg_start.as<uint32_t>(), seg_first.as<uint32_t>(), seg_iota.as<uint32_t>());
+  B2_TRY(s.seg_start.alloc(B * 4));
+  B2_TRY(s.seg_first.alloc(B * 4));
+  B2_TRY(s.seg_first2.alloc(B * 4));
+  B2_TRY(s.seg_iota.alloc(B * 4));
+  B2_TRY(s.seg_of_rank.alloc(B * 4));
+  B2_TRY(s.batch_coords.alloc(B * 12));
+  B2_TRY(s.existing_id.alloc(B * 4));
+  B2_TRY(s.is_new.alloc(B * 4));
+  B2_TRY(s.new_rank.alloc(B * 4));
+  segment_heads_kernel<<<grid, 256, 0, st>>>(n, s.flags.as<uint32_t>(), s.seg_incl.as<uint32_t>(), idx, s.seg_start.as<uint32_t>(), s.seg_first.as<uint32_t>(), s.seg_iota.as<uint32_t>());
   auto sort_first_touch = [&](void* t, size_t& b) {
-    return cub::DeviceRadixSort::SortPairs(t, b, seg_first.as<uint32_t>(), seg_first2.as<uint32_t>(), seg_iota.as<uint32_t>(), seg_of_rank.as<uint32_t>(), static_cast<int>(B), 0, 32, st);
+    return cub::DeviceRadixSort::SortPairs(t, b, s.seg_first.as<uint32_t>(), s.seg_first2.as<uint32_t>(), s.seg_iota.as<uint32_t>(), s.seg_of_rank.as<uint32_t>(), static_cast<int>(B), 0, 32, st);
   };
-  auto rank_new = [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, is_new.as<uint32_t>(), new_rank.as<uint32_t>(), static_cast<int>(B), st); };
-  B2_TRY(cub_reserve(tmp2, st, sort_first_touch, rank_new));
-  B2_TRY(cub_launch(tmp2, sort_first_touch));
+  auto rank_new = [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, s.is_new.as<uint32_t>(), s.new_rank.as<uint32_t>(), static_cast<int>(B), st); };
+  B2_TRY(cub_reserve(s.tmp2, st, sort_first_touch, rank_new));
+  B2_TRY(cub_launch(s.tmp2, sort_first_touch));
 
   const unsigned vgrid = static_cast<unsigned>((B + 127) / 128);
-  batch_voxels_kernel<<<vgrid, 128, 0, st>>>(rp, point_stride, B, inv_leaf, idx, seg_start.as<uint32_t>(), seg_of_rank.as<uint32_t>(), vm->d_buckets.as<VoxelBucket>(),
-                                             static_cast<uint32_t>(vm->num_buckets / kGroup - 1), V_old, batch_coords.as<int32_t>(), existing_id.as<int32_t>(), is_new.as<uint32_t>());
-  B2_TRY(cub_launch(tmp2, rank_new));
+  batch_voxels_kernel<<<vgrid, 128, 0, st>>>(rp, point_stride, B, inv_leaf, idx, s.seg_start.as<uint32_t>(), s.seg_of_rank.as<uint32_t>(), vm->d_buckets.as<VoxelBucket>(),
+                                             vm->group_mask(), V_old, s.batch_coords.as<int32_t>(), s.existing_id.as<int32_t>(), s.is_new.as<uint32_t>());
+  B2_TRY(cub_launch(s.tmp2, rank_new));
   uint32_t last_rank = 0, last_new = 0;
-  B2_CUDA(cudaMemcpyAsync(&last_rank, new_rank.as<uint32_t>() + (B - 1), 4, cudaMemcpyDeviceToHost, st));
-  B2_CUDA(cudaMemcpyAsync(&last_new, is_new.as<uint32_t>() + (B - 1), 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(&last_rank, s.new_rank.as<uint32_t>() + (B - 1), 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(&last_new, s.is_new.as<uint32_t>() + (B - 1), 4, cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
   s.B = B;
   s.num_new = static_cast<size_t>(last_rank) + last_new;
@@ -582,7 +590,7 @@ b2_status lru_sweep_and_rebuild(b2_voxelmap* vm) {
   vm->lru_counter++;
   if (vm->lru_counter % vm->lru_clear_cycle == 0 && vm->num_voxels > 0) {
     const size_t V = vm->num_voxels;
-    DeviceBuffer keep, pos, tmp3, rec2, coords2, lru2, counts2;
+    DeviceBuffer keep, pos, tmp3;
     B2_TRY(keep.alloc(V * 4));
     B2_TRY(pos.alloc(V * 4));
     const unsigned g = static_cast<unsigned>((V + 255) / 256);
@@ -594,23 +602,56 @@ b2_status lru_sweep_and_rebuild(b2_voxelmap* vm) {
     B2_CUDA(cudaStreamSynchronize(st));
     const size_t kept = static_cast<size_t>(last_pos) + last_keep;
     if (kept != V) {
-      const size_t cap = vm->capacity;
-      B2_TRY(rec2.alloc(cap * vm->rec_doubles * sizeof(double)));
-      B2_TRY(coords2.alloc(cap * 3 * sizeof(int32_t)));
-      B2_TRY(lru2.alloc(cap * sizeof(uint32_t)));
-      if (vm->d_counts) B2_TRY(counts2.alloc(cap * sizeof(uint32_t)));
-      lru_compact_kernel<<<g, 256, 0, st>>>(keep.as<uint32_t>(), pos.as<uint32_t>(), V, vm->rec_doubles, vm->d_records.as<double>(), vm->d_coords.as<int32_t>(), vm->d_lru.as<uint32_t>(),
-                                            vm->d_counts.as<uint32_t>(), rec2.as<double>(), coords2.as<int32_t>(), lru2.as<uint32_t>(), counts2.as<uint32_t>());
-      B2_CUDA(cudaGetLastError());
-      B2_CUDA(cudaStreamSynchronize(st));
-      vm->d_records = std::move(rec2), vm->d_coords = std::move(coords2), vm->d_lru = std::move(lru2);
-      if (counts2) vm->d_counts = std::move(counts2);
+      B2_TRY(set_voxel_arrays(vm, vm->capacity, vm->slots, [&](VoxelArrays& a) -> b2_status {
+        lru_compact_kernel<<<g, 256, 0, st>>>(keep.as<uint32_t>(), pos.as<uint32_t>(), V, voxel_payload_doubles(vm->slots), vm->d_records.as<double>(), vm->d_coords.as<int32_t>(),
+                                              vm->d_lru.as<uint32_t>(), vm->d_counts.as<uint32_t>(), a.records.as<double>(), a.coords.as<int32_t>(), a.lru.as<uint32_t>(),
+                                              a.counts.as<uint32_t>());
+        B2_CUDA(cudaGetLastError());
+        B2_CUDA(cudaStreamSynchronize(st));
+        return B2_OK;
+      }));
       vm->num_voxels = kept;
     }
   }
   B2_TRY(rebuild_table(vm));
   B2_CUDA(cudaStreamSynchronize(st));
   return B2_OK;
+}
+
+// IncrementalVoxelMap::insert (incremental_voxelmap_impl.hpp:31-68) for both maps: the batch is segmented into voxels by two stable
+// radix sorts (points of a voxel stay in insertion order, voxels are ranked by first touch), voxels that already exist are found
+// through the table and continued, new ones get the next ids in first-touch order; `cell` is the per-voxel step; then the LRU sweep
+// and the table rebuild.  `slots` is the map's layout, or the one an iVox's first insert gives it.  Every check that can fail runs
+// before the map changes; `on_change` runs when it does.
+template <typename Cell, typename OnChange>
+b2_status insert_batch(b2_voxelmap* vm, int slots, const Cell& cell, OnChange&& on_change, const double* points, int point_stride, const double* covs, int cov_stride,
+                       size_t n) {
+  B2_CUDA(cudaSetDevice(vm->ctx->device));
+  cudaStream_t st = vm->ctx->stream;
+  if (n > 0) {
+    const size_t V_old = vm->num_voxels;
+    BatchSegments sg;
+    B2_TRY(segment_batch(vm, points, point_stride, covs, cov_stride, n, sg));
+    const size_t V_new = V_old + sg.num_new;
+    if (slots == 0)
+      B2_REQUIRE(V_new < (1ull << 30), "b2_voxelmap_insert: too many voxels");
+    else  // the factor kernel's ring carries voxel * slots + slot as a 32-bit id
+      B2_REQUIRE(V_new * static_cast<size_t>(slots) < (1ull << 31), "b2_ivox_insert: %zu voxels x %d slots exceed 2^31 point records", V_new, slots);
+    if (slots != vm->slots)  // an iVox's first insert: nothing is stored yet, so the slot layout copies nothing
+      B2_TRY(set_voxel_arrays(vm, std::max<size_t>(V_new, 1), slots, [](VoxelArrays&) { return B2_OK; }));
+    else
+      B2_TRY(reserve_voxels(vm, V_new));
+    on_change();
+    insert_voxels_kernel<<<static_cast<unsigned>((sg.B + 127) / 128), 128, 0, st>>>(cell, sg.raw_p.as<double>(), point_stride, sg.raw_c.as<double>(), cov_stride, n, sg.B, sg.idx(),
+                                                                                     sg.seg_start.as<uint32_t>(), sg.seg_of_rank.as<uint32_t>(), sg.batch_coords.as<int32_t>(),
+                                                                                     sg.existing_id.as<int32_t>(), sg.new_rank.as<uint32_t>(), V_old, static_cast<uint32_t>(vm->lru_counter),
+                                                                                     vm->d_records.as<double>(), vm->d_counts.as<uint32_t>(), vm->d_coords.as<int32_t>(),
+                                                                                     vm->d_lru.as<uint32_t>());
+    B2_CUDA(cudaGetLastError());
+    vm->num_voxels = V_new;
+    B2_CUDA(cudaStreamSynchronize(st));  // the scratch buffers above are released at scope exit
+  }
+  return lru_sweep_and_rebuild(vm);
 }
 
 }  // namespace
@@ -629,12 +670,13 @@ b2_status b2_voxelmap_create_from_voxels(b2_ctx* ctx, double resolution, const i
   B2_REQUIRE(V == 0 || (coords && means && covs), "b2_voxelmap_create_from_voxels: NULL voxel arrays");
   B2_REQUIRE(V < (1ull << 30), "b2_voxelmap_create_from_voxels: too many voxels");
   B2_CUDA(cudaSetDevice(ctx->device));
+  auto vm = std::make_unique<b2_voxelmap>();
+  B2_TRY(init_map(*vm, ctx, resolution, V));
 
   // host-side table build in id order (deterministic placement), duplicate coordinates rejected
-  const size_t nb = bucket_count_for(V);
-  const uint32_t gmask = static_cast<uint32_t>(nb / kGroup - 1);
-  std::vector<VoxelBucket> buckets(nb, VoxelBucket{-1, -1, -1, -1});
-  std::vector<double> records(std::max<size_t>(V, 1) * kRecordDoubles, 0.0);
+  const uint32_t gmask = vm->group_mask();
+  std::vector<VoxelBucket> buckets(vm->num_buckets, VoxelBucket{-1, -1, -1, -1});
+  std::vector<double> records(V * kRecordDoubles);
   for (size_t r = 0; r < V; r++) {
     const int x = coords[r * 3], y = coords[r * 3 + 1], z = coords[r * 3 + 2];
     uint32_t g = voxel_hash(x, y, z) & gmask;
@@ -653,22 +695,17 @@ b2_status b2_voxelmap_create_from_voxels(b2_ctx* ctx, double resolution, const i
     }
     double* rec = &records[r * kRecordDoubles];
     for (int k = 0; k < 3; k++) rec[k] = means[r * 3 + k];
-    const double* c = covs + r * 9;
-    rec[3] = c[0];
-    rec[4] = c[1];
-    rec[5] = c[2];
-    rec[6] = c[4];
-    rec[7] = c[5];
-    rec[8] = c[8];
+    cov_upper(covs + r * 9, 9, rec + 3);
     rec[9] = num_points ? static_cast<double>(num_points[r]) : 1.0;
   }
 
-  auto vm = std::make_unique<b2_voxelmap>();
-  B2_TRY(init_map(*vm, ctx, resolution, V));
   cudaStream_t st = ctx->stream;
-  B2_CUDA(cudaMemcpyAsync(vm->d_buckets.get(), buckets.data(), nb * sizeof(VoxelBucket), cudaMemcpyHostToDevice, st));
-  B2_CUDA(cudaMemcpyAsync(vm->d_records.get(), records.data(), records.size() * sizeof(double), cudaMemcpyHostToDevice, st));
-  if (V > 0) B2_CUDA(cudaMemcpyAsync(vm->d_coords.get(), coords, V * 3 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  if (V > 0) {
+    B2_CUDA(cudaMemcpyAsync(vm->d_buckets.get(), buckets.data(), buckets.size() * sizeof(VoxelBucket), cudaMemcpyHostToDevice, st));
+    B2_CUDA(cudaMemcpyAsync(vm->d_records.get(), records.data(), records.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+    B2_CUDA(cudaMemcpyAsync(vm->d_coords.get(), coords, V * 3 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  }
+  vm->num_voxels = V;
   B2_CUDA(cudaStreamSynchronize(st));
   *out = vm.release();
   return B2_OK;
@@ -679,7 +716,12 @@ b2_status b2_voxelmap_create(b2_ctx* ctx, double resolution, b2_voxelmap** out) 
   *out = nullptr;
   B2_REQUIRE(ctx != nullptr, "b2_voxelmap_create: ctx is NULL");
   B2_REQUIRE(resolution > 0.0, "b2_voxelmap_create: resolution must be positive");
-  return b2_voxelmap_create_from_voxels(ctx, resolution, nullptr, nullptr, nullptr, nullptr, 0, out);
+  B2_CUDA(cudaSetDevice(ctx->device));
+  auto vm = std::make_unique<b2_voxelmap>();
+  B2_TRY(init_map(*vm, ctx, resolution, 0));
+  B2_CUDA(cudaStreamSynchronize(ctx->stream));
+  *out = vm.release();
+  return B2_OK;
 }
 
 b2_status b2_voxelmap_set_lru(b2_voxelmap* vm, size_t lru_horizon, size_t lru_clear_cycle) {
@@ -690,36 +732,15 @@ b2_status b2_voxelmap_set_lru(b2_voxelmap* vm, size_t lru_horizon, size_t lru_cl
   return B2_OK;
 }
 
-// IncrementalVoxelMap<GaussianVoxel>::insert (ann/impl/incremental_voxelmap_impl.hpp:31-68) on the device: the batch is
-// segmented into voxels by two stable radix sorts (points of a voxel stay in insertion order, voxels are ranked by first
-// touch), voxels that already exist are found through the table and continued, new ones get the next ids in first-touch
-// order, then the LRU sweep and the table rebuild.  Deterministic; ids, counts, means and covariances equal the CPU map's.
+// IncrementalVoxelMap<GaussianVoxel>::insert on the device (insert_batch).  Deterministic; ids, counts, means and covariances equal
+// the CPU map's.
 b2_status b2_voxelmap_insert(b2_voxelmap* vm, const double* points, int point_stride, const double* covs, int cov_stride, size_t n) {
   B2_REQUIRE(vm != nullptr, "b2_voxelmap_insert: vm is NULL");
   B2_REQUIRE(point_stride == 3 || point_stride == 4, "b2_voxelmap_insert: point_stride must be 3 or 4");
   B2_REQUIRE(cov_stride == 9 || cov_stride == 16, "b2_voxelmap_insert: cov_stride must be 9 or 16");
   B2_REQUIRE(n == 0 || (points && covs), "error: points/covs have not been allocated!!");  // GaussianVoxel::add reads covs
   B2_REQUIRE(n < (1ull << 31), "b2_voxelmap_insert: at most 2^31-1 points per insert");
-  b2_ctx* ctx = vm->ctx;
-  B2_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
-  const size_t V_old = vm->num_voxels;
-
-  if (n > 0) {
-    BatchSegments sg;
-    B2_TRY(segment_batch(vm, points, point_stride, covs, cov_stride, n, sg));
-    const size_t B = sg.B, num_new = sg.num_new;
-    B2_REQUIRE(V_old + num_new < (1ull << 30), "b2_voxelmap_insert: too many voxels");
-    B2_TRY(reserve_voxels(vm, V_old + num_new));
-    const unsigned vgrid = static_cast<unsigned>((B + 127) / 128);
-    accumulate_voxels_kernel<<<vgrid, 128, 0, st>>>(sg.raw_p.as<double>(), point_stride, sg.raw_c.as<double>(), cov_stride, n, B, sg.idx(), sg.seg_start.as<uint32_t>(), sg.seg_of_rank.as<uint32_t>(),
-                                                    sg.batch_coords.as<int32_t>(), sg.existing_id.as<int32_t>(), sg.new_rank.as<uint32_t>(), V_old, static_cast<uint32_t>(vm->lru_counter),
-                                                    vm->d_records.as<double>(), vm->d_coords.as<int32_t>(), vm->d_lru.as<uint32_t>());
-    B2_CUDA(cudaGetLastError());
-    vm->num_voxels = V_old + num_new;
-    B2_CUDA(cudaStreamSynchronize(st));  // the scratch buffers above are released at scope exit
-  }
-  return lru_sweep_and_rebuild(vm);
+  return insert_batch(vm, 0, GaussianCell{}, [] {}, points, point_stride, covs, cov_stride, n);
 }
 
 b2_status b2_voxelmap_create_from_points(b2_ctx* ctx, double resolution, const double* points, int point_stride, const double* covs, int cov_stride,
@@ -770,15 +791,7 @@ b2_status b2_voxelmap_download(const b2_voxelmap* vm, int32_t* coords, double* m
     const double* q = &rec[r * kRecordDoubles];
     if (means)
       for (int k = 0; k < 3; k++) means[r * 3 + k] = q[k];
-    if (covs) {
-      double* c = covs + r * 9;
-      c[0] = q[3];
-      c[1] = c[3] = q[4];
-      c[2] = c[6] = q[5];
-      c[4] = q[6];
-      c[5] = c[7] = q[7];
-      c[8] = q[8];
-    }
+    if (covs) cov_full(q + 3, covs + r * 9);
     if (num_points) num_points[r] = static_cast<int32_t>(q[9]);
   }
   return B2_OK;
@@ -807,9 +820,7 @@ b2_status b2_voxelmap_save_compact(const b2_voxelmap* vm, const char* path) {
     GaussianVoxelData& d = serial[r];
     for (int k = 0; k < 3; k++) d.coord[k] = coords[r * 3 + k], d.mean[k] = static_cast<float>(means[r * 3 + k]);
     d.num_points = cnt[r];
-    const double* c = &covs[r * 9];
-    d.cov[0] = static_cast<float>(c[0]), d.cov[1] = static_cast<float>(c[1]), d.cov[2] = static_cast<float>(c[2]);
-    d.cov[3] = static_cast<float>(c[4]), d.cov[4] = static_cast<float>(c[5]), d.cov[5] = static_cast<float>(c[8]);
+    cov_upper(&covs[r * 9], 9, d.cov);
     d.intensity = 0.0f;  // intensities are not part of the scan-matching path
   }
   std::FILE* fp = std::fopen(path, "wb");
@@ -851,8 +862,7 @@ b2_status b2_voxelmap_load(b2_ctx* ctx, const char* path, b2_voxelmap** out) {
     const GaussianVoxelData& d = serial[r];
     for (int k = 0; k < 3; k++) coords[r * 3 + k] = d.coord[k], means[r * 3 + k] = d.mean[k];
     cnt[r] = d.num_points;
-    double* c = &covs[r * 9];
-    c[0] = d.cov[0], c[1] = c[3] = d.cov[1], c[2] = c[6] = d.cov[2], c[4] = d.cov[3], c[5] = c[7] = d.cov[4], c[8] = d.cov[5];
+    cov_full(d.cov, &covs[r * 9]);
   }
   B2_TRY(b2_voxelmap_create_from_voxels(ctx, resolution, coords.data(), means.data(), covs.data(), cnt.data(), V, out));
   (*out)->lru_counter = lru_count, (*out)->lru_clear_cycle = lru_cycle ? lru_cycle : 10, (*out)->lru_horizon = lru_thresh;
@@ -870,7 +880,7 @@ b2_status b2_overlap(const b2_voxelmap* const* targets, size_t num_targets, cons
     B2_REQUIRE(targets[j] != nullptr, "error: Failed to cast target voxelmap to GaussianVoxelMapGPU!!");  // gaussian_voxelmap_gpu_funcs.cu:70-75
     B2_REQUIRE(targets[j]->ctx->device == ctx->device, "b2_overlap: map %zu lives on another device", j);
     maps[j].buckets = targets[j]->d_buckets.as<const VoxelBucket>();
-    maps[j].mask = static_cast<uint32_t>(targets[j]->num_buckets / kGroup - 1);
+    maps[j].mask = targets[j]->group_mask();
     maps[j].pad = 0;
     maps[j].inv_leaf = targets[j]->inv_resolution;
     std::memcpy(maps[j].T, Ts_target_source + 16 * j, 12 * sizeof(double));
@@ -1002,7 +1012,7 @@ b2_status b2_voxelmap_lookup(const b2_voxelmap* vm, const double* points, int po
   B2_TRY(di.alloc(n * sizeof(int32_t)));
   B2_CUDA(cudaMemcpyAsync(dp.get(), points, n * point_stride * sizeof(double), cudaMemcpyHostToDevice, st));
   lookup_points_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(dp.as<double>(), point_stride, n, vm->inv_resolution, vm->d_buckets.as<VoxelBucket>(),
-                                                                              static_cast<uint32_t>(vm->num_buckets / kGroup - 1), di.as<int32_t>());
+                                                                              vm->group_mask(), di.as<int32_t>());
   B2_CUDA(cudaGetLastError());
   B2_CUDA(cudaMemcpyAsync(out_index, di.get(), n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
@@ -1019,8 +1029,7 @@ b2_status b2_ivox_create(b2_ctx* ctx, double resolution, b2_ivox** out) {
   B2_REQUIRE(resolution > 0.0, "b2_ivox_create: resolution must be positive");
   B2_CUDA(cudaSetDevice(ctx->device));
   auto iv = std::make_unique<b2_ivox>();
-  B2_TRY(init_map(iv->map, ctx, resolution, 0));  // empty table; the per-voxel arrays get their layout at the first insert
-  B2_CUDA(cudaMemsetAsync(iv->map.d_buckets.get(), 0xFF, iv->map.num_buckets * sizeof(VoxelBucket), ctx->stream));
+  B2_TRY(init_map(iv->map, ctx, resolution, 0));  // the per-voxel arrays get their slot layout at the first insert
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
   *out = iv.release();
   return B2_OK;
@@ -1065,8 +1074,8 @@ b2_status b2_ivox_set_insertion_setting(b2_ivox* iv, double min_dist_in_cell, in
   B2_REQUIRE(min_dist_in_cell >= 0.0, "b2_ivox_set_insertion_setting: negative min_dist_in_cell");
   B2_REQUIRE(max_num_points_in_cell >= 1 && max_num_points_in_cell <= kIvoxMaxPointsInCell, "b2_ivox_set_insertion_setting: max_num_points_in_cell must be 1..%d",
              kIvoxMaxPointsInCell);
-  if (iv->stride > 0 && max_num_points_in_cell > iv->stride)
-    return fail(B2_ERR_INVALID_STATE, "b2_ivox_set_insertion_setting: the map's voxels were laid out for %d points each by the first insert", iv->stride);
+  if (iv->map.slots > 0 && max_num_points_in_cell > iv->map.slots)
+    return fail(B2_ERR_INVALID_STATE, "b2_ivox_set_insertion_setting: the map's voxels were laid out for %d points each by the first insert", iv->map.slots);
   iv->min_sq_dist_in_cell = min_dist_in_cell * min_dist_in_cell;  // flat_container.hpp:19
   iv->max_num_points_in_cell = max_num_points_in_cell;
   return B2_OK;
@@ -1078,47 +1087,12 @@ b2_status b2_ivox_insert(b2_ivox* iv, const double* points, int point_stride, co
   B2_REQUIRE(covs == nullptr || cov_stride == 9 || cov_stride == 16, "b2_ivox_insert: cov_stride must be 9 or 16");
   B2_REQUIRE(n == 0 || points != nullptr, "b2_ivox_insert: points is NULL");
   B2_REQUIRE(n < (1ull << 31), "b2_ivox_insert: at most 2^31-1 points per insert");
-  b2_voxelmap* vm = &iv->map;
-  b2_ctx* ctx = vm->ctx;
-  B2_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
-  if (n > 0) {
-    const int with_covs = covs != nullptr ? 1 : 0;
-    B2_REQUIRE(iv->has_covs < 0 || iv->has_covs == with_covs, "b2_ivox_insert: the map holds points %s covariances; inserts cannot mix both",
-               iv->has_covs ? "with" : "without");
-    const int stride = iv->stride > 0 ? iv->stride : iv->max_num_points_in_cell;  // the first insert fixes the slot layout
-    const size_t V_old = vm->num_voxels;
-    BatchSegments sg;
-    B2_TRY(segment_batch(vm, points, point_stride, covs, cov_stride, n, sg));
-    const size_t V_new = V_old + sg.num_new;
-    // the factor kernel's ring carries voxel * stride + slot as a 32-bit id
-    B2_REQUIRE(V_new * static_cast<size_t>(stride) < (1ull << 31), "b2_ivox_insert: %zu voxels x %d slots exceed 2^31 point records", V_new, stride);
-    if (iv->stride == 0) {
-      // nothing is stored yet: make the per-voxel arrays in the slot layout, and commit the layout only once they exist
-      const size_t cap = std::max<size_t>(V_new, 1), rd = static_cast<size_t>(stride) * kRecordDoubles;
-      DeviceBuffer rec, coords, lru, counts;
-      B2_TRY(rec.alloc(cap * rd * sizeof(double)));
-      B2_TRY(coords.alloc(cap * 3 * sizeof(int32_t)));
-      B2_TRY(lru.alloc(cap * sizeof(uint32_t)));
-      B2_TRY(counts.alloc(cap * sizeof(uint32_t)));
-      vm->d_records = std::move(rec), vm->d_coords = std::move(coords), vm->d_lru = std::move(lru), vm->d_counts = std::move(counts);
-      vm->capacity = cap;
-      vm->rec_doubles = rd;
-      iv->stride = stride;
-    } else {
-      B2_TRY(reserve_voxels(vm, V_new));
-    }
-    iv->has_covs = with_covs;
-    const unsigned vgrid = static_cast<unsigned>((sg.B + 127) / 128);
-    ivox_add_kernel<<<vgrid, 128, 0, st>>>(sg.raw_p.as<double>(), point_stride, sg.raw_c.as<double>(), cov_stride, n, sg.B, sg.idx(), sg.seg_start.as<uint32_t>(),
-                                           sg.seg_of_rank.as<uint32_t>(), sg.batch_coords.as<int32_t>(), sg.existing_id.as<int32_t>(), sg.new_rank.as<uint32_t>(), V_old,
-                                           static_cast<uint32_t>(vm->lru_counter), iv->stride, iv->max_num_points_in_cell, iv->min_sq_dist_in_cell, vm->d_records.as<double>(),
-                                           vm->d_counts.as<uint32_t>(), vm->d_coords.as<int32_t>(), vm->d_lru.as<uint32_t>());
-    B2_CUDA(cudaGetLastError());
-    vm->num_voxels = V_new;
-    B2_CUDA(cudaStreamSynchronize(st));
-  }
-  return lru_sweep_and_rebuild(vm);
+  const int with_covs = covs != nullptr ? 1 : 0;
+  B2_REQUIRE(n == 0 || iv->has_covs < 0 || iv->has_covs == with_covs, "b2_ivox_insert: the map holds points %s covariances; inserts cannot mix both",
+             iv->has_covs ? "with" : "without");
+  const int slots = iv->map.slots > 0 ? iv->map.slots : iv->max_num_points_in_cell;  // the first insert fixes the slot layout
+  const FlatCell cell{slots, iv->max_num_points_in_cell, iv->min_sq_dist_in_cell};
+  return insert_batch(&iv->map, slots, cell, [&] { iv->has_covs = with_covs; }, points, point_stride, covs, cov_stride, n);
 }
 
 b2_status b2_ivox_get_info(const b2_ivox* iv, b2_ivox_info* info) {
@@ -1146,7 +1120,7 @@ b2_status b2_ivox_download(const b2_ivox* iv, int32_t* coords, int32_t* counts, 
   B2_CUDA(cudaSetDevice(vm->ctx->device));
   cudaStream_t st = vm->ctx->stream;
   std::vector<uint32_t> cnt(V);
-  std::vector<double> rec(V * vm->rec_doubles);
+  std::vector<double> rec(V * voxel_payload_doubles(vm->slots));
   B2_CUDA(cudaMemcpyAsync(cnt.data(), vm->d_counts.get(), V * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaMemcpyAsync(rec.data(), vm->d_records.get(), rec.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
   if (coords) B2_CUDA(cudaMemcpyAsync(coords, vm->d_coords.get(), V * 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -1155,18 +1129,10 @@ b2_status b2_ivox_download(const b2_ivox* iv, int32_t* coords, int32_t* counts, 
   for (size_t v = 0; v < V; v++) {
     if (counts) counts[v] = static_cast<int32_t>(cnt[v]);
     for (uint32_t s = 0; s < cnt[v]; s++, o++) {
-      const double* q = &rec[(v * iv->stride + s) * kRecordDoubles];
+      const double* q = &rec[(v * vm->slots + s) * kRecordDoubles];
       if (points)
         for (int k = 0; k < 3; k++) points[o * 3 + k] = q[k];
-      if (covs) {
-        double* c = covs + o * 9;
-        c[0] = q[3];
-        c[1] = c[3] = q[4];
-        c[2] = c[6] = q[5];
-        c[4] = q[6];
-        c[5] = c[7] = q[7];
-        c[8] = q[8];
-      }
+      if (covs) cov_full(q + 3, covs + o * 9);
     }
   }
   return B2_OK;
@@ -1187,8 +1153,8 @@ b2_status b2_ivox_knn(const b2_ivox* iv, const double* queries, int query_stride
   B2_TRY(ds.alloc(nq * k * sizeof(double)));
   B2_CUDA(cudaMemcpyAsync(dq.get(), queries, nq * query_stride * sizeof(double), cudaMemcpyHostToDevice, st));
   ivox_knn_kernel<<<static_cast<unsigned>((nq + 127) / 128), 128, 0, st>>>(dq.as<double>(), query_stride, nq, k, max_sq_dist, vm->d_buckets.as<VoxelBucket>(),
-                                                                           static_cast<uint32_t>(vm->num_buckets / kGroup - 1), vm->inv_resolution, vm->d_records.as<double>(),
-                                                                           vm->d_counts.as<uint32_t>(), iv->stride, iv->neighbor_mode, vm->num_voxels,
+                                                                           vm->group_mask(), vm->inv_resolution, vm->d_records.as<double>(),
+                                                                           vm->d_counts.as<uint32_t>(), vm->slots, iv->neighbor_mode, vm->num_voxels,
                                                                            di.as<long long>(), ds.as<double>());
   B2_CUDA(cudaGetLastError());
   B2_CUDA(cudaMemcpyAsync(out_index, di.get(), nq * k * sizeof(long long), cudaMemcpyDeviceToHost, st));

@@ -58,11 +58,25 @@ def assert_same_knn(dev, ref, q, k, max_sq):
                 assert idx[i][j] == ri[j], (i, j)
 
 
-@pytest.mark.parametrize("mode", [1, 7, 19, 27])
-def test_map_and_knn_match_restatement(g, mode):
+def as_layout(pts, covs, layout):
+    """The frame in one of the insert input layouts: xyz with 3x3 covariances, xyzw (w = 1) with 4x4, or xyz without covariances."""
+    if layout == "xyzw-4x4":
+        covs4 = np.zeros((len(covs), 4, 4))
+        covs4[:, :3, :3] = covs
+        covs4[:, 3, 3] = 1.0
+        return np.hstack([pts, np.ones((len(pts), 1))]), covs4
+    return pts, (None if layout == "xyz" else covs)
+
+
+@pytest.mark.parametrize(
+    "mode,layout",
+    [pytest.param(m, "xyz-3x3", id=str(m)) for m in (1, 7, 19, 27)] + [pytest.param(7, layout, id=f"7-{layout}") for layout in ("xyzw-4x4", "xyz")],
+)
+def test_map_and_knn_match_restatement(g, mode, layout):
     dev, ref = make_pair(g, mode)
     rng = np.random.default_rng(mode)
-    for f, (pts, covs) in enumerate(trajectory_frames()):
+    for f, frame in enumerate(trajectory_frames()):
+        pts, covs = as_layout(*frame, layout)
         dev.insert(pts, covs)
         ref.insert(pts, covs)
         assert_same_map(dev, ref)

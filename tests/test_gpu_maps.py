@@ -50,6 +50,30 @@ def test_incremental_insert_and_lru_match_cpu_map_bitwise(g):
     assert max(sizes) > sizes[-1] or any(b < a for a, b in zip(sizes, sizes[1:]))  # the LRU sweep removed voxels at some point
 
 
+def test_xyzw_4x4_insert_equals_xyz_3x3_insert_bitwise(g):
+    """The same clouds inserted as (xyz, 3 x 3 covariances) and as (xyzw with w = 1, 4 x 4 covariances): after EVERY insert the two
+    maps download bit-identical voxels and answer lookups identically, LRU evictions included."""
+    a, b = g.GaussianVoxelMapGPU(0.5), g.GaussianVoxelMapGPU(0.5)
+    a.set_lru(3, 4)
+    b.set_lru(3, 4)
+    sizes = []
+    for step in range(25):
+        pts, covs = syn.make_cloud(6000 + 37 * step, stream=200 + step, scale=0.2)
+        pts = pts + np.array([1.5 * step, 0.3 * step, 0.0])
+        covs4 = np.zeros((len(covs), 4, 4))
+        covs4[:, :3, :3] = covs
+        covs4[:, 3, 3] = 1.0
+        a.insert(g.PointCloud(pts, covs))
+        b.insert(g.PointCloud(np.hstack([pts, np.ones((len(pts), 1))]), covs4))
+        got_a, got_b = a.download(), b.download()
+        for k in ("coords", "n", "means", "covs"):
+            assert np.array_equal(got_a[k], got_b[k]), (step, k)
+        sizes.append(a.num_voxels)
+        q = pts[::7] + 0.01
+        assert np.array_equal(a.lookup_voxel_index(q), b.lookup_voxel_index(q))
+    assert max(sizes) > sizes[-1] or any(y < x for x, y in zip(sizes, sizes[1:]))  # the LRU sweep removed voxels at some point
+
+
 def test_factor_sees_map_growth(g):
     """A factor built over a map keeps working, with the new contents, after further insert() calls (descriptor refresh)."""
     tp, tc = syn.make_cloud(30000, stream=1, scale=0.25)

@@ -278,10 +278,10 @@ b2_status b2_cloud_create_with_normals(b2_ctx* ctx, const double* points, int po
     c->normal_bytes = force64 ? 8 : (compact || !(nflags & 1u)) ? 4 : 8;
     B2_TRY(c->d_normals.alloc(3 * c->n_pad * c->normal_bytes));
     const unsigned ngrid = static_cast<unsigned>((c->n_pad + 255) / 256);
-    if (c->normal_bytes == 4)
-      gather_normals_kernel<float><<<ngrid, 256, 0, st>>>(raw_n.as<const double>(), normal_stride, c->d_perm.as<const uint32_t>(), n, c->n_pad, c->d_normals.as<float>());
-    else
-      gather_normals_kernel<double><<<ngrid, 256, 0, st>>>(raw_n.as<const double>(), normal_stride, c->d_perm.as<const uint32_t>(), n, c->n_pad, c->d_normals.as<double>());
+    with_storage(c->normal_bytes, [&](auto t) {
+      using NT = decltype(t);
+      gather_normals_kernel<NT><<<ngrid, 256, 0, st>>>(raw_n.as<const double>(), normal_stride, c->d_perm.as<const uint32_t>(), n, c->n_pad, c->d_normals.as<NT>());
+    });
     B2_CUDA(cudaGetLastError());
     B2_CUDA(cudaStreamSynchronize(st));  // raw_n goes out of scope
   }
@@ -293,14 +293,13 @@ b2_status b2_cloud_create_with_normals(b2_ctx* ctx, const double* points, int po
   const double* rp = raw_p.as<const double>();
   const double* rc = raw_c.as<const double>();
   const uint32_t* perm = c->d_perm.as<const uint32_t>();
-  if (c->point_bytes == 4 && c->cov_bytes != 8)
-    gather_planes_kernel<float, float><<<grid, 256, 0, st>>>(rp, point_stride, rc, cov_stride, perm, n, c->n_pad, c->d_points.as<float>(), c->d_covs.as<float>());
-  else if (c->point_bytes == 4)
-    gather_planes_kernel<float, double><<<grid, 256, 0, st>>>(rp, point_stride, rc, cov_stride, perm, n, c->n_pad, c->d_points.as<float>(), c->d_covs.as<double>());
-  else if (c->cov_bytes != 8)
-    gather_planes_kernel<double, float><<<grid, 256, 0, st>>>(rp, point_stride, rc, cov_stride, perm, n, c->n_pad, c->d_points.as<double>(), c->d_covs.as<float>());
-  else
-    gather_planes_kernel<double, double><<<grid, 256, 0, st>>>(rp, point_stride, rc, cov_stride, perm, n, c->n_pad, c->d_points.as<double>(), c->d_covs.as<double>());
+  with_storage(c->point_bytes, [&](auto p) {
+    with_storage(c->cov_bytes, [&](auto v) {  // no covariances: the float instantiation, which writes none
+      using PT = decltype(p);
+      using CT = decltype(v);
+      gather_planes_kernel<PT, CT><<<grid, 256, 0, st>>>(rp, point_stride, rc, cov_stride, perm, n, c->n_pad, c->d_points.as<PT>(), c->d_covs.as<CT>());
+    });
+  });
   B2_CUDA(cudaGetLastError());
   B2_CUDA(cudaStreamSynchronize(st));
 
@@ -335,10 +334,10 @@ b2_status b2_cloud_download_normals(const b2_cloud* c, double* out_normals) {
   DeviceBuffer d_out;
   B2_TRY(d_out.alloc(c->n * 3 * sizeof(double)));
   const unsigned grid = static_cast<unsigned>((c->n + 255) / 256);
-  if (c->normal_bytes == 4)
-    scatter_normals_kernel<float><<<grid, 256, 0, st>>>(c->d_normals.as<const float>(), c->d_perm.as<const uint32_t>(), c->n, c->n_pad, d_out.as<double>());
-  else
-    scatter_normals_kernel<double><<<grid, 256, 0, st>>>(c->d_normals.as<const double>(), c->d_perm.as<const uint32_t>(), c->n, c->n_pad, d_out.as<double>());
+  with_storage(c->normal_bytes, [&](auto t) {
+    using NT = decltype(t);
+    scatter_normals_kernel<NT><<<grid, 256, 0, st>>>(c->d_normals.as<const NT>(), c->d_perm.as<const uint32_t>(), c->n, c->n_pad, d_out.as<double>());
+  });
   B2_CUDA(cudaGetLastError());
   B2_CUDA(cudaMemcpyAsync(out_normals, d_out.get(), c->n * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));

@@ -114,24 +114,34 @@ __device__ __forceinline__ double ivox_sq_dist(double px, double py, double pz, 
   return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
 }
 
+// What a neighbour search in an iVox needs: its voxel table, its point records (slots per voxel, in voxel id order), the points
+// stored per voxel, and the neighbour voxel mode.
+struct IvoxView {
+  VoxelTableView table;
+  const double* records;
+  const uint32_t* counts;
+  int slots;
+  int mode;  // 1, 7, 19 or 27
+};
+
 // Nearest stored point of an iVox to q within max_sq (KnnResult<1>: strict '<', ties to the first point visited -- neighbour
-// voxels in offset order, points in slot order).  Returns the record id voxel * stride + slot, or -1.
-__device__ __forceinline__ int ivox_nn1(const VoxelBucket* __restrict__ buckets, uint32_t group_mask, double inv_leaf, const double* __restrict__ records,
-                                        const uint32_t* __restrict__ counts, int stride, int mode, double qx, double qy, double qz, double max_sq, double* out_sq) {
+// voxels in offset order, points in slot order).  Returns the record id voxel * slots + slot, or -1.
+__device__ __forceinline__ int ivox_nn1(const IvoxView& iv, double qx, double qy, double qz, double max_sq, double* out_sq) {
+  const double inv_leaf = iv.table.inv_leaf;
   const int cx = voxel_coord1(qx, inv_leaf), cy = voxel_coord1(qy, inv_leaf), cz = voxel_coord1(qz, inv_leaf);
   double best = max_sq;
   int best_id = -1;
 #pragma unroll 1
-  for (int t = 0; t < mode; t++) {
+  for (int t = 0; t < iv.mode; t++) {
     int dx, dy, dz;
-    ivox_offset(mode, t, dx, dy, dz);
-    const int v = lookup_voxel(buckets, group_mask, cx + dx, cy + dy, cz + dz);
+    ivox_offset(iv.mode, t, dx, dy, dz);
+    const int v = lookup_voxel(iv.table.buckets, iv.table.group_mask, cx + dx, cy + dy, cz + dz);
     if (v < 0) continue;
-    const int c = static_cast<int>(__ldg(counts + v));
-    const int first = v * stride;
+    const int c = static_cast<int>(__ldg(iv.counts + v));
+    const int first = v * iv.slots;
 #pragma unroll 1
     for (int s = 0; s < c; s++) {
-      const double* r = records + static_cast<size_t>(first + s) * kRecordDoubles;
+      const double* r = iv.records + static_cast<size_t>(first + s) * kRecordDoubles;
       const double2 xy = __ldg(reinterpret_cast<const double2*>(r));
       const double d = ivox_sq_dist(xy.x, xy.y, __ldg(r + 2), qx, qy, qz);
       if (d < best) {

@@ -52,11 +52,13 @@ struct TreeProbeWarps {
   static constexpr int kIPL = 1;
 };
 
+// SEARCH: what the probe warps search; the descriptor holds it in its member `voxel`, `tree` or `ivox`.
 // SOURCE_COV: the kind reads the source cloud's covariances (ICP kinds do not; their CT is a dummy).
 // METRIC: the weight matrix of accumulate_point_f (0 GICP / VGICP, 1 point-to-point ICP, 2 point-to-plane ICP).
 // VALIDATE: the probe warps also stream the source normals and reject points that face away from the sensor (surface validation).
-template <class Warps, bool SOURCE_COV, int METRIC, bool VALIDATE = false>
+template <class Warps, Search SEARCH, bool SOURCE_COV, int METRIC, bool VALIDATE = false>
 struct Traits : Warps {
+  static constexpr Search kSearch = SEARCH;
   static constexpr bool kSourceCov = SOURCE_COV;
   static constexpr int kMetric = METRIC;
   static constexpr bool kValidate = VALIDATE;
@@ -72,19 +74,19 @@ struct Traits : Warps {
   static_assert(kWarpPoints * 4 % 128 == 0 || Warps::kPPL == 1, "coordinate prefetch works on whole lines");
 };
 
-// One entry per b2_factor_kind.  Every kind but the two VGICP ones searches a kd-tree or an iVox.
+// One entry per b2_factor_kind.
 template <int KIND>
 struct KindTraits;
 template <>
-struct KindTraits<B2_FACTOR_VGICP> : Traits<VoxelProbeWarps, true, 0> {};
+struct KindTraits<B2_FACTOR_VGICP> : Traits<VoxelProbeWarps, Search::Voxel, true, 0> {};
 template <>
-struct KindTraits<B2_FACTOR_GICP> : Traits<TreeProbeWarps, true, 0> {};
+struct KindTraits<B2_FACTOR_GICP> : Traits<TreeProbeWarps, Search::Tree, true, 0> {};
 template <>
-struct KindTraits<B2_FACTOR_ICP> : Traits<TreeProbeWarps, false, 1> {};
+struct KindTraits<B2_FACTOR_ICP> : Traits<TreeProbeWarps, Search::Tree, false, 1> {};
 template <>
-struct KindTraits<B2_FACTOR_ICP_PLANE> : Traits<TreeProbeWarps, false, 2> {};
+struct KindTraits<B2_FACTOR_ICP_PLANE> : Traits<TreeProbeWarps, Search::Tree, false, 2> {};
 template <>
-struct KindTraits<B2_FACTOR_GICP_IVOX> : Traits<TreeProbeWarps, true, 0> {};
+struct KindTraits<B2_FACTOR_GICP_IVOX> : Traits<TreeProbeWarps, Search::Ivox, true, 0> {};
 // VGICP with surface validation.  A probe lane also holds its points' normals from the coordinate load to the rejection test.  With
 // two points per lane that does not fit the 88 probe registers for launches over sets (ptxas: 120 - 144 bytes of stack), and the
 // accumulate warps cannot give any up (below 168 they spill).  One point per lane fits with 0 spill bytes in every instantiation.
@@ -92,7 +94,7 @@ struct ValidatedVoxelProbeWarps : VoxelProbeWarps {
   static constexpr int kPPL = 1;
 };
 template <>
-struct KindTraits<B2_FACTOR_VGICP_VALIDATED> : Traits<ValidatedVoxelProbeWarps, true, 0, true> {};
+struct KindTraits<B2_FACTOR_VGICP_VALIDATED> : Traits<ValidatedVoxelProbeWarps, Search::Voxel, true, 0, true> {};
 
 // Surface validation threshold: the reference's float constant (lookup_voxels.cuh:86, cos 80 deg) widened to double.
 constexpr double kSurfaceValidationThresh = static_cast<double>(0.174f);
@@ -296,8 +298,8 @@ __device__ __forceinline__ void load_operands(Batch& b, const double* __restrict
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// The kernel.  KIND: a b2_factor_kind; it selects the search (voxel hash probe, kd-tree 1-NN or iVox neighbour voxels) and
-// KindTraits<KIND>.  MODE: linearize / error-only.
+// The kernel.  KIND: a b2_factor_kind; KindTraits<KIND> gives its launch shape and its search (kSearch: voxel hash probe,
+// kd-tree 1-NN or iVox neighbour voxels).  MODE: linearize / error-only.
 // ---------------------------------------------------------------------------------------------------------------
 // SINGLE: the launch covers exactly one factor and its pose is the by-value parameter `pose` (linearize: the linearization
 // point; error: the evaluation point) -- DMUL / DFMA take it from uniform registers, nothing is read from host memory.
@@ -309,7 +311,7 @@ __device__ __forceinline__ void factor_kernel_body(const FactorDesc* __restrict_
   using K = KindTraits<KIND>;
   constexpr int kP = K::kP, kC = K::kC, kPPL = K::kPPL, kWarpPoints = K::kWarpPoints, kTile = K::kTile, kRing = K::kRing;
   constexpr int kRingsPerConsumer = K::kRingsPerConsumer, kIPL = K::kIPL;
-  constexpr bool kVoxel = KIND == B2_FACTOR_VGICP || KIND == B2_FACTOR_VGICP_VALIDATED;  // voxel hash probe
+  constexpr bool kVoxel = K::kSearch == Search::Voxel;  // voxel hash probe
   constexpr bool kValidate = K::kValidate && MODE == MODE_LINEARIZE;  // correspondences are only established when linearizing
   __shared__ Shared<K> sh;
   extern __shared__ __align__(16) unsigned char dyn_smem[];
@@ -351,12 +353,14 @@ __device__ __forceinline__ void factor_kernel_body(const FactorDesc* __restrict_
       const CT* __restrict__ cv = static_cast<const CT*>(dg->covs);
       const double* __restrict__ records = dg->records;
       int32_t* __restrict__ corr = dg->corr;
-      const VoxelBucket* __restrict__ buckets = dg->buckets;
-      const uint32_t bucket_mask = dg->bucket_mask;
-      const double inv_leaf = dg->inv_leaf;
-      // surface validation: the source normals (3 planes of n_pad, float32 or float64) travel in the descriptor's kd-tree fields
-      const void* __restrict__ nrm = kValidate ? dg->leaf_pts : nullptr;
-      const bool nrm_f32 = kValidate && dg->leaf_f32 != 0u;
+      // the voxel table of the voxel hash probe or of the iVox's neighbour voxels
+      const VoxelTableView table = K::kSearch == Search::Ivox ? dg->ivox.table : dg->voxel.table;
+      const VoxelBucket* __restrict__ buckets = table.buckets;
+      const uint32_t bucket_mask = table.group_mask;
+      const double inv_leaf = table.inv_leaf;
+      // surface validation: the source normals (3 planes of n_pad, float32 or float64)
+      const void* __restrict__ nrm = kValidate ? dg->voxel.normals : nullptr;
+      const bool nrm_f32 = kValidate && dg->voxel.normals_f32 != 0u;
       // Residuals / correspondences are evaluated at this pose (linearize: the linearization point itself).  It lives in
       // this warp's shared-memory slot, not in registers: 24 registers less per probe thread, re-read (broadcast) per tile.
       if (!SINGLE) {
@@ -369,7 +373,7 @@ __device__ __forceinline__ void factor_kernel_body(const FactorDesc* __restrict_
       }
       auto Rm = [&](int i) -> double { return SINGLE ? pose.m[(i / 3) * 4 + (i % 3)] : sh.probe_pose[p][i]; };
       auto tvec = [&](int i) -> double { return SINGLE ? pose.m[i * 4 + 3] : sh.probe_pose[p][9 + i]; };
-      const KdTreeView tv{dg->nodes, dg->leaf_pts, static_cast<int>(dg->leaf_f32)};
+      const KdTreeView tv = dg->tree.view;
       const double max_sq = dg->max_sq;
 
       // Virtual tile v of the factor (the CTA owns a contiguous range of them) is physical tile (v * S) mod n_tiles with
@@ -490,11 +494,10 @@ __device__ __forceinline__ void factor_kernel_body(const FactorDesc* __restrict_
                 g = (g + 1) & bucket_mask;
                 id[k] = match_group(load_group(buckets, g), cx[k], cy[k], cz[k]);
               }
-            } else if (KIND == B2_FACTOR_GICP_IVOX) {
-              // iVox: the neighbour voxels of the transformed point (offset order) through the bucket table, their point slots in
-              // order; the ivox's point counts travel in leaf_pts, slots per voxel | neighbour mode << 8 in ivox_slots_mode
-              id[k] = ok[k] ? ivox_nn1(buckets, bucket_mask, inv_leaf, records, static_cast<const uint32_t*>(dg->leaf_pts), static_cast<int>(dg->ivox_slots_mode & 0xffu),
-                                       static_cast<int>(dg->ivox_slots_mode >> 8), __dadd_rn(u[k][0], tvec(0)), __dadd_rn(u[k][1], tvec(1)), __dadd_rn(u[k][2], tvec(2)), max_sq, nullptr)
+            } else if (K::kSearch == Search::Ivox) {
+              // iVox: the neighbour voxels of the transformed point (offset order) through the bucket table, their point slots in order
+              id[k] = ok[k] ? ivox_nn1(IvoxView{table, records, dg->ivox.counts, dg->ivox.slots(), dg->ivox.mode()}, __dadd_rn(u[k][0], tvec(0)), __dadd_rn(u[k][1], tvec(1)),
+                                       __dadd_rn(u[k][2], tvec(2)), max_sq, nullptr)
                             : -1;
             } else {
               double sq;

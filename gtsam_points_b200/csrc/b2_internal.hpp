@@ -128,6 +128,14 @@ b2_status cub_run(DeviceBuffer& scratch, cudaStream_t st, Call&& call) {
   return cub_launch(scratch, call);
 }
 
+// Storage precision of a plane array: calls fn(T{}) with T = double for 8-byte elements, float otherwise (4 bytes, or an absent
+// array that the instantiation does not read).
+template <class Fn>
+auto with_storage(int bytes, Fn&& fn) {
+  if (bytes == 8) return fn(double{});
+  return fn(float{});
+}
+
 inline size_t round_up(size_t x, size_t m) { return (x + m - 1) / m * m; }
 inline uint64_t next_pow2(uint64_t x) {
   uint64_t p = 1;
@@ -145,6 +153,16 @@ struct alignas(16) VoxelBucket {
 
 // Buckets per group of a voxel table (b2_device.cuh: bucket groups); the number of groups is a power of two.
 constexpr int kGroup = 2;
+
+// What a lookup in a voxel table needs (b2_voxelmap::table()).  24 bytes: the factor descriptor and the overlap kernel's
+// per-map record hold it at fixed offsets.
+struct VoxelTableView {
+  const VoxelBucket* buckets;
+  uint32_t group_mask;  // bucket groups - 1
+  uint32_t pad;
+  double inv_leaf;      // 1 / voxel resolution
+};
+static_assert(sizeof(VoxelTableView) == 24, "VoxelTableView layout");
 
 // One target record: mean (3), upper-triangular covariance (6), number of points (1).  80 bytes = 5 x LDG.128.
 // Used for voxels (VGICP) and for target points (GICP, count = 1).
@@ -243,6 +261,7 @@ struct b2_voxelmap {
   int slots = 0;                 // point slots per voxel (0: Gaussian voxel records)
   b2::DeviceBuffer d_counts;     // slots > 0 only, uint32: points stored per voxel (slots 0..count-1 of its records are occupied)
   uint32_t group_mask() const { return static_cast<uint32_t>(num_buckets / b2::kGroup - 1); }  // bucket groups - 1
+  b2::VoxelTableView table() const { return {d_buckets.as<const b2::VoxelBucket>(), group_mask(), 0u, inv_resolution}; }
   size_t device_bytes() const { return d_buckets.bytes() + d_records.bytes() + d_coords.bytes() + d_lru.bytes() + d_counts.bytes(); }
 };
 

@@ -210,8 +210,7 @@ __global__ void lru_compact_kernel(const uint32_t* __restrict__ keep, const uint
 
 // IncrementalVoxelMap::knn_search (incremental_voxelmap_impl.hpp:71-92) with KnnResult<-1> (knn_result.hpp:84-109): one thread per
 // query, neighbour voxels in offset order, points in slot order, strict '<' against the current worst, stable insertion.
-__global__ void ivox_knn_kernel(const double* __restrict__ q, int qstride, size_t nq, int k, double max_sq, const VoxelBucket* __restrict__ buckets, uint32_t gmask,
-                                double inv_leaf, const double* __restrict__ records, const uint32_t* __restrict__ counts, int stride, int mode, size_t num_voxels,
+__global__ void ivox_knn_kernel(const double* __restrict__ q, int qstride, size_t nq, int k, double max_sq, const IvoxView iv, size_t num_voxels,
                                 long long* __restrict__ out_idx, double* __restrict__ out_sq) {
   const size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
   if (i >= nq) return;
@@ -220,15 +219,15 @@ __global__ void ivox_knn_kernel(const double* __restrict__ q, int qstride, size_
   for (int j = 0; j < k; j++) idx[j] = -1, sq[j] = max_sq;
   if (num_voxels == 0) return;
   const double qx = q[i * qstride], qy = q[i * qstride + 1], qz = q[i * qstride + 2];
-  const int cx = voxel_coord1(qx, inv_leaf), cy = voxel_coord1(qy, inv_leaf), cz = voxel_coord1(qz, inv_leaf);
+  const int cx = voxel_coord1(qx, iv.table.inv_leaf), cy = voxel_coord1(qy, iv.table.inv_leaf), cz = voxel_coord1(qz, iv.table.inv_leaf);
   int found = 0;
-  for (int t = 0; t < mode; t++) {
+  for (int t = 0; t < iv.mode; t++) {
     int dx, dy, dz;
-    ivox_offset(mode, t, dx, dy, dz);
-    const int v = lookup_voxel(buckets, gmask, cx + dx, cy + dy, cz + dz);
+    ivox_offset(iv.mode, t, dx, dy, dz);
+    const int v = lookup_voxel(iv.table.buckets, iv.table.group_mask, cx + dx, cy + dy, cz + dz);
     if (v < 0) continue;
-    const int c = static_cast<int>(counts[v]);
-    const double* rec = records + static_cast<size_t>(v) * stride * kRecordDoubles;
+    const int c = static_cast<int>(iv.counts[v]);
+    const double* rec = iv.records + static_cast<size_t>(v) * iv.slots * kRecordDoubles;
     for (int s = 0; s < c; s++) {
       const double d = ivox_sq_dist(rec[s * kRecordDoubles], rec[s * kRecordDoubles + 1], rec[s * kRecordDoubles + 2], qx, qy, qz);
       if (d >= sq[k - 1]) continue;
@@ -264,24 +263,20 @@ __global__ void insert_buckets_kernel(const int32_t* __restrict__ coords, size_t
   }
 }
 
-__global__ void lookup_points_kernel(const double* __restrict__ pts, int pstride, size_t n, double inv_leaf, const VoxelBucket* __restrict__ buckets,
-                                     uint32_t mask, int32_t* __restrict__ out) {
+__global__ void lookup_points_kernel(const double* __restrict__ pts, int pstride, size_t n, const VoxelTableView table, int32_t* __restrict__ out) {
   const size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
   if (i >= n) return;
-  const int x = voxel_coord1(pts[i * pstride + 0], inv_leaf);
-  const int y = voxel_coord1(pts[i * pstride + 1], inv_leaf);
-  const int z = voxel_coord1(pts[i * pstride + 2], inv_leaf);
-  out[i] = lookup_voxel(buckets, mask, x, y, z);
+  const int x = voxel_coord1(pts[i * pstride + 0], table.inv_leaf);
+  const int y = voxel_coord1(pts[i * pstride + 1], table.inv_leaf);
+  const int z = voxel_coord1(pts[i * pstride + 2], table.inv_leaf);
+  out[i] = lookup_voxel(table.buckets, table.group_mask, x, y, z);
 }
 
 // overlap_gpu (src/gtsam_points/types/gaussian_voxelmap_gpu_funcs.cu:65-194): a source point counts if, for the FIRST map j in
 // order, T_j p falls into one of its voxels.  float64 with the CPU map's operation order (CPU / GPU agree exactly, where the
 // reference's float32 path promises ~1 %: src/test/test_voxelmap.cpp:231-239).
 struct OverlapMap {
-  const VoxelBucket* buckets;
-  uint32_t mask;
-  uint32_t pad;
-  double inv_leaf;
+  VoxelTableView table;
   double T[12];  // rows of [R | t]
 };
 template <typename PT>
@@ -296,9 +291,9 @@ __global__ void overlap_kernel(const PT* __restrict__ pts, size_t n, size_t n_pa
 #pragma unroll
       for (int r = 0; r < 3; r++) {
         const double q = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(m.T[r * 4 + 0], x), __dmul_rn(m.T[r * 4 + 1], y)), __dmul_rn(m.T[r * 4 + 2], z)), m.T[r * 4 + 3]);
-        c[r] = voxel_coord1(q, m.inv_leaf);
+        c[r] = voxel_coord1(q, m.table.inv_leaf);
       }
-      hit = lookup_voxel(m.buckets, m.mask, c[0], c[1], c[2]) >= 0;
+      hit = lookup_voxel(m.table.buckets, m.table.group_mask, c[0], c[1], c[2]) >= 0;
     }
   }
   const unsigned b = __ballot_sync(0xffffffffu, hit);
@@ -879,10 +874,7 @@ b2_status b2_overlap(const b2_voxelmap* const* targets, size_t num_targets, cons
   for (size_t j = 0; j < num_targets; j++) {
     B2_REQUIRE(targets[j] != nullptr, "error: Failed to cast target voxelmap to GaussianVoxelMapGPU!!");  // gaussian_voxelmap_gpu_funcs.cu:70-75
     B2_REQUIRE(targets[j]->ctx->device == ctx->device, "b2_overlap: map %zu lives on another device", j);
-    maps[j].buckets = targets[j]->d_buckets.as<const VoxelBucket>();
-    maps[j].mask = targets[j]->group_mask();
-    maps[j].pad = 0;
-    maps[j].inv_leaf = targets[j]->inv_resolution;
+    maps[j].table = targets[j]->table();
     std::memcpy(maps[j].T, Ts_target_source + 16 * j, 12 * sizeof(double));
   }
   if (source->n == 0) {
@@ -895,10 +887,10 @@ b2_status b2_overlap(const b2_voxelmap* const* targets, size_t num_targets, cons
   B2_CUDA(cudaMemcpyAsync(d_maps.get(), maps.data(), maps.size() * sizeof(OverlapMap), cudaMemcpyHostToDevice, st));
   B2_CUDA(cudaMemsetAsync(d_count.get(), 0, sizeof(unsigned long long), st));
   const unsigned grid = static_cast<unsigned>((source->n + 255) / 256);
-  if (source->point_bytes == 4)
-    overlap_kernel<float><<<grid, 256, 0, st>>>(source->d_points.as<const float>(), source->n, source->n_pad, d_maps.as<OverlapMap>(), static_cast<int>(num_targets), d_count.as<unsigned long long>());
-  else
-    overlap_kernel<double><<<grid, 256, 0, st>>>(source->d_points.as<const double>(), source->n, source->n_pad, d_maps.as<OverlapMap>(), static_cast<int>(num_targets), d_count.as<unsigned long long>());
+  with_storage(source->point_bytes, [&](auto p) {
+    using PT = decltype(p);
+    overlap_kernel<PT><<<grid, 256, 0, st>>>(source->d_points.as<const PT>(), source->n, source->n_pad, d_maps.as<OverlapMap>(), static_cast<int>(num_targets), d_count.as<unsigned long long>());
+  });
   B2_CUDA(cudaGetLastError());
   unsigned long long cnt = 0;
   B2_CUDA(cudaMemcpyAsync(&cnt, d_count.get(), sizeof(cnt), cudaMemcpyDeviceToHost, st));
@@ -1011,8 +1003,7 @@ b2_status b2_voxelmap_lookup(const b2_voxelmap* vm, const double* points, int po
   B2_TRY(dp.alloc(n * point_stride * sizeof(double)));
   B2_TRY(di.alloc(n * sizeof(int32_t)));
   B2_CUDA(cudaMemcpyAsync(dp.get(), points, n * point_stride * sizeof(double), cudaMemcpyHostToDevice, st));
-  lookup_points_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(dp.as<double>(), point_stride, n, vm->inv_resolution, vm->d_buckets.as<VoxelBucket>(),
-                                                                              vm->group_mask(), di.as<int32_t>());
+  lookup_points_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(dp.as<double>(), point_stride, n, vm->table(), di.as<int32_t>());
   B2_CUDA(cudaGetLastError());
   B2_CUDA(cudaMemcpyAsync(out_index, di.get(), n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
@@ -1152,10 +1143,9 @@ b2_status b2_ivox_knn(const b2_ivox* iv, const double* queries, int query_stride
   B2_TRY(di.alloc(nq * k * sizeof(long long)));
   B2_TRY(ds.alloc(nq * k * sizeof(double)));
   B2_CUDA(cudaMemcpyAsync(dq.get(), queries, nq * query_stride * sizeof(double), cudaMemcpyHostToDevice, st));
-  ivox_knn_kernel<<<static_cast<unsigned>((nq + 127) / 128), 128, 0, st>>>(dq.as<double>(), query_stride, nq, k, max_sq_dist, vm->d_buckets.as<VoxelBucket>(),
-                                                                           vm->group_mask(), vm->inv_resolution, vm->d_records.as<double>(),
-                                                                           vm->d_counts.as<uint32_t>(), vm->slots, iv->neighbor_mode, vm->num_voxels,
-                                                                           di.as<long long>(), ds.as<double>());
+  const IvoxView view{vm->table(), vm->d_records.as<const double>(), vm->d_counts.as<const uint32_t>(), vm->slots, iv->neighbor_mode};
+  ivox_knn_kernel<<<static_cast<unsigned>((nq + 127) / 128), 128, 0, st>>>(dq.as<double>(), query_stride, nq, k, max_sq_dist, view, vm->num_voxels, di.as<long long>(),
+                                                                           ds.as<double>());
   B2_CUDA(cudaGetLastError());
   B2_CUDA(cudaMemcpyAsync(out_index, di.get(), nq * k * sizeof(long long), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaMemcpyAsync(out_sq_dist, ds.get(), nq * k * sizeof(double), cudaMemcpyDeviceToHost, st));

@@ -9,7 +9,7 @@ held to the 1e-9 bar with bit-identical correspondences:
 * one set holding all 16 (kind, PT, CT) groups: one launch per group, every factor against its oracle, then again with a
   correspondence-update tolerance that freezes the GICP / ICP / iVox factors on the second call;
 * one-factor sets of the 12 kinds with a by-value instantiation, through the host-pose path;
-* the 4 GICP target storages (build_target_records_kernel<PT, CT>) and the 2 ICP ones;
+* the 4 GICP target storages (gather_leaf_records_kernel<PT, CT>) and the 2 ICP ones;
 * COMPACT_F32 storage of every kind with source covariances, against the oracle fed the float32-rounded inputs.
 A CPU test reads the kernels compiled into the library and checks that the parametrisation covers every one of them.
 """
@@ -259,7 +259,7 @@ TARGET_STORAGES = [(pb, cb) for pb in (4, 8) for cb in (4, 8)]
 @pytest.mark.gpu
 @pytest.mark.parametrize("storage", TARGET_STORAGES, ids=[f"p{pb}c{cb}" for pb, cb in TARGET_STORAGES])
 def test_gicp_target_storages(g, scene, storage):
-    """Each target storage builds its records with its own build_target_records_kernel<PT, CT>; the kd-tree's leaf records
+    """Each target storage builds its records with its own gather_leaf_records_kernel<PT, CT>; the kd-tree's leaf records
     follow the target points (float32 for float32-exact points)."""
     pb, cb = storage
     tp, tc = scene["tp"][:15000], scene["tc"][:15000]

@@ -244,22 +244,26 @@ def test_enabling_validation_where_it_cannot_apply(g, scene):
 
 
 def test_point_to_plane_icp_from_cloud_normals(g, scene):
+    """The cloud's normal planes give the same factor, bit for bit, as the host normal array, for float64 normals and for
+    float32-exact ones (stored as float32 planes)."""
     rng = np.random.default_rng(12)
-    tn = rng.normal(size=(len(scene["tp"]), 3))
-    tn /= np.linalg.norm(tn, axis=1, keepdims=True)
-    tgt = g.PointCloud(scene["tp"], normals=tn)
+    tn64 = rng.normal(size=(len(scene["tp"]), 3))
+    tn64 /= np.linalg.norm(tn64, axis=1, keepdims=True)
     src = g.PointCloud(scene["sp"])
-    tree = g.KdTree(tgt)
-    from_cloud = g.IntegratedPointToPlaneICPFactor(0, 1, tgt, src, target_tree=tree)
-    h = C.c_void_p()
-    bare = g.PointCloud(scene["tp"])  # the same target without normals: they come as the host array
-    capi.check(capi.lib().b2_icp_factor_create(tgt.ctx.h, bare.h, tree.h, src.h, 1, capi.dptr(np.ascontiguousarray(tn)), C.byref(h)))
     delta = np.ascontiguousarray(scene["poses"][5])
-    buf = np.zeros(capi.B2_LINEARIZED_DOUBLES)
-    capi.check(capi.lib().b2_factor_linearize(h, capi.dptr(delta), capi.dptr(buf)))
-    from_cloud.linearize({0: np.eye(4), 1: delta})
-    host = capi.unpack_linearized(buf)
-    assert all(np.array_equal(host[k], from_cloud._last[k]) for k in host)
-    capi.lib().b2_factor_destroy(h)
+    for normal_bytes, tn in ((8, tn64), (4, tn64.astype(np.float32).astype(np.float64))):
+        tgt = g.PointCloud(scene["tp"], normals=tn)
+        assert tgt.info().normal_bytes == normal_bytes
+        tree = g.KdTree(tgt)
+        from_cloud = g.IntegratedPointToPlaneICPFactor(0, 1, tgt, src, target_tree=tree)
+        h = C.c_void_p()
+        bare = g.PointCloud(scene["tp"])  # the same target without normals: they come as the host array
+        capi.check(capi.lib().b2_icp_factor_create(tgt.ctx.h, bare.h, tree.h, src.h, 1, capi.dptr(np.ascontiguousarray(tn)), C.byref(h)))
+        buf = np.zeros(capi.B2_LINEARIZED_DOUBLES)
+        capi.check(capi.lib().b2_factor_linearize(h, capi.dptr(delta), capi.dptr(buf)))
+        from_cloud.linearize({0: np.eye(4), 1: delta})
+        host = capi.unpack_linearized(buf)
+        assert all(np.array_equal(host[k], from_cloud._last[k]) for k in host), f"{normal_bytes}-byte normals"
+        capi.lib().b2_factor_destroy(h)
     with pytest.raises((capi.B2Error, ValueError)):
         g.IntegratedPointToPlaneICPFactor(0, 1, g.PointCloud(scene["tp"]), src, target_tree=tree)

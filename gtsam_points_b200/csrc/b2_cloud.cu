@@ -22,28 +22,11 @@
 namespace b2 {
 namespace {
 
-__device__ __forceinline__ unsigned long long encode_ordered(double v) {
-  unsigned long long b = static_cast<unsigned long long>(__double_as_longlong(v));
-  return (b & 0x8000000000000000ull) ? ~b : (b | 0x8000000000000000ull);
-}
-__host__ __device__ __forceinline__ double decode_ordered(unsigned long long e) {
-  unsigned long long b = (e & 0x8000000000000000ull) ? (e & 0x7fffffffffffffffull) : ~e;
-#ifdef __CUDA_ARCH__
-  return __longlong_as_double(static_cast<long long>(b));
-#else
-  double d;
-  memcpy(&d, &b, sizeof(d));
-  return d;
-#endif
-}
-
 struct ScanResult {
-  unsigned long long mins[3];
+  unsigned long long mins[3];  // encode_ordered images
   unsigned long long maxs[3];
   unsigned int flags;  // bit0: some coordinate not f32-exact, bit1: some cov entry not f32-exact, bit2: non-finite value
 };
-
-__device__ __forceinline__ bool f32_exact(double v) { return static_cast<double>(static_cast<float>(v)) == v; }
 
 // One pass over the raw arrays: bounding box + representability flags (pts == nullptr: covariances only).
 __global__ void scan_raw_kernel(const double* __restrict__ pts, int pstride, const double* __restrict__ covs, int cstride, size_t n,
@@ -424,8 +407,7 @@ b2_status b2_cloud_create_with_normals(b2_ctx* ctx, const double* points, int po
     if (!src) return B2_OK;
     *dst = src;  // n == 0: the host pointer marks that the cloud has the array; it is never read
     if (n == 0) return B2_OK;
-    B2_TRY(buf.alloc(n * stride * sizeof(double)));
-    B2_CUDA(cudaMemcpyAsync(buf.get(), src, n * stride * sizeof(double), cudaMemcpyHostToDevice, st));
+    B2_TRY(buf.upload(src, n * stride * sizeof(double), st));
     *dst = buf.as<const double>();
     return B2_OK;
   };
@@ -457,16 +439,9 @@ b2_status b2_cloud_create_voxelgrid(b2_ctx* ctx, double resolution, const double
   avg.point_stride = 3, avg.cov_stride = 9, avg.normal_stride = 3;
   if (n > 0) {
     DeviceBuffer raw_p, raw_c, raw_n, keys, keys2, vals, vals2, d_kept, tmp, starts;
-    B2_TRY(raw_p.alloc(n * point_stride * sizeof(double)));
-    B2_CUDA(cudaMemcpyAsync(raw_p.get(), points, n * point_stride * sizeof(double), cudaMemcpyHostToDevice, st));
-    if (covs) {
-      B2_TRY(raw_c.alloc(n * cov_stride * sizeof(double)));
-      B2_CUDA(cudaMemcpyAsync(raw_c.get(), covs, n * cov_stride * sizeof(double), cudaMemcpyHostToDevice, st));
-    }
-    if (normals) {
-      B2_TRY(raw_n.alloc(n * normal_stride * sizeof(double)));
-      B2_CUDA(cudaMemcpyAsync(raw_n.get(), normals, n * normal_stride * sizeof(double), cudaMemcpyHostToDevice, st));
-    }
+    B2_TRY(raw_p.upload(points, n * point_stride * sizeof(double), st));
+    if (covs) B2_TRY(raw_c.upload(covs, n * cov_stride * sizeof(double), st));
+    if (normals) B2_TRY(raw_n.upload(normals, n * normal_stride * sizeof(double), st));
     B2_TRY(keys.alloc(n * sizeof(unsigned long long)));
     B2_TRY(keys2.alloc(n * sizeof(unsigned long long)));
     B2_TRY(vals.alloc(n * sizeof(uint32_t)));

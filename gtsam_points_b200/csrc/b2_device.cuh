@@ -1,4 +1,4 @@
-// b2_device.cuh -- device helpers shared by the voxel-map and factor kernels.
+// b2_device.cuh -- device helpers shared by the voxel-map, kd-tree and factor kernels.
 #pragma once
 
 #include "b2_internal.hpp"
@@ -78,6 +78,31 @@ __device__ __forceinline__ int lookup_voxel(const VoxelBucket* __restrict__ buck
   }
 }
 
+// ---- neighbour searches (the kd-tree's, b2_kdtree.cuh, and the iVox's) ----
+
+// Squared distance (dx*dx + dy*dy) + dz*dz with individually rounded operations: the expression of the CPU path's kd-tree and of
+// FlatContainer::add / ::knn_search (flat_container.hpp:33-72; the w's of the homogeneous 4-vectors cancel), so that every
+// neighbour search gives the CPU's distances bit for bit.
+__device__ __forceinline__ double kd_sq_dist(double px, double py, double pz, double qx, double qy, double qz) {
+  const double dx = __dsub_rn(px, qx), dy = __dsub_rn(py, qy), dz = __dsub_rn(pz, qz);
+  return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+}
+
+// A k-NN candidate list with KnnResult semantics (knn_result.hpp:84-109): slot i is (dist[i * stride], idx[i * stride]), sorted by
+// distance, unfilled slots hold (max_sq, -1).  A candidate enters iff d < dist[(k - 1) * stride] -- the caller tests that, against
+// a copy of the worst it may keep in a register -- and is placed after every stored candidate whose distance is <= d (stable); the
+// last slot drops out.
+template <typename Index>
+__device__ __forceinline__ void knn_insert(double* __restrict__ dist, Index* __restrict__ idx, int k, int stride, double d, Index j) {
+  int pos = k - 1;
+  for (; pos > 0 && d < dist[(pos - 1) * stride]; pos--) {
+    dist[pos * stride] = dist[(pos - 1) * stride];
+    idx[pos * stride] = idx[(pos - 1) * stride];
+  }
+  dist[pos * stride] = d;
+  idx[pos * stride] = j;
+}
+
 // ---- iVox (IncrementalVoxelMap<FlatContainer>) ----
 constexpr int kIvoxMaxPointsInCell = B2_IVOX_MAX_POINTS_IN_CELL;
 
@@ -107,13 +132,6 @@ __host__ __device__ __forceinline__ void ivox_offset(int mode, int t, int& dx, i
   }
 }
 
-// (stored - query).squaredNorm() over the homogeneous 4-vectors (the w's cancel): ((d0^2 + d1^2) + d2^2) with individually
-// rounded operations -- the expression of the oracle's kd-tree (FlatContainer::add / ::knn_search, flat_container.hpp:33-72)
-__device__ __forceinline__ double ivox_sq_dist(double px, double py, double pz, double qx, double qy, double qz) {
-  const double dx = __dsub_rn(px, qx), dy = __dsub_rn(py, qy), dz = __dsub_rn(pz, qz);
-  return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
-}
-
 // What a neighbour search in an iVox needs: its voxel table, its point records (slots per voxel, in voxel id order), the points
 // stored per voxel, and the neighbour voxel mode.
 struct IvoxView {
@@ -124,13 +142,13 @@ struct IvoxView {
   int mode;  // 1, 7, 19 or 27
 };
 
-// Nearest stored point of an iVox to q within max_sq (KnnResult<1>: strict '<', ties to the first point visited -- neighbour
-// voxels in offset order, points in slot order).  Returns the record id voxel * slots + slot, or -1.
-__device__ __forceinline__ int ivox_nn1(const IvoxView& iv, double qx, double qy, double qz, double max_sq, double* out_sq) {
+// The iVox neighbour walk (IncrementalVoxelMap::knn_search, incremental_voxelmap_impl.hpp:71-92): visit(d, v, s) for every point
+// stored in the neighbour voxels of q -- voxels in offset order, then the voxel's points in slot order -- with d its squared
+// distance to q.  A voxel the table does not hold is skipped, so an empty map (every bucket empty) visits nothing.
+template <typename Visit>
+__device__ __forceinline__ void ivox_visit(const IvoxView& iv, double qx, double qy, double qz, Visit&& visit) {
   const double inv_leaf = iv.table.inv_leaf;
   const int cx = voxel_coord1(qx, inv_leaf), cy = voxel_coord1(qy, inv_leaf), cz = voxel_coord1(qz, inv_leaf);
-  double best = max_sq;
-  int best_id = -1;
 #pragma unroll 1
   for (int t = 0; t < iv.mode; t++) {
     int dx, dy, dz;
@@ -143,13 +161,22 @@ __device__ __forceinline__ int ivox_nn1(const IvoxView& iv, double qx, double qy
     for (int s = 0; s < c; s++) {
       const double* r = iv.records + static_cast<size_t>(first + s) * kRecordDoubles;
       const double2 xy = __ldg(reinterpret_cast<const double2*>(r));
-      const double d = ivox_sq_dist(xy.x, xy.y, __ldg(r + 2), qx, qy, qz);
-      if (d < best) {
-        best = d;
-        best_id = first + s;
-      }
+      visit(kd_sq_dist(xy.x, xy.y, __ldg(r + 2), qx, qy, qz), v, s);
     }
   }
+}
+
+// Nearest stored point of an iVox to q within max_sq (KnnResult<1>: strict '<', ties to the first point visited).  Returns the
+// record id voxel * slots + slot, or -1.
+__device__ __forceinline__ int ivox_nn1(const IvoxView& iv, double qx, double qy, double qz, double max_sq, double* out_sq) {
+  double best = max_sq;
+  int best_id = -1;
+  ivox_visit(iv, qx, qy, qz, [&](double d, int v, int s) {
+    if (d < best) {
+      best = d;
+      best_id = v * iv.slots + s;
+    }
+  });
   if (out_sq) *out_sq = best;
   return best_id;
 }

@@ -8,6 +8,7 @@
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
+#include <cstring>
 #include <initializer_list>
 #include <string>
 #include <utility>
@@ -77,6 +78,12 @@ class DeviceBuffer {
     p_ = nullptr;
     bytes_ = 0;
   }
+  // alloc(bytes), then an asynchronous copy of `bytes` from the host pointer `src` on `st`
+  b2_status upload(const void* src, size_t bytes, cudaStream_t st) {
+    B2_TRY(alloc(bytes));
+    B2_CUDA(cudaMemcpyAsync(p_, src, bytes, cudaMemcpyHostToDevice, st));
+    return B2_OK;
+  }
   void* get() const { return p_; }
   template <typename T>
   T* as() const {
@@ -135,6 +142,26 @@ auto with_storage(int bytes, Fn&& fn) {
   if (bytes == 8) return fn(double{});
   return fn(float{});
 }
+
+// Order-preserving image of a double: unsigned comparison of the images orders the doubles as < does (-0 before +0), so atomicMin /
+// atomicMax on images fold bounding boxes and the images sort as 64-bit keys.
+__device__ __forceinline__ unsigned long long encode_ordered(double v) {
+  const unsigned long long b = static_cast<unsigned long long>(__double_as_longlong(v));
+  return (b & 0x8000000000000000ull) ? ~b : (b | 0x8000000000000000ull);
+}
+__host__ __device__ __forceinline__ double decode_ordered(unsigned long long e) {
+  const unsigned long long b = (e & 0x8000000000000000ull) ? (e & 0x7fffffffffffffffull) : ~e;
+#ifdef __CUDA_ARCH__
+  return __longlong_as_double(static_cast<long long>(b));
+#else
+  double d;
+  std::memcpy(&d, &b, sizeof(d));
+  return d;
+#endif
+}
+
+// v survives the round trip through float32 unchanged: the test behind every float32 storage choice (cloud planes, kd-tree leaves)
+__device__ __forceinline__ bool f32_exact(double v) { return static_cast<double>(static_cast<float>(v)) == v; }
 
 inline size_t round_up(size_t x, size_t m) { return (x + m - 1) / m * m; }
 inline uint64_t next_pow2(uint64_t x) {
@@ -202,6 +229,13 @@ struct alignas(16) KdNodeGPU {
   double thresh;
   uint32_t a;
   uint32_t b;
+};
+
+// What a kd-tree search needs (b2_kdtree::view()): the nodes and the points in leaf order.
+struct KdTreeView {
+  const KdNodeGPU* nodes;
+  const void* leaf_points;  // float4[n] (f32 != 0) or double4-as-2x-double2[n] records in leaf order
+  int f32;
 };
 
 // ---- cloud assembly (b2_cloud.cu) ------------------------------------------------------------------
@@ -314,6 +348,7 @@ struct b2_kdtree {
   size_t n_pad = 0;
   b2::DeviceBuffer d_leaf_index;   // uint32: leaf position -> caller index
   uint64_t cloud_uid = 0;          // b2_cloud::uid of the cloud the tree was built from (0: built from host points)
+  b2::KdTreeView view() const { return {d_nodes.as<const b2::KdNodeGPU>(), d_leaf_points.get(), leaf_f32 ? 1 : 0}; }
 };
 
 // B2_FACTOR_VGICP_VALIDATED names a kernel instantiation only (a VGICP factor with surface validation on, launch_kind below);

@@ -19,7 +19,6 @@
 #include <algorithm>
 #include <climits>
 #include <cmath>
-#include <cstring>
 #include <memory>
 #include <vector>
 
@@ -31,17 +30,6 @@ namespace b2 {
 namespace {
 
 constexpr int kMaxLeaf = 16;
-
-// order-preserving map double -> uint64 (sort keys, atomicMin / atomicMax on coordinates)
-__host__ __device__ __forceinline__ unsigned long long ordered_bits(double v) {
-  unsigned long long b;
-#ifdef __CUDA_ARCH__
-  b = static_cast<unsigned long long>(__double_as_longlong(v));
-#else
-  std::memcpy(&b, &v, sizeof(b));
-#endif
-  return (b & 0x8000000000000000ull) ? ~b : (b | 0x8000000000000000ull);
-}
 
 struct Range {
   uint32_t first, last;
@@ -71,7 +59,7 @@ __global__ void scan_points_kernel(const double* __restrict__ pts, int stride, s
 #pragma unroll
     for (int a = 0; a < 3; a++) {
       const double v = pts[i * stride + a];
-      lossy |= static_cast<double>(static_cast<float>(v)) != v;
+      lossy |= !f32_exact(v);
       bad |= !isfinite(v);
     }
   }
@@ -99,15 +87,10 @@ __global__ void bbox_level_kernel(const double* __restrict__ pts, int stride, si
   unsigned long long* b = bbox + static_cast<size_t>(rank[k]) * 6;
 #pragma unroll
   for (int a = 0; a < 3; a++) {
-    const unsigned long long o = ordered_bits(p[a]);
+    const unsigned long long o = encode_ordered(p[a]);
     atomicMin(&b[a], o);
     atomicMax(&b[3 + a], o);
   }
-}
-
-__device__ __forceinline__ double from_ordered_bits_dev(unsigned long long o) {
-  const unsigned long long b = (o & 0x8000000000000000ull) ? (o & 0x7fffffffffffffffull) : ~o;
-  return __longlong_as_double(static_cast<long long>(b));
 }
 
 // per internal node (indexed by rank): axis of largest extent + the segment it occupies in `order`
@@ -119,7 +102,7 @@ __global__ void axis_level_kernel(const Range* __restrict__ level, uint32_t coun
   const unsigned long long* b = bbox + static_cast<size_t>(r) * 6;
   double ext[3];
 #pragma unroll
-  for (int a = 0; a < 3; a++) ext[a] = from_ordered_bits_dev(b[3 + a]) - from_ordered_bits_dev(b[a]);
+  for (int a = 0; a < 3; a++) ext[a] = decode_ordered(b[3 + a]) - decode_ordered(b[a]);
   int ax = 0;
   if (ext[1] > ext[ax]) ax = 1;
   if (ext[2] > ext[ax]) ax = 2;
@@ -134,7 +117,7 @@ __global__ void keys_level_kernel(const double* __restrict__ pts, int stride, si
   const size_t pos = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
   if (pos >= n) return;
   const int k = find_range(level, count, static_cast<uint32_t>(pos));
-  keys[pos] = (k >= 0 && flag[k]) ? ordered_bits(pts[static_cast<size_t>(order[pos]) * stride + axis[rank[k]]]) : 0ull;
+  keys[pos] = (k >= 0 && flag[k]) ? encode_ordered(pts[static_cast<size_t>(order[pos]) * stride + axis[rank[k]]]) : 0ull;
 }
 
 __global__ void emit_level_kernel(const double* __restrict__ pts, int stride, const uint32_t* __restrict__ order_sorted, const Range* __restrict__ level, uint32_t count,
@@ -187,24 +170,34 @@ __global__ void knn1_kernel(KdTreeView tree, const double* __restrict__ q, int q
 }
 
 // ---- k nearest neighbours (k <= B2_KNN_MAX_K) and covariance estimation on top of it ------------------------------------
-constexpr int kKnnWarps = 4;  // warps per CTA of the k-NN kernels (scratch: k x 32 x 12 bytes per warp)
+constexpr int kKnnWarps = 4;  // warps per CTA of the k-NN kernels
+
+// The k-NN kernels' dynamic shared memory: the k-NN lists of all kKnnWarps x 32 lanes, [warp][slot][lane] distances, then the
+// indices in the same layout.  knn_scratch gives a lane its column of both (slot j at [j * 32]).
+size_t knn_smem_bytes(int k) { return static_cast<size_t>(kKnnWarps) * k * 32 * (sizeof(double) + sizeof(int)); }
+__device__ __forceinline__ void knn_scratch(int k, int warp, int lane, double*& dist, int*& idx) {
+  extern __shared__ __align__(16) unsigned char knn_smem[];
+  const size_t col = static_cast<size_t>(warp) * k * 32 + lane;
+  dist = reinterpret_cast<double*>(knn_smem) + col;
+  idx = reinterpret_cast<int*>(reinterpret_cast<double*>(knn_smem) + static_cast<size_t>(kKnnWarps) * k * 32) + col;
+}
 
 // queries: device array nq x stride.  out_index / out_sq_dist: nq x k, sorted by distance, (-1, max_sq) beyond the number found.
 __global__ void __launch_bounds__(kKnnWarps * 32) knn_kernel(KdTreeView view, const double* __restrict__ q, int stride, size_t nq, int k, double max_sq,
                                                              const uint32_t* __restrict__ leaf_index, long long* __restrict__ out_index, double* __restrict__ out_sq) {
-  extern __shared__ __align__(16) unsigned char knn_smem[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  double* sdist = reinterpret_cast<double*>(knn_smem) + static_cast<size_t>(warp) * k * 32;
-  int* sidx = reinterpret_cast<int*>(reinterpret_cast<double*>(knn_smem) + static_cast<size_t>(kKnnWarps) * k * 32) + static_cast<size_t>(warp) * k * 32;
+  double* sdist;
+  int* sidx;
+  knn_scratch(k, warp, lane, sdist, sidx);
   const size_t i = (blockIdx.x * static_cast<size_t>(kKnnWarps) + warp) * 32 + lane;
   const bool active = i < nq;
   const size_t ii = active ? i : 0;
-  kdtree_knn_warp(view, q[ii * stride], q[ii * stride + 1], q[ii * stride + 2], active, k, max_sq, sdist, sidx, lane);
+  kdtree_knn_warp(view, q[ii * stride], q[ii * stride + 1], q[ii * stride + 2], active, k, max_sq, sdist, sidx);
   if (!active) return;
   for (int j = 0; j < k; j++) {
-    const int s = sidx[j * 32 + lane];
+    const int s = sidx[j * 32];
     out_index[i * k + j] = s < 0 ? -1ll : static_cast<long long>(leaf_index[s]);
-    out_sq[i * k + j] = sdist[j * 32 + lane];
+    out_sq[i * k + j] = sdist[j * 32];
   }
 }
 
@@ -302,28 +295,18 @@ template <bool NORMALS>
 __global__ void __launch_bounds__(kKnnWarps * 32) covariance_kernel(KdTreeView view, size_t n, int k, double ev0, double ev1, double ev2,
                                                                     const uint32_t* __restrict__ leaf_index, double* __restrict__ out_cov /* n x 9, caller order */,
                                                                     double* __restrict__ out_normals /* n x 3, caller order (NORMALS only) */) {
-  extern __shared__ __align__(16) unsigned char knn_smem[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  double* sdist = reinterpret_cast<double*>(knn_smem) + static_cast<size_t>(warp) * k * 32;
-  int* sidx = reinterpret_cast<int*>(reinterpret_cast<double*>(knn_smem) + static_cast<size_t>(kKnnWarps) * k * 32) + static_cast<size_t>(warp) * k * 32;
+  double* sdist;
+  int* sidx;
+  knn_scratch(k, warp, lane, sdist, sidx);
   const size_t i = (blockIdx.x * static_cast<size_t>(kKnnWarps) + warp) * 32 + lane;
   const bool active = i < n;
-  auto point = [&](size_t j, double& x, double& y, double& z) {
-    if (view.f32) {
-      const float4 p = __ldg(static_cast<const float4*>(view.leaf_points) + j);
-      x = p.x, y = p.y, z = p.z;
-    } else {
-      const double2* pp = static_cast<const double2*>(view.leaf_points) + 2 * j;
-      const double2 a = __ldg(pp), b = __ldg(pp + 1);
-      x = a.x, y = a.y, z = b.x;
-    }
-  };
-  double qx = 0, qy = 0, qz = 0;
-  if (active) point(i, qx, qy, qz);
-  kdtree_knn_warp(view, qx, qy, qz, active, k, 1.7976931348623157e308, sdist, sidx, lane);
+  const double3 q = active ? leaf_point(view, i) : make_double3(0.0, 0.0, 0.0);
+  const double qx = q.x, qy = q.y, qz = q.z;
+  kdtree_knn_warp(view, qx, qy, qz, active, k, 1.7976931348623157e308, sdist, sidx);
   if (!active) return;
   double* out = out_cov + static_cast<size_t>(leaf_index[i]) * 9;
-  if (sidx[(k - 1) * 32 + lane] < 0) {  // fewer than k neighbours: identity (covariance_estimation.cpp:27-31)
+  if (sidx[(k - 1) * 32] < 0) {  // fewer than k neighbours: identity (covariance_estimation.cpp:27-31)
 #pragma unroll
     for (int a = 0; a < 9; a++) out[a] = (a % 4 == 0) ? 1.0 : 0.0;
     if (NORMALS) store_normal_of(out, 3, qx, qy, qz, out_normals + static_cast<size_t>(leaf_index[i]) * 3);
@@ -331,8 +314,8 @@ __global__ void __launch_bounds__(kKnnWarps * 32) covariance_kernel(KdTreeView v
   }
   double sp[3] = {0, 0, 0}, sc[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}};
   for (int j = 0; j < k; j++) {
-    double p[3];
-    point(static_cast<size_t>(sidx[j * 32 + lane]), p[0], p[1], p[2]);
+    const double3 pj = leaf_point(view, static_cast<size_t>(sidx[j * 32]));
+    const double p[3] = {pj.x, pj.y, pj.z};
 #pragma unroll
     for (int a = 0; a < 3; a++) {
       sp[a] = __dadd_rn(sp[a], p[a]);
@@ -372,70 +355,19 @@ __global__ void normals_from_covs_kernel(const double* __restrict__ pts, int pst
 }
 
 // ---- radius search ----------------------------------------------------------------------------------------------------
-// The packet walk of kdtree_knn_warp with a fixed per-lane limit r2 (0 for inactive lanes) in place of the k-th best distance:
-// a node is visited iff some lane has limit > bound, and hit(d, j) is called for every leaf position j with squared distance
-// d < r2 (small_kdtree.hpp:480-523), in traversal order.  The walk depends only on the warp's queries, so two passes over
-// the same queries see the same hits in the same order.
-template <typename Hit>
-__device__ __forceinline__ void kdtree_radius_warp(const KdTreeView& t, double qx, double qy, double qz, bool active, double r2, Hit&& hit) {
-  constexpr unsigned kFull = 0xffffffffu;
-  uint32_t stack_node[kKdStackDepth];
-  double stack_bound[kKdStackDepth];
-  int sp = 0;
-  const double lim = active ? r2 : 0.0;
-  uint32_t node_idx = 0;
-  double bound = 0.0;
-  while (true) {
-    if (__any_sync(kFull, lim > bound)) {
-      const KdNodeGPU n = load_node(t.nodes + node_idx);  // warp-uniform address
-      if (n.b < 4u) {
-        const double qa = n.b == 0u ? qx : (n.b == 1u ? qy : qz);
-        const double diff = __dsub_rn(qa, n.thresh);
-        const double d2 = __dmul_rn(diff, diff);
-        const bool left = diff < 0.0;
-        const bool need = lim > bound;
-        const int nl = __popc(__ballot_sync(kFull, need && left)), nr = __popc(__ballot_sync(kFull, need && !left));
-        const bool go_left = nl >= nr;
-        const bool mine = (left == go_left);
-        const double sep = bound > d2 ? bound : d2;
-        stack_node[sp] = go_left ? n.a + 1u : n.a;
-        stack_bound[sp] = mine ? sep : bound;
-        sp++;
-        node_idx = go_left ? n.a : n.a + 1u;
-        bound = mine ? bound : sep;
-        continue;
-      }
-      const uint32_t first = n.a, cnt = n.b - 4u;
-      if (t.f32) {
-        const float4* __restrict__ pts = static_cast<const float4*>(t.leaf_points);
-        for (uint32_t j = first; j < first + cnt; j++) {
-          const float4 p = __ldg(pts + j);
-          const double d = kd_sq_dist(static_cast<double>(p.x), static_cast<double>(p.y), static_cast<double>(p.z), qx, qy, qz);
-          if (d < lim) hit(d, j);
-        }
-      } else {
-        const double2* __restrict__ pts = static_cast<const double2*>(t.leaf_points);
-        for (uint32_t j = first; j < first + cnt; j++) {
-          const double2 a = __ldg(pts + 2 * static_cast<size_t>(j)), b = __ldg(pts + 2 * static_cast<size_t>(j) + 1);
-          const double d = kd_sq_dist(a.x, a.y, b.x, qx, qy, qz);
-          if (d < lim) hit(d, j);
-        }
-      }
-    }
-    if (sp == 0) break;
-    sp--;
-    node_idx = stack_node[sp];
-    bound = stack_bound[sp];
-  }
-}
+// Two passes of the walk over the same queries with the fixed limit r2 (0 for a lane without a query), so both see the same
+// hits -- points with squared distance d < r2 (small_kdtree.hpp:480-523) -- in the same order.
 
 // pass 1: the number of points inside the radius of every query
 __global__ void radius_count_kernel(KdTreeView view, const double* __restrict__ q, int stride, size_t nq, double r2, unsigned long long* __restrict__ count) {
   const size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
   const bool active = i < nq;
   const size_t ii = active ? i : 0;
+  const double lim = active ? r2 : 0.0;
   unsigned long long c = 0;
-  kdtree_radius_warp(view, q[ii * stride], q[ii * stride + 1], q[ii * stride + 2], active, r2, [&](double, uint32_t) { c++; });
+  kdtree_walk_warp(view, q[ii * stride], q[ii * stride + 1], q[ii * stride + 2], [&] { return lim; }, [&](double d, uint32_t) {
+    if (d < lim) c++;
+  });
   if (active) count[i] = c;
 }
 
@@ -445,11 +377,14 @@ __global__ void radius_fill_kernel(KdTreeView view, const double* __restrict__ q
   const size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
   const bool active = i < nq;
   const size_t ii = active ? i : 0;
+  const double lim = active ? r2 : 0.0;
   unsigned long long pos = active ? offset[i] : 0;
-  kdtree_radius_warp(view, q[ii * stride], q[ii * stride + 1], q[ii * stride + 2], active, r2, [&](double d, uint32_t j) {
-    hit_index[pos] = leaf_index[j];
-    hit_sq[pos] = d;
-    pos++;
+  kdtree_walk_warp(view, q[ii * stride], q[ii * stride + 1], q[ii * stride + 2], [&] { return lim; }, [&](double d, uint32_t j) {
+    if (d < lim) {
+      hit_index[pos] = leaf_index[j];
+      hit_sq[pos] = d;
+      pos++;
+    }
   });
 }
 
@@ -465,10 +400,6 @@ __global__ void radius_gather_kernel(size_t nq, const unsigned long long* __rest
     out_sq[dst + r] = hit_sq[src + r];
   }
 }
-
-size_t knn_smem_bytes(int k) { return static_cast<size_t>(kKnnWarps) * k * 32 * (sizeof(double) + sizeof(int)); }
-
-KdTreeView tree_view(const b2_kdtree* t) { return KdTreeView{t->d_nodes.as<const KdNodeGPU>(), t->d_leaf_points.get(), t->leaf_f32 ? 1 : 0}; }
 
 }  // namespace
 }  // namespace b2
@@ -488,10 +419,9 @@ b2_status build_tree(b2_ctx* ctx, const double* dp, int point_stride, size_t n, 
 
   if (n == 0) {  // an empty tree: one empty leaf
     const KdNodeGPU root{0.0, 0u, 4u};
-    B2_TRY(t->d_nodes.alloc(sizeof(KdNodeGPU)));
+    B2_TRY(t->d_nodes.upload(&root, sizeof(root), st));
     B2_TRY(t->d_leaf_points.alloc(32));
     B2_TRY(t->d_leaf_index.alloc(sizeof(uint32_t)));
-    B2_CUDA(cudaMemcpyAsync(t->d_nodes.get(), &root, sizeof(root), cudaMemcpyHostToDevice, st));
     B2_CUDA(cudaStreamSynchronize(st));
     t->num_nodes = 1;
     t->leaf_f32 = true;
@@ -600,10 +530,7 @@ b2_status b2_kdtree_create(b2_ctx* ctx, const double* points, int point_stride, 
   B2_REQUIRE(n < (1ull << 31), "b2_kdtree_create: at most 2^31-1 points");
   B2_CUDA(cudaSetDevice(ctx->device));
   DeviceBuffer d_pts;
-  if (n > 0) {
-    B2_TRY(d_pts.alloc(n * point_stride * sizeof(double)));
-    B2_CUDA(cudaMemcpyAsync(d_pts.get(), points, n * point_stride * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-  }
+  if (n > 0) B2_TRY(d_pts.upload(points, n * point_stride * sizeof(double), ctx->stream));
   return build_tree(ctx, d_pts.as<const double>(), point_stride, n, out);
 }
 
@@ -640,11 +567,10 @@ b2_status b2_kdtree_knn1(const b2_kdtree* t, const double* queries, int query_st
   B2_CUDA(cudaSetDevice(t->ctx->device));
   cudaStream_t st = t->ctx->stream;
   DeviceBuffer dq, di, ds;
-  B2_TRY(dq.alloc(nq * query_stride * sizeof(double)));
+  B2_TRY(dq.upload(queries, nq * query_stride * sizeof(double), st));
   B2_TRY(di.alloc(nq * sizeof(long long)));
   B2_TRY(ds.alloc(nq * sizeof(double)));
-  B2_CUDA(cudaMemcpyAsync(dq.get(), queries, nq * query_stride * sizeof(double), cudaMemcpyHostToDevice, st));
-  knn1_kernel<<<static_cast<unsigned>((nq + 127) / 128), 128, 0, st>>>(tree_view(t), dq.as<const double>(), query_stride, nq, max_sq_dist, t->d_leaf_index.as<const uint32_t>(),
+  knn1_kernel<<<static_cast<unsigned>((nq + 127) / 128), 128, 0, st>>>(t->view(), dq.as<const double>(), query_stride, nq, max_sq_dist, t->d_leaf_index.as<const uint32_t>(),
                                                                       di.as<long long>(), ds.as<double>());
   B2_CUDA(cudaGetLastError());
   if (out_index) B2_CUDA(cudaMemcpyAsync(out_index, di.get(), nq * sizeof(long long), cudaMemcpyDeviceToHost, st));
@@ -664,20 +590,12 @@ b2_status b2_kdtree_knn(const b2_kdtree* t, const double* queries, int query_str
   B2_CUDA(cudaSetDevice(t->ctx->device));
   cudaStream_t st = t->ctx->stream;
   DeviceBuffer dq, di, ds;
-  B2_TRY(dq.alloc(nq * query_stride * sizeof(double)));
+  B2_TRY(dq.upload(queries, nq * query_stride * sizeof(double), st));
   B2_TRY(di.alloc(nq * k * sizeof(long long)));
   B2_TRY(ds.alloc(nq * k * sizeof(double)));
-  B2_CUDA(cudaMemcpyAsync(dq.get(), queries, nq * query_stride * sizeof(double), cudaMemcpyHostToDevice, st));
   const size_t smem = knn_smem_bytes(k);
   B2_CUDA(cudaFuncSetAttribute(reinterpret_cast<const void*>(knn_kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-  if (t->n == 0) {
-    std::vector<long long> idx(nq * k, -1);
-    std::vector<double> sq(nq * k, max_sq_dist);
-    if (out_index) std::memcpy(out_index, idx.data(), idx.size() * sizeof(long long));
-    if (out_sq_dist) std::memcpy(out_sq_dist, sq.data(), sq.size() * sizeof(double));
-    return B2_OK;
-  }
-  knn_kernel<<<static_cast<unsigned>((nq + kKnnWarps * 32 - 1) / (kKnnWarps * 32)), kKnnWarps * 32, smem, st>>>(tree_view(t), dq.as<const double>(), query_stride, nq, k, max_sq_dist,
+  knn_kernel<<<static_cast<unsigned>((nq + kKnnWarps * 32 - 1) / (kKnnWarps * 32)), kKnnWarps * 32, smem, st>>>(t->view(), dq.as<const double>(), query_stride, nq, k, max_sq_dist,
                                                                                                              t->d_leaf_index.as<const uint32_t>(), di.as<long long>(), ds.as<double>());
   B2_CUDA(cudaGetLastError());
   if (out_index) B2_CUDA(cudaMemcpyAsync(out_index, di.get(), nq * k * sizeof(long long), cudaMemcpyDeviceToHost, st));
@@ -703,14 +621,13 @@ b2_status b2_kdtree_radius_search(const b2_kdtree* t, const double* queries, int
   const double r2 = radius * radius;
   const unsigned grid = static_cast<unsigned>((nq + 127) / 128);
   DeviceBuffer dq, dcount, doff, dscan;
-  B2_TRY(dq.alloc(nq * query_stride * sizeof(double)));
+  B2_TRY(dq.upload(queries, nq * query_stride * sizeof(double), st));
   B2_TRY(dcount.alloc((nq + 1) * sizeof(unsigned long long)));
   B2_TRY(doff.alloc((nq + 1) * sizeof(unsigned long long)));
   unsigned long long* count = dcount.as<unsigned long long>();
   unsigned long long* off = doff.as<unsigned long long>();
-  B2_CUDA(cudaMemcpyAsync(dq.get(), queries, nq * query_stride * sizeof(double), cudaMemcpyHostToDevice, st));
   B2_CUDA(cudaMemsetAsync(count + nq, 0, sizeof(unsigned long long), st));  // offset[nq] = total
-  radius_count_kernel<<<grid, 128, 0, st>>>(tree_view(t), dq.as<const double>(), query_stride, nq, r2, count);
+  radius_count_kernel<<<grid, 128, 0, st>>>(t->view(), dq.as<const double>(), query_stride, nq, r2, count);
   B2_CUDA(cudaGetLastError());
   B2_TRY(cub_run(dscan, st, [&](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, count, off, static_cast<int>(nq + 1), st); }));
   std::vector<unsigned long long> h_off(nq + 1);
@@ -732,7 +649,7 @@ b2_status b2_kdtree_radius_search(const b2_kdtree* t, const double* queries, int
     B2_TRY(hit_idx[b].alloc(total * sizeof(uint32_t)));
     B2_TRY(hit_sq[b].alloc(total * sizeof(double)));
   }
-  radius_fill_kernel<<<grid, 128, 0, st>>>(tree_view(t), dq.as<const double>(), query_stride, nq, r2, off, t->d_leaf_index.as<const uint32_t>(), hit_idx[0].as<uint32_t>(),
+  radius_fill_kernel<<<grid, 128, 0, st>>>(t->view(), dq.as<const double>(), query_stride, nq, r2, off, t->d_leaf_index.as<const uint32_t>(), hit_idx[0].as<uint32_t>(),
                                            hit_sq[0].as<double>());
   B2_CUDA(cudaGetLastError());
   const int items = static_cast<int>(total), segs = static_cast<int>(nq);
@@ -770,7 +687,7 @@ b2_status launch_covariances(const b2_kdtree* t, int k_neighbors, const double* 
   const size_t smem = knn_smem_bytes(k_neighbors);
   const auto kernel = d_normals ? covariance_kernel<true> : covariance_kernel<false>;
   B2_CUDA(cudaFuncSetAttribute(reinterpret_cast<const void*>(kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-  kernel<<<static_cast<unsigned>((n + kKnnWarps * 32 - 1) / (kKnnWarps * 32)), kKnnWarps * 32, smem, t->ctx->stream>>>(tree_view(t), n, k_neighbors, ev[0], ev[1], ev[2],
+  kernel<<<static_cast<unsigned>((n + kKnnWarps * 32 - 1) / (kKnnWarps * 32)), kKnnWarps * 32, smem, t->ctx->stream>>>(t->view(), n, k_neighbors, ev[0], ev[1], ev[2],
                                                                                                                   t->d_leaf_index.as<const uint32_t>(), d_cov, d_normals);
   B2_CUDA(cudaGetLastError());
   return B2_OK;
@@ -849,11 +766,9 @@ b2_status b2_estimate_normals_from_covs(b2_ctx* ctx, const double* points, int p
   B2_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   DeviceBuffer dp, dc, dn;
-  B2_TRY(dp.alloc(n * point_stride * sizeof(double)));
-  B2_TRY(dc.alloc(n * cov_stride * sizeof(double)));
+  B2_TRY(dp.upload(points, n * point_stride * sizeof(double), st));
+  B2_TRY(dc.upload(covs, n * cov_stride * sizeof(double), st));
   B2_TRY(dn.alloc(n * 3 * sizeof(double)));
-  B2_CUDA(cudaMemcpyAsync(dp.get(), points, n * point_stride * sizeof(double), cudaMemcpyHostToDevice, st));
-  B2_CUDA(cudaMemcpyAsync(dc.get(), covs, n * cov_stride * sizeof(double), cudaMemcpyHostToDevice, st));
   normals_from_covs_kernel<<<static_cast<unsigned>((n + 127) / 128), 128, 0, st>>>(dp.as<const double>(), point_stride, dc.as<const double>(), cov_stride, n, dn.as<double>());
   B2_CUDA(cudaGetLastError());
   B2_CUDA(cudaMemcpyAsync(out_normals, dn.get(), n * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));

@@ -149,7 +149,7 @@ struct FlatCell {
       const size_t i = b.idx[j];
       const double* p = b.pts + i * b.pstride;
       bool reject = false;
-      for (int q = 0; q < cnt && !reject; q++) reject = ivox_sq_dist(rec[q * kRecordDoubles + 0], rec[q * kRecordDoubles + 1], rec[q * kRecordDoubles + 2], p[0], p[1], p[2]) < min_sq;
+      for (int q = 0; q < cnt && !reject; q++) reject = kd_sq_dist(rec[q * kRecordDoubles + 0], rec[q * kRecordDoubles + 1], rec[q * kRecordDoubles + 2], p[0], p[1], p[2]) < min_sq;
       if (reject) continue;
       double* o = rec + static_cast<size_t>(cnt) * kRecordDoubles;
       o[0] = p[0], o[1] = p[1], o[2] = p[2];
@@ -209,38 +209,17 @@ __global__ void lru_compact_kernel(const uint32_t* __restrict__ keep, const uint
 }
 
 // IncrementalVoxelMap::knn_search (incremental_voxelmap_impl.hpp:71-92) with KnnResult<-1> (knn_result.hpp:84-109): one thread per
-// query, neighbour voxels in offset order, points in slot order, strict '<' against the current worst, stable insertion.
-__global__ void ivox_knn_kernel(const double* __restrict__ q, int qstride, size_t nq, int k, double max_sq, const IvoxView iv, size_t num_voxels,
-                                long long* __restrict__ out_idx, double* __restrict__ out_sq) {
+// query, the iVox neighbour walk into the query's k-NN list, which lives in the output rows.
+__global__ void ivox_knn_kernel(const double* __restrict__ q, int qstride, size_t nq, int k, double max_sq, const IvoxView iv, long long* __restrict__ out_idx,
+                                double* __restrict__ out_sq) {
   const size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
   if (i >= nq) return;
   long long* idx = out_idx + i * k;
   double* sq = out_sq + i * k;
   for (int j = 0; j < k; j++) idx[j] = -1, sq[j] = max_sq;
-  if (num_voxels == 0) return;
-  const double qx = q[i * qstride], qy = q[i * qstride + 1], qz = q[i * qstride + 2];
-  const int cx = voxel_coord1(qx, iv.table.inv_leaf), cy = voxel_coord1(qy, iv.table.inv_leaf), cz = voxel_coord1(qz, iv.table.inv_leaf);
-  int found = 0;
-  for (int t = 0; t < iv.mode; t++) {
-    int dx, dy, dz;
-    ivox_offset(iv.mode, t, dx, dy, dz);
-    const int v = lookup_voxel(iv.table.buckets, iv.table.group_mask, cx + dx, cy + dy, cz + dz);
-    if (v < 0) continue;
-    const int c = static_cast<int>(iv.counts[v]);
-    const double* rec = iv.records + static_cast<size_t>(v) * iv.slots * kRecordDoubles;
-    for (int s = 0; s < c; s++) {
-      const double d = ivox_sq_dist(rec[s * kRecordDoubles], rec[s * kRecordDoubles + 1], rec[s * kRecordDoubles + 2], qx, qy, qz);
-      if (d >= sq[k - 1]) continue;
-      int loc = min(found, k - 1);
-      for (; loc > 0 && d < sq[loc - 1]; loc--) {
-        idx[loc] = idx[loc - 1];
-        sq[loc] = sq[loc - 1];
-      }
-      idx[loc] = (static_cast<long long>(v) << 32) | s;
-      sq[loc] = d;
-      found = min(found + 1, k);
-    }
-  }
+  ivox_visit(iv, q[i * qstride], q[i * qstride + 1], q[i * qstride + 2], [&](double d, int v, int s) {
+    if (d < sq[k - 1]) knn_insert(sq, idx, k, 1, d, (static_cast<long long>(v) << 32) | s);
+  });
 }
 
 __global__ void insert_buckets_kernel(const int32_t* __restrict__ coords, size_t num_voxels, VoxelBucket* __restrict__ buckets, uint32_t mask) {
@@ -499,10 +478,8 @@ b2_status segment_batch(b2_voxelmap* vm, const double* points, int point_stride,
   cudaStream_t st = vm->ctx->stream;
   const double inv_leaf = vm->inv_resolution;
   const size_t V_old = vm->num_voxels;
-  B2_TRY(s.raw_p.alloc(n * point_stride * sizeof(double)));
-  if (covs) B2_TRY(s.raw_c.alloc(n * cov_stride * sizeof(double)));
-  B2_CUDA(cudaMemcpyAsync(s.raw_p.get(), points, n * point_stride * sizeof(double), cudaMemcpyHostToDevice, st));
-  if (covs) B2_CUDA(cudaMemcpyAsync(s.raw_c.get(), covs, n * cov_stride * sizeof(double), cudaMemcpyHostToDevice, st));
+  B2_TRY(s.raw_p.upload(points, n * point_stride * sizeof(double), st));
+  if (covs) B2_TRY(s.raw_c.upload(covs, n * cov_stride * sizeof(double), st));
   B2_TRY(s.key_z.alloc(n * 4));
   B2_TRY(s.key_z2.alloc(n * 4));
   B2_TRY(s.idx_a.alloc(n * 4));
@@ -901,9 +878,8 @@ b2_status b2_overlap(const b2_voxelmap* const* targets, size_t num_targets, cons
     return B2_OK;
   }
   DeviceBuffer d_maps, d_count;
-  B2_TRY(d_maps.alloc(maps.size() * sizeof(OverlapMap)));
+  B2_TRY(d_maps.upload(maps.data(), maps.size() * sizeof(OverlapMap), st));
   B2_TRY(d_count.alloc(sizeof(unsigned long long)));
-  B2_CUDA(cudaMemcpyAsync(d_maps.get(), maps.data(), maps.size() * sizeof(OverlapMap), cudaMemcpyHostToDevice, st));
   B2_CUDA(cudaMemsetAsync(d_count.get(), 0, sizeof(unsigned long long), st));
   const unsigned grid = static_cast<unsigned>((source->n + 255) / 256);
   with_storage(source->point_bytes, [&](auto p) {
@@ -970,13 +946,12 @@ b2_status b2_merge_frames(b2_ctx* ctx, const double* poses, const b2_cloud* cons
   }
   DeviceBuffer d_frames, keys, keys2, vals, vals2, starts, d_min, tmp, d_xyz, d_cov;
   const int ni = static_cast<int>(total);
-  B2_TRY(d_frames.alloc(num_frames * sizeof(MergeFrame)));
+  B2_TRY(d_frames.upload(h.data(), num_frames * sizeof(MergeFrame), st));
   B2_TRY(keys.alloc(total * 8));
   B2_TRY(keys2.alloc(total * 8));
   B2_TRY(vals.alloc(total * 4));
   B2_TRY(vals2.alloc(total * 4));
   B2_TRY(d_min.alloc(8));
-  B2_CUDA(cudaMemcpyAsync(d_frames.get(), h.data(), num_frames * sizeof(MergeFrame), cudaMemcpyHostToDevice, st));
   for (size_t f = 0; f < num_frames; f++)
     if (h[f].n) merge_keys_kernel<<<(h[f].n + 255) / 256, 256, 0, st>>>(d_frames.as<MergeFrame>(), static_cast<int>(f), 1.0 / downsample_resolution, keys.as<unsigned long long>(), vals.as<uint32_t>());
   auto min_key = [&](void* t, size_t& b) {
@@ -1011,9 +986,8 @@ b2_status b2_voxelmap_lookup(const b2_voxelmap* vm, const double* points, int po
   B2_CUDA(cudaSetDevice(vm->ctx->device));
   cudaStream_t st = vm->ctx->stream;
   DeviceBuffer dp, di;
-  B2_TRY(dp.alloc(n * point_stride * sizeof(double)));
+  B2_TRY(dp.upload(points, n * point_stride * sizeof(double), st));
   B2_TRY(di.alloc(n * sizeof(int32_t)));
-  B2_CUDA(cudaMemcpyAsync(dp.get(), points, n * point_stride * sizeof(double), cudaMemcpyHostToDevice, st));
   lookup_points_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(dp.as<double>(), point_stride, n, vm->table(), di.as<int32_t>());
   B2_CUDA(cudaGetLastError());
   B2_CUDA(cudaMemcpyAsync(out_index, di.get(), n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -1150,13 +1124,11 @@ b2_status b2_ivox_knn(const b2_ivox* iv, const double* queries, int query_stride
   B2_CUDA(cudaSetDevice(vm->ctx->device));
   cudaStream_t st = vm->ctx->stream;
   DeviceBuffer dq, di, ds;
-  B2_TRY(dq.alloc(nq * query_stride * sizeof(double)));
+  B2_TRY(dq.upload(queries, nq * query_stride * sizeof(double), st));
   B2_TRY(di.alloc(nq * k * sizeof(long long)));
   B2_TRY(ds.alloc(nq * k * sizeof(double)));
-  B2_CUDA(cudaMemcpyAsync(dq.get(), queries, nq * query_stride * sizeof(double), cudaMemcpyHostToDevice, st));
   const IvoxView view{vm->table(), vm->d_records.as<const double>(), vm->d_counts.as<const uint32_t>(), vm->slots, iv->neighbor_mode};
-  ivox_knn_kernel<<<static_cast<unsigned>((nq + 127) / 128), 128, 0, st>>>(dq.as<double>(), query_stride, nq, k, max_sq_dist, view, vm->num_voxels, di.as<long long>(),
-                                                                           ds.as<double>());
+  ivox_knn_kernel<<<static_cast<unsigned>((nq + 127) / 128), 128, 0, st>>>(dq.as<double>(), query_stride, nq, k, max_sq_dist, view, di.as<long long>(), ds.as<double>());
   B2_CUDA(cudaGetLastError());
   B2_CUDA(cudaMemcpyAsync(out_index, di.get(), nq * k * sizeof(long long), cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaMemcpyAsync(out_sq_dist, ds.get(), nq * k * sizeof(double), cudaMemcpyDeviceToHost, st));

@@ -279,7 +279,15 @@ b2_status assemble_cloud(b2_ctx* ctx, const RawCloud& raw, unsigned flags, const
   const bool compact = flags & B2_CLOUD_COMPACT_F32;
   const bool force64 = flags & B2_CLOUD_FORCE_F64;
   c->cov_bytes = raw.covs ? (force64 ? 8 : (compact || !(h_res.flags & 2u)) ? 4 : 8) : 0;
+  double mn[3] = {0.0, 0.0, 0.0}, mx[3] = {0.0, 0.0, 0.0};
+  if (rp && n > 0) {
+    for (int k = 0; k < 3; k++) {
+      mn[k] = decode_ordered(h_res.mins[k]);
+      mx[k] = decode_ordered(h_res.maxs[k]);
+    }
+  }
   if (like) {
+    for (int k = 0; k < 3; k++) c->centre[k] = like->centre[k];
     c->point_bytes = like->point_bytes;
     c->reordered = like->reordered;
     B2_TRY(c->d_points.alloc(like->d_points.bytes()));
@@ -289,17 +297,13 @@ b2_status assemble_cloud(b2_ctx* ctx, const RawCloud& raw, unsigned flags, const
       B2_CUDA(cudaMemcpyAsync(c->d_perm.get(), like->d_perm.get(), like->d_perm.bytes(), cudaMemcpyDeviceToDevice, st));
     }
   } else {
+    for (int k = 0; k < 3; k++) c->centre[k] = 0.5 * (mn[k] + mx[k]);
     c->point_bytes = force64 ? 8 : (compact || !(h_res.flags & 1u)) ? 4 : 8;
     c->reordered = !(flags & B2_CLOUD_NO_REORDER) && n > 1;
   }
 
   // Morton permutation
   if (!like && c->reordered) {
-    double mn[3], mx[3];
-    for (int k = 0; k < 3; k++) {
-      mn[k] = decode_ordered(h_res.mins[k]);
-      mx[k] = decode_ordered(h_res.maxs[k]);
-    }
     const double extent = std::max(std::max(mx[0] - mn[0], mx[1] - mn[1]), std::max(mx[2] - mn[2], 1e-9));
     const double scale = 65535.0 / extent;
     B2_TRY(d_keys.alloc(n * sizeof(unsigned long long)));

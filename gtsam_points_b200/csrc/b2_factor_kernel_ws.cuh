@@ -144,6 +144,7 @@ struct Shared {
   uint32_t done[K::kP];  // factor runs completed by the probe warp (tail is final for run e once done == e + 1)
   uint32_t ack[K::kP];   // factor runs the accumulate warp has finished draining
   double probe_pose[K::kP][12];  // per probe warp: R (9, row-major) | t (3) of the factor run it is working on
+  double c[3];  // linearize: the expansion point R centre (FactorDesc::centre) of the accumulate side's current factor run
 };
 
 // tiles of CTA c: [c * T / G, (c + 1) * T / G) -- contiguous and balanced; the host uses the same formula for the slots
@@ -224,7 +225,7 @@ __device__ __forceinline__ void flush_factor(Shared<K>& sh, double (&v)[kAcc], i
     consumer_barrier<kC>();
     return;
   }
-  epilogue_build(sh.A, sh.X, sh.D, sh.tot, sh.R, sh.t, ctid);
+  epilogue_build(sh.A, sh.X, sh.D, sh.tot, sh.R, sh.t, sh.c, ctid);
   consumer_barrier<kC>();
   double* rec = out + static_cast<size_t>(d.out_index) * B2_LINEARIZED_DOUBLES;
   epilogue_store(rec, sh.A, sh.X, sh.D, sh.tot, ctid);
@@ -564,15 +565,17 @@ __device__ __forceinline__ void factor_kernel_body(const FactorDesc* __restrict_
         reinterpret_cast<uint32_t*>(&sh.desc)[ctid] = SINGLE ? reinterpret_cast<const uint32_t*>(&pose.desc)[ctid] : __ldg(reinterpret_cast<const uint32_t*>(descs + f) + ctid);
       consumer_barrier<kC>();
       const FactorDesc& d = sh.desc;
-      if (ctid < 21) {
+      if (ctid < (MODE == MODE_LINEARIZE ? 24 : 21)) {
         const double* pe = SINGLE ? pose.m : ((MODE == MODE_ERROR ? poses_eval : poses_lin) + static_cast<size_t>(d.out_index) * 16);
         const double* pl = (MODE == MODE_ERROR) ? d.lin_pose : pe;
         if (ctid < 9)
           sh.R[ctid] = pe[(ctid / 3) * 4 + ctid % 3];
         else if (ctid < 12)
           sh.t[ctid - 9] = pe[(ctid - 9) * 4 + 3];
-        else
+        else if (ctid < 21)
           sh.RL[ctid - 12] = pl[((ctid - 12) / 3) * 4 + (ctid - 12) % 3];
+        else
+          sh.c[ctid - 21] = expansion_point(pe, 4, d.centre, ctid - 21);  // linearize: c = R centre of this run
       }
       consumer_barrier<kC>();
       constexpr bool kConstRL = SINGLE && MODE == MODE_LINEARIZE;
@@ -587,6 +590,8 @@ __device__ __forceinline__ void factor_kernel_body(const FactorDesc* __restrict_
       }
       auto rl = [&](int i) -> double { return kConstRL ? pose.m[(i / 3) * 4 + (i % 3)] : RLr[kConstRL ? 0 : i]; };
       auto tt = [&](int i) -> double { return SINGLE ? pose.m[i * 4 + 3] : tr[SINGLE ? 0 : i]; };
+      // the expansion point stays in shared memory: read per batch, it costs the accumulate warps no registers
+      auto cc = [&](int i) -> double { return sh.c[i]; };
 #pragma unroll
       for (int k = 0; k < kAcc; k++) acc[k] = 0.0;
       const double* __restrict__ records = d.records;
@@ -648,11 +653,11 @@ __device__ __forceinline__ void factor_kernel_body(const FactorDesc* __restrict_
           if (nb == kBatch) {
             // full batch (uniform branch): no per-lane predicates, the kIPL bodies sit in one basic block and interleave
 #pragma unroll
-            for (int j = 0; j < kIPL; j++) accumulate_point_f<MODE, K::kMetric>(acc, rl, tt, b[j].u0, b[j].u1, b[j].u2, b[j].T, b[j].A);
+            for (int j = 0; j < kIPL; j++) accumulate_point_f<MODE, K::kMetric>(acc, rl, tt, cc, b[j].u0, b[j].u1, b[j].u2, b[j].T, b[j].A);
           } else {
 #pragma unroll
             for (int j = 0; j < kIPL; j++)
-              if (b[j].valid) accumulate_point_f<MODE, K::kMetric>(acc, rl, tt, b[j].u0, b[j].u1, b[j].u2, b[j].T, b[j].A);
+              if (b[j].valid) accumulate_point_f<MODE, K::kMetric>(acc, rl, tt, cc, b[j].u0, b[j].u1, b[j].u2, b[j].T, b[j].A);
           }
         }
         if (fin) {

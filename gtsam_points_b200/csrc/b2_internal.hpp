@@ -296,6 +296,9 @@ struct b2_cloud {
   int cov_bytes = 0;     // 0, 4 or 8
   int normal_bytes = 0;  // 0, 4 or 8
   bool reordered = false;
+  // centre of the points' bounding box, 0.5 * (min + max) per axis (0 for an empty cloud): the factor kernels expand the
+  // per-correspondence Jacobian about this point so that coordinates far from the cloud's own origin do not cancel
+  double centre[3] = {0.0, 0.0, 0.0};
   b2::DeviceBuffer d_points;  // 3 planes (x, y, z) of n_pad elements
   b2::DeviceBuffer d_covs;    // 6 planes (c00, c01, c02, c11, c12, c22) of n_pad elements
   b2::DeviceBuffer d_normals; // 3 planes (nx, ny, nz) of n_pad elements (empty if the cloud has no normals)

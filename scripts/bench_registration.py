@@ -8,14 +8,14 @@ normals from 10 neighbours estimated on the device.  Per input it takes medians 
       parameters, dof 6): its matching alone (both feature 1-NN passes and the compaction: max_iterations = 0), the whole call, and
       FPFH + GNC end to end; gnc_loop is the whole call's median minus the matching's; the same stages by CUDA events on the
       context's stream;
-  (b) the same chains on the CPU oracles (tests/registration_oracle.cpp, tests/gnc_oracle.cpp) on all host cores, timed once
+  (b) the same chains on the CPU oracles (tests/registration_oracle.cpp) on all host cores, timed once
       (it takes minutes at the synthetic size): brute-force FPFH, then RANSAC with a brute-force 1-NN per sample, or GNC with
       brute-force matching.
 Then, per input, a second JSON line with the PFH and keypoint stages (radius 5 m, 10000 neighbours), medians over --reps between
 device synchronisations: PFH and FPFH of the target over all points and at 1 % and 10 % of its points (a seeded random choice), and
 PFH of both clouds followed by RANSAC or GNC, end to end.  The pair counts are summed from the neighbour counts of the device radius
 search (m (m - 1) / 2 per row for PFH, m - 1 per SPFH row for FPFH), and pairs per second is that count over the median time.  With
-the CPU oracle (tests/pfh_oracle.cpp), its PFH over all points and its PFH and FPFH at 10 % are timed once each.
+the CPU oracle (tests/registration_oracle.cpp), its PFH over all points and its PFH and FPFH at 10 % are timed once each.
 Prints the card name, power limit and max SM clock of the same run, then the JSON lines.
 
   python scripts/bench_registration.py [--reps 5] [--synthetic 100000] [--no-cpu] [--pfh-only]
@@ -35,8 +35,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 
 import gtsam_points_b200 as g  # noqa: E402
-import gnc_oracle as go  # noqa: E402
-import pfh_oracle as po  # noqa: E402
 import registration_cases as rc  # noqa: E402
 import registration_oracle as ro  # noqa: E402
 from gtsam_points_b200 import synthetic as syn  # noqa: E402
@@ -114,8 +112,7 @@ def run(name, tp, src, reps, cpu):
         out[f"gpu_{k}_event_ms"] = round(statistics.median(e), 3)
     out["gpu_gnc_loop_ms"] = round(out["gpu_gnc_ms"] - out["gpu_gnc_match_ms"], 3)
     if cpu:
-        threads = ro.max_threads()
-        go.lib()  # compiled on first use: outside the timed window
+        threads = ro.max_threads()  # compiles the oracle on first use: outside the timed window
         t = time.perf_counter()
         tf_c, _, _ = ro.fpfh(tgt.points, tgt.normals, 5.0, 10000, threads)
         sf_c, _, _ = ro.fpfh(source.points, source.normals, 5.0, 10000, threads)
@@ -123,7 +120,7 @@ def run(name, tp, src, reps, cpu):
         ro.ransac(tgt.points, source.points, tf_c, sf_c, dof=6, num_threads=threads)
         out["cpu_oracle_end_to_end_ms"] = round((time.perf_counter() - t) * 1e3, 1)
         t = time.perf_counter()
-        go.gnc(tgt.points, source.points, tf_c, sf_c, dof=6, num_threads=threads)
+        ro.gnc(tgt.points, source.points, tf_c, sf_c, dof=6, num_threads=threads)
         out["cpu_oracle_gnc_end_to_end_ms"] = round((t_fpfh + time.perf_counter() - t) * 1e3, 1)
         out["cpu_threads"] = threads
     return out
@@ -178,9 +175,9 @@ def run_pfh(name, tp, src, reps, cpu):
         out[f"{k}_error_m"], out[f"{k}_error_rad"] = round(et, 4), round(er, 5)
     if cpu:
         threads = ro.max_threads()
-        for k, fn in (("pfh_all", lambda: po.pfh(tgt.points, tgt.normals, 5.0, 10000, threads)),
-                      ("pfh_kp10", lambda: po.pfh(tgt.points, tgt.normals, 5.0, 10000, threads, indices=kp[10])),
-                      ("fpfh_kp10", lambda: po.fpfh_at(tgt.points, tgt.normals, kp[10], 5.0, 10000, threads))):
+        for k, fn in (("pfh_all", lambda: ro.pfh(tgt.points, tgt.normals, 5.0, 10000, threads)),
+                      ("pfh_kp10", lambda: ro.pfh(tgt.points, tgt.normals, 5.0, 10000, threads, indices=kp[10])),
+                      ("fpfh_kp10", lambda: ro.fpfh_at(tgt.points, tgt.normals, kp[10], 5.0, 10000, threads))):
             t = time.perf_counter()
             fn()
             out[f"cpu_oracle_{k}_ms"] = round((time.perf_counter() - t) * 1e3, 1)

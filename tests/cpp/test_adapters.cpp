@@ -7,32 +7,7 @@
 //     gtsam_points::NonlinearFactorSet + LinearizationHook::register_hook) compiled and RUN against header mocks.
 // Inputs and expected values come from a binary file written by the python test (oracle results).
 //   usage: test_adapters <case.bin>
-#include <algorithm>
-#include <cmath>
-#include <cstdio>
-#include <cstring>
-#include <vector>
-
-#include "gtsam_points_b200/gtsam_points_b200.hpp"
-
-using namespace gtsam_points_b200;
-
-static std::vector<double> read_vec(FILE* f) {
-  std::uint64_t n = 0;
-  if (fread(&n, 8, 1, f) != 1) throw std::runtime_error("short read");
-  std::vector<double> v(n);
-  if (n && fread(v.data(), 8, n, f) != n) throw std::runtime_error("short read");
-  return v;
-}
-
-static double relerr(const double* a, const double* b, int n) {
-  double num = 0, den = 0;
-  for (int i = 0; i < n; i++) {
-    num = std::fmax(num, std::fabs(a[i] - b[i]));
-    den = std::fmax(den, std::fabs(b[i]));
-  }
-  return num / std::fmax(den, 1e-300);
-}
+#include "driver.hpp"
 
 // the reference's frame shape (types/point_cloud.hpp:103-118): raw pointers to Vector4d / Matrix4d arrays + size()
 struct Vec4d {
@@ -47,67 +22,6 @@ struct FrameLike {
   Mat4d* covs = nullptr;
   std::size_t size() const { return num_points; }
 };
-
-// ---- differences between the two builds, in one place ----
-#ifdef B2_HAVE_GTSAM
-static void insert_pose(Values& values, Key k, const std::vector<double>& T) {
-  gtsam::Matrix4 m;
-  for (int i = 0; i < 4; i++)
-    for (int j = 0; j < 4; j++) m(i, j) = T[i * 4 + j];
-  values.insert(k, gtsam::Pose3(m));
-}
-static FixedPose fixed_pose(const std::vector<double>& T) {
-  gtsam::Matrix4 m;
-  for (int i = 0; i < 4; i++)
-    for (int j = 0; j < 4; j++) m(i, j) = T[i * 4 + j];
-  return gtsam::Pose3(m);
-}
-struct Hess {  // row-major copies of the blocks of a gtsam::HessianFactor
-  double G11[36], G12[36], G22[36], g1[6], g2[6], f;
-  bool binary;
-};
-static Hess unpack(const LinearFactorPtr& lf) {
-  auto h = factor_pointer_cast<gtsam::HessianFactor>(lf);
-  Hess o{};
-  o.binary = h->keys().size() == 2;
-  for (int i = 0; i < 6; i++) {
-    for (int j = 0; j < 6; j++) {
-      o.G22[i * 6 + j] = h->G22(i, j);
-      if (o.binary) o.G11[i * 6 + j] = h->G11(i, j), o.G12[i * 6 + j] = h->G12(i, j);
-    }
-    o.g2[i] = h->g2(i);
-    if (o.binary) o.g1[i] = h->g1(i);
-  }
-  o.f = h->f;
-  return o;
-}
-#else
-static void insert_pose(Values& values, Key k, const std::vector<double>& T) {
-  Mat4 a;
-  std::copy(T.begin(), T.end(), a.begin());
-  values.insert(k, a);
-}
-static FixedPose fixed_pose(const std::vector<double>& T) {
-  Mat4 a;
-  std::copy(T.begin(), T.end(), a.begin());
-  return a;
-}
-struct Hess {
-  double G11[36], G12[36], G22[36], g1[6], g2[6], f;
-  bool binary;
-};
-static Hess unpack(const LinearFactorPtr& h) {
-  Hess o{};
-  o.binary = h->keys.size() == 2;
-  std::memcpy(o.G11, h->G11, sizeof(o.G11));
-  std::memcpy(o.G12, h->G12, sizeof(o.G12));
-  std::memcpy(o.G22, h->G22, sizeof(o.G22));
-  std::memcpy(o.g1, h->g1, sizeof(o.g1));
-  std::memcpy(o.g2, h->g2, sizeof(o.g2));
-  o.f = h->f;
-  return o;
-}
-#endif
 
 static int check_against(const Hess& h, const std::vector<double>& e, double tol) {
   int fails = 0;
@@ -126,16 +40,14 @@ static int check_against(const Hess& h, const std::vector<double>& e, double tol
 }
 
 int main(int argc, char** argv) {
-  if (argc < 2) return 2;
-  FILE* f = fopen(argv[1], "rb");
-  if (!f) return 2;
-  const auto tp = read_vec(f), tc = read_vec(f), sp = read_vec(f), sc = read_vec(f);
-  const auto Tt = read_vec(f), Ts = read_vec(f), Ts2 = read_vec(f);
-  const auto exp_vgicp = read_vec(f), exp_gicp = read_vec(f), exp_err = read_vec(f);
-  const auto res = read_vec(f);
-  const auto exp_unary = read_vec(f), exp_overlap = read_vec(f);
-  const auto exp_icp = read_vec(f), exp_merge = read_vec(f), exp_cov = read_vec(f);  // ICP linearization, merged-frame size, first covariances
-  fclose(f);
+  Case in(argc, argv);
+  if (!in) return 2;
+  const auto tp = in.next(), tc = in.next(), sp = in.next(), sc = in.next();
+  const auto Tt = in.next(), Ts = in.next(), Ts2 = in.next();
+  const auto exp_vgicp = in.next(), exp_gicp = in.next(), exp_err = in.next();
+  const auto res = in.next();
+  const auto exp_unary = in.next(), exp_overlap = in.next();
+  const auto exp_icp = in.next(), exp_merge = in.next(), exp_cov = in.next();  // ICP linearization, merged-frame size, first covariances
   const std::size_t nt = tp.size() / 4, ns = sp.size() / 4;
   const double tol = 1e-9;
   int fails = 0;

@@ -2,42 +2,17 @@
 // estimate_pose_gnc_gpu with the reference's GNCParams field names, against the oracle's GNC result.  Built standalone and with
 // -I tests/cpp/mock_gtsam by tests/test_gnc_cpp.py; inputs and expected values come from a binary file written by that test.
 //   usage: test_gnc <case.bin>
-#include <cmath>
-#include <cstdio>
-#include <stdexcept>
-#include <vector>
-
-#include "gtsam_points_b200/gtsam_points_b200.hpp"
-
-using namespace gtsam_points_b200;
-
-static std::vector<double> read_vec(FILE* f) {
-  std::uint64_t n = 0;
-  if (fread(&n, 8, 1, f) != 1) throw std::runtime_error("short read");
-  std::vector<double> v(n);
-  if (n && fread(v.data(), 8, n, f) != n) throw std::runtime_error("short read");
-  return v;
-}
-
-#define EXPECT(cond)                                                \
-  do {                                                              \
-    if (!(cond)) {                                                  \
-      std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #cond); \
-      return 1;                                                     \
-    }                                                               \
-  } while (0)
+#include "driver.hpp"
 
 int main(int argc, char** argv) {
-  if (argc < 2) return 2;
-  FILE* fp = std::fopen(argv[1], "rb");
-  if (!fp) return 2;
-  const auto tgt_p = read_vec(fp);  // N x 4 (x, y, z, 1)
-  const auto src_p = read_vec(fp);  // M x 4
-  const auto tgt_f = read_vec(fp);  // the oracle's FPFH rows, N x 33
-  const auto src_f = read_vec(fp);  // M x 33
-  const auto pairs = read_vec(fp);  // the oracle's correspondences, (target, source) per pair
-  const auto want = read_vec(fp);   // the oracle's GNC result: T (16), num_inliers, slack (default parameters)
-  std::fclose(fp);
+  Case in(argc, argv);
+  if (!in) return 2;
+  const auto tgt_p = in.next();  // N x 4 (x, y, z, 1)
+  const auto src_p = in.next();  // M x 4
+  const auto tgt_f = in.next();  // the oracle's FPFH rows, N x 33
+  const auto src_f = in.next();  // M x 33
+  const auto pairs = in.next();  // the oracle's correspondences, (target, source) per pair
+  const auto want = in.next();   // the oracle's GNC result: T (16), num_inliers, slack (default parameters)
   const std::size_t N = tgt_p.size() / 4, M = src_p.size() / 4;
 
   auto ctx = Context::default_context();

@@ -4,83 +4,14 @@
 // of the map and checks that the factor re-associates.  Built standalone and with -I tests/cpp/mock_gtsam by
 // tests/test_ivox_cpp.py; inputs and expected values come from a binary file written by that test.
 //   usage: test_ivox <case.bin>
-#include <cmath>
-#include <cstdio>
-#include <cstring>
-#include <vector>
-
-#include "gtsam_points_b200/gtsam_points_b200.hpp"
-
-using namespace gtsam_points_b200;
-
-static std::vector<double> read_vec(FILE* f) {
-  std::uint64_t n = 0;
-  if (fread(&n, 8, 1, f) != 1) throw std::runtime_error("short read");
-  std::vector<double> v(n);
-  if (n && fread(v.data(), 8, n, f) != n) throw std::runtime_error("short read");
-  return v;
-}
-
-static double relerr(const double* a, const double* b, int n) {
-  double num = 0, den = 0;
-  for (int i = 0; i < n; i++) {
-    num = std::fmax(num, std::fabs(a[i] - b[i]));
-    den = std::fmax(den, std::fabs(b[i]));
-  }
-  return num / std::fmax(den, 1e-300);
-}
-
-#ifdef B2_HAVE_GTSAM
-static void insert_pose(Values& values, Key k, const std::vector<double>& T) {
-  gtsam::Matrix4 m;
-  for (int i = 0; i < 4; i++)
-    for (int j = 0; j < 4; j++) m(i, j) = T[i * 4 + j];
-  values.insert(k, gtsam::Pose3(m));
-}
-static FixedPose identity_pose() {
-  gtsam::Matrix4 m;
-  for (int i = 0; i < 4; i++)
-    for (int j = 0; j < 4; j++) m(i, j) = i == j ? 1.0 : 0.0;
-  return gtsam::Pose3(m);
-}
-static void source_block(const LinearFactorPtr& lf, double* G22, double* g2, double* f) {
-  auto h = factor_pointer_cast<gtsam::HessianFactor>(lf);
-  for (int i = 0; i < 6; i++) {
-    for (int j = 0; j < 6; j++) G22[i * 6 + j] = h->G22(i, j);
-    g2[i] = h->g2(i);
-  }
-  *f = h->f;
-}
-#else
-static void insert_pose(Values& values, Key k, const std::vector<double>& T) {
-  Mat4 a;
-  std::copy(T.begin(), T.end(), a.begin());
-  values.insert(k, a);
-}
-static FixedPose identity_pose() { return Mat4{1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1}; }
-static void source_block(const LinearFactorPtr& h, double* G22, double* g2, double* f) {
-  std::memcpy(G22, h->G22, sizeof(double) * 36);
-  std::memcpy(g2, h->g2, sizeof(double) * 6);
-  *f = h->f;
-}
-#endif
-
-// unary factor against the map frame: only the source block exists
-static int check_source(const LinearFactorPtr& lf, const std::vector<double>& e, double tol) {
-  double G22[36], g2[6], f, eg[6];
-  source_block(lf, G22, g2, &f);
-  for (int i = 0; i < 6; i++) eg[i] = -e[114 + i];
-  return (relerr(G22, e.data() + 36, 36) > tol) + (relerr(g2, eg, 6) > tol) + (std::fabs(f - e[120]) > tol * e[120]);
-}
+#include "driver.hpp"
 
 int main(int argc, char** argv) {
-  if (argc < 2) return 2;
-  FILE* f = fopen(argv[1], "rb");
-  if (!f) return 2;
-  const auto m0p = read_vec(f), m0c = read_vec(f), m1p = read_vec(f), m1c = read_vec(f), m2p = read_vec(f), m2c = read_vec(f);
-  const auto sp = read_vec(f), sc = read_vec(f), Ts = read_vec(f), Ts2 = read_vec(f);
-  const auto exp_lin = read_vec(f), exp_err = read_vec(f), exp_corr = read_vec(f), queries = read_vec(f), exp_knn = read_vec(f), exp_lin2 = read_vec(f);
-  fclose(f);
+  Case in(argc, argv);
+  if (!in) return 2;
+  const auto m0p = in.next(), m0c = in.next(), m1p = in.next(), m1c = in.next(), m2p = in.next(), m2c = in.next();
+  const auto sp = in.next(), sc = in.next(), Ts = in.next(), Ts2 = in.next();
+  const auto exp_lin = in.next(), exp_err = in.next(), exp_corr = in.next(), queries = in.next(), exp_knn = in.next(), exp_lin2 = in.next();
   const double tol = 1e-9;
   int fails = 0;
 

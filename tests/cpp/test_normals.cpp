@@ -3,22 +3,7 @@
 // IntegratedICPFactor taking the target cloud's normals, against the same factor given the host array.  Built standalone and with
 // -I tests/cpp/mock_gtsam by tests/test_normals_cpp.py; inputs and expected values come from a binary file written by that test.
 //   usage: test_normals <case.bin>
-#include <cmath>
-#include <cstdio>
-#include <cstring>
-#include <vector>
-
-#include "gtsam_points_b200/gtsam_points_b200.hpp"
-
-using namespace gtsam_points_b200;
-
-static std::vector<double> read_vec(FILE* f) {
-  std::uint64_t n = 0;
-  if (fread(&n, 8, 1, f) != 1) throw std::runtime_error("short read");
-  std::vector<double> v(n);
-  if (n && fread(v.data(), 8, n, f) != n) throw std::runtime_error("short read");
-  return v;
-}
+#include "driver.hpp"
 
 // the reference's PointCloud shape, with normals (types/point_cloud.hpp:103-108).  The frame of tests/cpp/mock_gtsam has no
 // `normals` member, so this struct is what exercises from_frame's "frame has normals" branch; test_adapters.cpp's frames
@@ -31,36 +16,11 @@ struct Frame {
   const double (*normals)[4] = nullptr;
 };
 
-#ifdef B2_HAVE_GTSAM
-static void insert_pose(Values& values, Key k, const std::vector<double>& T) {
-  gtsam::Matrix4 m;
-  for (int i = 0; i < 4; i++)
-    for (int j = 0; j < 4; j++) m(i, j) = T[i * 4 + j];
-  values.insert(k, gtsam::Pose3(m));
-}
-#else
-static void insert_pose(Values& values, Key k, const std::vector<double>& T) {
-  Mat4 a;
-  std::copy(T.begin(), T.end(), a.begin());
-  values.insert(k, a);
-}
-#endif
-
-#define EXPECT(cond)                                             \
-  do {                                                           \
-    if (!(cond)) {                                               \
-      std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #cond); \
-      return 1;                                                  \
-    }                                                            \
-  } while (0)
-
 int main(int argc, char** argv) {
-  if (argc < 2) return 2;
-  FILE* fp = std::fopen(argv[1], "rb");
-  if (!fp) return 2;
-  const auto tp = read_vec(fp), tc = read_vec(fp), sp = read_vec(fp), sc = read_vec(fp), sn = read_vec(fp), tn3 = read_vec(fp), T = read_vec(fp);
-  const auto want_inliers = read_vec(fp), want_corr = read_vec(fp);
-  std::fclose(fp);
+  Case in(argc, argv);
+  if (!in) return 2;
+  const auto tp = in.next(), tc = in.next(), sp = in.next(), sc = in.next(), sn = in.next(), tn3 = in.next(), T = in.next();
+  const auto want_inliers = in.next(), want_corr = in.next();
   const std::size_t nt = tp.size() / 4, ns = sp.size() / 4;
 
   auto target = std::make_shared<Frame>();

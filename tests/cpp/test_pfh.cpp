@@ -2,30 +2,7 @@
 // indices, and the indices overload of estimate_fpfh_gpu, against the CPU oracle's rows.  Built standalone and with
 // -I tests/cpp/mock_gtsam by tests/test_pfh_cpp.py; inputs and expected values come from a binary file written by that test.
 //   usage: test_pfh <case.bin>
-#include <cstdio>
-#include <cstring>
-#include <stdexcept>
-#include <vector>
-
-#include "gtsam_points_b200/gtsam_points_b200.hpp"
-
-using namespace gtsam_points_b200;
-
-static std::vector<double> read_vec(FILE* f) {
-  std::uint64_t n = 0;
-  if (fread(&n, 8, 1, f) != 1) throw std::runtime_error("short read");
-  std::vector<double> v(n);
-  if (n && fread(v.data(), 8, n, f) != n) throw std::runtime_error("short read");
-  return v;
-}
-
-#define EXPECT(cond)                                                \
-  do {                                                              \
-    if (!(cond)) {                                                  \
-      std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #cond); \
-      return 1;                                                     \
-    }                                                               \
-  } while (0)
+#include "driver.hpp"
 
 // rows k of `got` (dim wide) differ from `want` only where flag[k] is set; returns the number that differ, or -1
 static long compare(const std::vector<double>& got, const std::vector<double>& want, const std::vector<double>& flag, int dim) {
@@ -40,18 +17,16 @@ static long compare(const std::vector<double>& got, const std::vector<double>& w
 }
 
 int main(int argc, char** argv) {
-  if (argc < 2) return 2;
-  FILE* fp = std::fopen(argv[1], "rb");
-  if (!fp) return 2;
-  const auto pts = read_vec(fp);       // N x 4 (x, y, z, 1)
-  const auto nrm = read_vec(fp);       // N x 4 (nx, ny, nz, 0)
-  const auto idx_d = read_vec(fp);     // K indices
-  const auto pfh_want = read_vec(fp);  // the oracle's PFH rows at the indices, K x 125
-  const auto pfh_edge = read_vec(fp);  // K
-  const auto fpfh_want = read_vec(fp); // the oracle's FPFH rows at the indices, K x 33
-  const auto fpfh_edge = read_vec(fp); // K
-  const auto radius = read_vec(fp);    // search radius
-  std::fclose(fp);
+  Case in(argc, argv);
+  if (!in) return 2;
+  const auto pts = in.next();       // N x 4 (x, y, z, 1)
+  const auto nrm = in.next();       // N x 4 (nx, ny, nz, 0)
+  const auto idx_d = in.next();     // K indices
+  const auto pfh_want = in.next();  // the oracle's PFH rows at the indices, K x 125
+  const auto pfh_edge = in.next();  // K
+  const auto fpfh_want = in.next(); // the oracle's FPFH rows at the indices, K x 33
+  const auto fpfh_edge = in.next(); // K
+  const auto radius = in.next();    // search radius
   const std::size_t N = pts.size() / 4, K = idx_d.size();
   std::vector<int> idx(K);
   for (std::size_t k = 0; k < K; k++) idx[k] = static_cast<int>(idx_d[k]);

@@ -3,34 +3,7 @@
 // tests/test_posed_frames_cpp.py computes with the numpy restatement (tests/posed_ref.py).  Built standalone and with
 // -I tests/cpp/mock_gtsam.
 //   usage: test_posed_frames <case.bin>    (xyz n x 3, cov n x 9, T 16, posed xyz n x 3, posed cov n x 9)
-#include <cstdio>
-#include <cstring>
-#include <stdexcept>
-#include <vector>
-
-#include "gtsam_points_b200/gtsam_points_b200.hpp"
-
-using namespace gtsam_points_b200;
-
-static std::vector<double> read_vec(FILE* f) {
-  std::uint64_t n = 0;
-  if (fread(&n, 8, 1, f) != 1) throw std::runtime_error("short read");
-  std::vector<double> v(n);
-  if (n && fread(v.data(), 8, n, f) != n) throw std::runtime_error("short read");
-  return v;
-}
-
-#define EXPECT(cond)                                                \
-  do {                                                              \
-    if (!(cond)) {                                                  \
-      std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #cond); \
-      return 1;                                                     \
-    }                                                               \
-  } while (0)
-
-static bool same_bits(const std::vector<double>& a, const std::vector<double>& b) {
-  return a.size() == b.size() && (a.empty() || std::memcmp(a.data(), b.data(), a.size() * sizeof(double)) == 0);
-}
+#include "driver.hpp"
 
 static void voxelmap_download(const GaussianVoxelMapGPU& vm, std::vector<double>& means, std::vector<double>& covs, std::vector<int32_t>& counts) {
   const std::size_t V = vm.num_voxels();
@@ -39,11 +12,9 @@ static void voxelmap_download(const GaussianVoxelMapGPU& vm, std::vector<double>
 }
 
 int main(int argc, char** argv) {
-  if (argc < 2) return 2;
-  FILE* f = std::fopen(argv[1], "rb");
-  if (!f) return 2;
-  const std::vector<double> xyz = read_vec(f), cov = read_vec(f), Tv = read_vec(f), pxyz = read_vec(f), pcov = read_vec(f);
-  std::fclose(f);
+  Case in(argc, argv);
+  if (!in) return 2;
+  const std::vector<double> xyz = in.next(), cov = in.next(), Tv = in.next(), pxyz = in.next(), pcov = in.next();
   const std::size_t n = xyz.size() / 3;
   Mat4 T;
   std::copy(Tv.begin(), Tv.end(), T.begin());

@@ -3,34 +3,7 @@
 // the CPU voxel-grid oracle's output and the same factor built from host arrays.  Built standalone and with
 // -I tests/cpp/mock_gtsam by tests/test_preprocess_cpp.py; inputs and expected values come from a binary file written by that test.
 //   usage: test_preprocess <case.bin>
-#include <cstdio>
-#include <cstring>
-#include <stdexcept>
-#include <vector>
-
-#include "gtsam_points_b200/gtsam_points_b200.hpp"
-
-using namespace gtsam_points_b200;
-
-static std::vector<double> read_vec(FILE* f) {
-  std::uint64_t n = 0;
-  if (fread(&n, 8, 1, f) != 1) throw std::runtime_error("short read");
-  std::vector<double> v(n);
-  if (n && fread(v.data(), 8, n, f) != n) throw std::runtime_error("short read");
-  return v;
-}
-
-#define EXPECT(cond)                                                \
-  do {                                                              \
-    if (!(cond)) {                                                  \
-      std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #cond); \
-      return 1;                                                     \
-    }                                                               \
-  } while (0)
-
-static bool same_bits(const std::vector<double>& a, const std::vector<double>& b) {
-  return a.size() == b.size() && (a.empty() || std::memcmp(a.data(), b.data(), a.size() * sizeof(double)) == 0);
-}
+#include "driver.hpp"
 
 static std::vector<double> download_points(const PointCloudGPU& c) {
   std::vector<double> p(c.size() * 3);
@@ -39,15 +12,13 @@ static std::vector<double> download_points(const PointCloudGPU& c) {
 }
 
 int main(int argc, char** argv) {
-  if (argc < 2) return 2;
-  FILE* fp = std::fopen(argv[1], "rb");
-  if (!fp) return 2;
-  const auto tgt_raw = read_vec(fp);   // N x 4 (x, y, z, 1)
-  const auto src_raw = read_vec(fp);   // M x 4
-  const auto res = read_vec(fp);       // resolution
-  const auto tgt_want = read_vec(fp);  // the oracle's voxel grid of the target, m x 3
-  const auto delta = read_vec(fp);     // 4 x 4
-  std::fclose(fp);
+  Case in(argc, argv);
+  if (!in) return 2;
+  const auto tgt_raw = in.next();   // N x 4 (x, y, z, 1)
+  const auto src_raw = in.next();   // M x 4
+  const auto res = in.next();       // resolution
+  const auto tgt_want = in.next();  // the oracle's voxel grid of the target, m x 3
+  const auto delta = in.next();     // 4 x 4
 
   auto ctx = Context::default_context();
   auto tgt_grid = voxelgrid_sampling_gpu(tgt_raw.data(), nullptr, nullptr, tgt_raw.size() / 4, res[0], ctx);

@@ -3,45 +3,19 @@
 // Built standalone and with -I tests/cpp/mock_gtsam by tests/test_registration_cpp.py; inputs and expected values come from a
 // binary file written by that test.
 //   usage: test_registration <case.bin>
-#include <cmath>
-#include <cstdio>
-#include <cstring>
-#include <stdexcept>
-#include <vector>
-
-#include "gtsam_points_b200/gtsam_points_b200.hpp"
-
-using namespace gtsam_points_b200;
-
-static std::vector<double> read_vec(FILE* f) {
-  std::uint64_t n = 0;
-  if (fread(&n, 8, 1, f) != 1) throw std::runtime_error("short read");
-  std::vector<double> v(n);
-  if (n && fread(v.data(), 8, n, f) != n) throw std::runtime_error("short read");
-  return v;
-}
-
-#define EXPECT(cond)                                                \
-  do {                                                              \
-    if (!(cond)) {                                                  \
-      std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #cond); \
-      return 1;                                                     \
-    }                                                               \
-  } while (0)
+#include "driver.hpp"
 
 int main(int argc, char** argv) {
-  if (argc < 2) return 2;
-  FILE* fp = std::fopen(argv[1], "rb");
-  if (!fp) return 2;
-  const auto tgt_p = read_vec(fp);  // N x 4 (x, y, z, 1)
-  const auto tgt_n = read_vec(fp);  // N x 4 (nx, ny, nz, 0)
-  const auto src_p = read_vec(fp);  // M x 4
-  const auto src_n = read_vec(fp);  // M x 4
-  const auto tgt_f = read_vec(fp);  // the oracle's FPFH rows, N x 33
-  const auto src_f = read_vec(fp);  // M x 33
-  const auto edge = read_vec(fp);   // 1 where the oracle flags a row at a bin edge, N + M
-  const auto want = read_vec(fp);   // the oracle's RANSAC result: T (16), num_inliers, hypothesis (max_iterations 1000, dof 6)
-  std::fclose(fp);
+  Case in(argc, argv);
+  if (!in) return 2;
+  const auto tgt_p = in.next();  // N x 4 (x, y, z, 1)
+  const auto tgt_n = in.next();  // N x 4 (nx, ny, nz, 0)
+  const auto src_p = in.next();  // M x 4
+  const auto src_n = in.next();  // M x 4
+  const auto tgt_f = in.next();  // the oracle's FPFH rows, N x 33
+  const auto src_f = in.next();  // M x 33
+  const auto edge = in.next();   // 1 where the oracle flags a row at a bin edge, N + M
+  const auto want = in.next();   // the oracle's RANSAC result: T (16), num_inliers, hypothesis (max_iterations 1000, dof 6)
   const std::size_t N = tgt_p.size() / 4, M = src_p.size() / 4;
 
   auto ctx = Context::default_context();

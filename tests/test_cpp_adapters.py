@@ -7,29 +7,12 @@ import subprocess
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "cpp", "test_adapters.cpp")
-LIBDIR = os.path.join(ROOT, "gtsam_points_b200", "lib")
-MOCK = os.path.join(ROOT, "tests", "cpp", "mock_gtsam")
-
-
-def build_driver(tmp_path, mock_gtsam: bool):
-    exe = str(tmp_path / ("test_adapters_gtsam" if mock_gtsam else "test_adapters"))
-    cmd = ["/usr/bin/g++", "-std=c++17", "-O2", "-Wall", "-Wno-unused-variable", "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gtsam_points_b200", "cpp", "include")]
-    if mock_gtsam:
-        cmd += ["-I", MOCK]
-    cmd += [SRC, "-o", exe, "-L", LIBDIR, "-lb2points", f"-Wl,-rpath,{LIBDIR}"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    return exe
+import native
 
 
 @pytest.mark.parametrize("mock_gtsam", [False, True])
-def test_adapters_compile_against_c_abi(tmp_path, mock_gtsam):
-    from gtsam_points_b200 import build
-
-    build.build()
-    exe = build_driver(tmp_path, mock_gtsam)
+def test_adapters_compile_against_c_abi(mock_gtsam):
+    exe = native.adapter_driver("test_adapters", mock_gtsam)
     assert os.path.exists(exe)
     if mock_gtsam:  # the GTSAM branch really was compiled: its symbols are in the binary
         syms = subprocess.run(["nm", "-C", exe], capture_output=True, text=True).stdout
@@ -38,11 +21,11 @@ def test_adapters_compile_against_c_abi(tmp_path, mock_gtsam):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("mock_gtsam", [False, True])
-def test_adapters_match_oracle_in_reference_call_order(tmp_path, mock_gtsam):
+def test_adapters_match_oracle_in_reference_call_order(mock_gtsam):
     import oracle_lib as orc
     from gtsam_points_b200 import synthetic as syn
 
-    exe = build_driver(tmp_path, mock_gtsam)
+    exe = native.adapter_driver("test_adapters", mock_gtsam)
     tp, tc = syn.make_cloud(30000, stream=1, scale=0.25)
     sp, sc = syn.make_cloud(12000, stream=2, scale=0.25)
     rng = np.random.default_rng(2)
@@ -70,12 +53,4 @@ def test_adapters_match_oracle_in_reference_call_order(tmp_path, mock_gtsam):
     eicp = orc.Factor(otgt, osrc, tree=orc.KdTree(otgt, 4), num_threads=4, icp="point").linearize_raw(d)
     merged_xyz, _ = orc.merge_frames(np.stack([Tt, Ts]), [otgt, osrc], 0.5)
     cov_head = orc.estimate_covariances(tp, 10, num_threads=4)[:256]
-    case = tmp_path / "case.bin"
-    with open(case, "wb") as f:
-        for a in (pad4(tp), pad44(tc), pad4(sp), pad44(sc), Tt, Ts, Ts2, ev, eg, errs, np.array([0.5]), ev, overlap, eicp, np.array([len(merged_xyz)]), cov_head):
-            a = np.ascontiguousarray(a, dtype=np.float64).ravel()
-            f.write(np.uint64(a.size).tobytes())
-            f.write(a.tobytes())
-    r = subprocess.run([exe, str(case)], capture_output=True, text=True, timeout=180)
-    assert r.returncode == 0, r.stdout + r.stderr
-    assert "OK" in r.stdout
+    native.run_driver(exe, (pad4(tp), pad44(tc), pad4(sp), pad44(sc), Tt, Ts, Ts2, ev, eg, errs, np.array([0.5]), ev, overlap, eicp, np.array([len(merged_xyz)]), cov_head), timeout=180)

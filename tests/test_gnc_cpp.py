@@ -1,34 +1,16 @@
 """The C++ adapters' GNC path (GNCParams, estimate_pose_gnc_gpu) compiles against the C ABI -- standalone and against the header mocks
 (tests/cpp/mock_gtsam).  On a GPU box the driver (tests/cpp/test_gnc.cpp) is checked against the CPU registration oracle."""
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "cpp", "test_gnc.cpp")
-LIBDIR = os.path.join(ROOT, "gtsam_points_b200", "lib")
-MOCK = os.path.join(ROOT, "tests", "cpp", "mock_gtsam")
-
-
-def build_driver(tmp_path, mock_gtsam: bool):
-    exe = str(tmp_path / ("test_gnc_gtsam" if mock_gtsam else "test_gnc"))
-    cmd = ["/usr/bin/g++", "-std=c++17", "-O2", "-Wall", "-Wno-unused-variable", "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gtsam_points_b200", "cpp", "include")]
-    if mock_gtsam:
-        cmd += ["-I", MOCK]
-    cmd += [SRC, "-o", exe, "-L", LIBDIR, "-lb2points", f"-Wl,-rpath,{LIBDIR}"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    return exe
+import native
 
 
 @pytest.mark.parametrize("mock_gtsam", [False, True])
-def test_gnc_adapters_compile(tmp_path, mock_gtsam):
-    from gtsam_points_b200 import build
-
-    build.build()
-    exe = build_driver(tmp_path, mock_gtsam)
+def test_gnc_adapters_compile(mock_gtsam):
+    exe = native.adapter_driver("test_gnc", mock_gtsam)
     syms = subprocess.run(["nm", "-C", exe], capture_output=True, text=True).stdout
     for s in ("b2_features_create", "b2_estimate_pose_gnc"):
         assert s in syms
@@ -36,14 +18,13 @@ def test_gnc_adapters_compile(tmp_path, mock_gtsam):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("mock_gtsam", [False, True])
-def test_gnc_driver(tmp_path, mock_gtsam):
-    import gnc_oracle as go
+def test_gnc_driver(mock_gtsam):
     import normals_ref
     import registration_cases as rc
     import registration_oracle as ro
     import voxelgrid_oracle as vo
 
-    exe = build_driver(tmp_path, mock_gtsam)
+    exe = native.adapter_driver("test_gnc", mock_gtsam)
     d = rc.kitti00()
     tgt = vo.voxelgrid_sampling(d["frame0"], 0.5)[0]
     src = vo.voxelgrid_sampling(d["frame1"], 0.5)[0]
@@ -53,15 +34,7 @@ def test_gnc_driver(tmp_path, mock_gtsam):
     sn = (P[:3, :3] @ sn.T).T
     tf, _, _ = ro.fpfh(tgt, tn, 5.0, 10000)
     sf, _, _ = ro.fpfh(src, sn, 5.0, 10000)
-    r = go.gnc(tgt, src, tf, sf)
+    r = ro.gnc(tgt, src, tf, sf)
     want = np.concatenate([r["T_target_source"].ravel(), [r["num_inliers"], r["slack"].sum()]])
 
-    case = tmp_path / "case.bin"
-    with open(case, "wb") as f:
-        for a in [np.concatenate([tgt, np.ones((len(tgt), 1))], 1), np.concatenate([src, np.ones((len(src), 1))], 1), tf, sf, r["C"].astype(np.float64), want]:
-            a = np.ascontiguousarray(a, dtype=np.float64).ravel()
-            f.write(np.uint64(a.size).tobytes())
-            f.write(a.tobytes())
-    res = subprocess.run([exe, str(case)], capture_output=True, text=True, timeout=300)
-    assert res.returncode == 0, res.stdout + res.stderr
-    assert "OK" in res.stdout
+    native.run_driver(exe, [np.concatenate([tgt, np.ones((len(tgt), 1))], 1), np.concatenate([src, np.ones((len(src), 1))], 1), tf, sf, r["C"].astype(np.float64), want], timeout=300)

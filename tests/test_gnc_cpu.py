@@ -1,9 +1,8 @@
-"""The GNC oracle (orc_gnc in tests/gnc_oracle.cpp) against plain numpy restatements of b2_estimate_pose_gnc's steps on small
+"""The GNC oracle (orc_gnc in tests/registration_oracle.cpp) against plain numpy restatements of b2_estimate_pose_gnc's steps on small
 clouds, and its end-to-end result on the KITTI-00 pair against the reference test's gates (src/test/test_global_registration.cpp)."""
 import numpy as np
 import pytest
 
-import gnc_oracle as go
 import registration_cases as rc
 import registration_oracle as ro
 
@@ -65,7 +64,7 @@ def np_gnc_loop(tgt, src, C, dof, max_iterations=64, inner_iterations=3, div_fac
 
 def test_samples_and_reciprocal_matching(scene):
     P, F, src, sf = scene
-    r = go.gnc(P, src, F, sf, max_init_samples=100, num_threads=2)
+    r = ro.gnc(P, src, F, sf, max_init_samples=100, num_threads=2)
     smp = r["samples"]
     assert not r["swapped"] and len(smp) == 100 and len(np.unique(smp)) == 100 and np.all(np.diff(smp) > 0) and smp.max() < len(src)
     o = _nn(sf[smp], F)
@@ -75,14 +74,14 @@ def test_samples_and_reciprocal_matching(scene):
     assert np.array_equal(r["C"], r["matched"]) and r["draws"] is None
     assert 0 < mutual.sum() < 100
     # without the reciprocal test every sample gives a pair
-    r = go.gnc(P, src, F, sf, max_init_samples=100, reciprocal_check=False, num_threads=2)
+    r = ro.gnc(P, src, F, sf, max_init_samples=100, reciprocal_check=False, num_threads=2)
     assert np.array_equal(r["C"], np.stack([o, smp], 1))
 
 
 def test_swapped_side(scene):
     P, F, src, sf = scene
     # the target (200 rows) is smaller than the source (240): the target is sampled, pairs still read (target, source)
-    r = go.gnc(src, P, sf, F, num_threads=2)
+    r = ro.gnc(src, P, sf, F, num_threads=2)
     assert r["swapped"] and np.array_equal(r["samples"], np.arange(200))
     o = _nn(sf, F)
     mutual = _nn(F[o], sf) == np.arange(200)
@@ -91,7 +90,7 @@ def test_swapped_side(scene):
 
 def test_tuple_check(scene):
     P, F, src, sf = scene
-    r = go.gnc(P, src, F, sf, reciprocal_check=False, tuple_check=True, max_num_tuples=40, num_threads=2)
+    r = ro.gnc(P, src, F, sf, reciprocal_check=False, tuple_check=True, max_num_tuples=40, num_threads=2)
     m, C, draws = r["matched"], r["C"], r["draws"]
     assert len(m) == 200 and draws is not None and draws.shape == (40, 3) and draws.max() < 200
     want = []
@@ -112,13 +111,13 @@ def test_tuple_check(scene):
     assert np.array_equal(C, np.array(sorted(first.values(), key=lambda p: p[1])))
     assert len(np.unique(C[:, 1])) == len(C) and np.all(np.diff(C[:, 1]) > 0)
     # under the branch's threshold (|C| <= 3 max_num_tuples) the check does not run
-    assert go.gnc(P, src, F, sf, reciprocal_check=False, tuple_check=True, max_num_tuples=67, num_threads=2)["draws"] is None
+    assert ro.gnc(P, src, F, sf, reciprocal_check=False, tuple_check=True, max_num_tuples=67, num_threads=2)["draws"] is None
 
 
 @pytest.mark.parametrize("dof", [6, 4])
 def test_loop_matches_numpy(scene, dof):
     P, F, src, sf = scene
-    r = go.gnc(P, src, F, sf, reciprocal_check=False, dof=dof, num_threads=2)
+    r = ro.gnc(P, src, F, sf, reciprocal_check=False, dof=dof, num_threads=2)
     T, inl = np_gnc_loop(P, src, r["C"], dof)
     assert np.abs(r["T_target_source"] - T).max() <= 1e-9
     assert abs(r["num_inliers"] - inl) <= r["slack"].sum()
@@ -130,7 +129,7 @@ def test_loop_matches_numpy(scene, dof):
 
 def test_first_alignment_is_kabsch(scene):
     P, F, src, sf = scene
-    r = go.gnc(P, src, F, sf, reciprocal_check=False, max_iterations=1, inner_iterations=1, num_threads=2)
+    r = ro.gnc(P, src, F, sf, reciprocal_check=False, max_iterations=1, inner_iterations=1, num_threads=2)
     C = r["C"]
     t, s = P[C[:, 0]], src[C[:, 1]]
     mt, ms = t.mean(0), s.mean(0)
@@ -143,10 +142,10 @@ def test_first_alignment_is_kabsch(scene):
 def test_empty_and_zero_iterations(scene):
     P, F, src, sf = scene
     for kw in (dict(max_iterations=0), dict(inner_iterations=0)):
-        r = go.gnc(P, src, F, sf, num_threads=2, **kw)
+        r = ro.gnc(P, src, F, sf, num_threads=2, **kw)
         assert np.array_equal(r["T_target_source"], np.eye(4)) and r["num_inliers"] == 0 and r["inlier_rate"] == 0.0
     # wrong matches never keep their edge ratios exactly: tuple_thresh = 1 empties C
-    r = go.gnc(P, src, F, np.roll(sf, 1, axis=0), reciprocal_check=False, tuple_check=True, max_num_tuples=10, tuple_thresh=1.0, num_threads=2)
+    r = ro.gnc(P, src, F, np.roll(sf, 1, axis=0), reciprocal_check=False, tuple_check=True, max_num_tuples=10, tuple_thresh=1.0, num_threads=2)
     assert len(r["C"]) == 0 and np.array_equal(r["T_target_source"], np.eye(4)) and r["inlier_rate"] == 0.0
 
 
@@ -166,7 +165,7 @@ def test_oracle_meets_the_reference_gate_on_kitti00(dof):
     src_n = (P[:3, :3] @ sn.T).T
     tf, _, _ = ro.fpfh(tgt, tn, 5.0, 10000)
     sf, _, _ = ro.fpfh(src_p, src_n, 5.0, 10000)
-    r = go.gnc(tgt, src_p, tf, sf, dof=dof)
+    r = ro.gnc(tgt, src_p, tf, sf, dof=dof)
     et, er = rc.pose_error(r["T_target_source"], T_off)
     assert et <= 0.5 and er <= 0.1, (et, er, len(r["C"]), r["num_inliers"])
     if dof == 4:

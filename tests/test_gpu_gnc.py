@@ -1,11 +1,10 @@
-"""GNC global registration on the device (b2_estimate_pose_gnc) against the CPU oracle (orc_gnc in tests/gnc_oracle.cpp),
+"""GNC global registration on the device (b2_estimate_pose_gnc) against the CPU oracle (orc_gnc in tests/registration_oracle.cpp),
 the reference's end-to-end gate (src/test/test_global_registration.cpp) run entirely on the device, and the feature 1-NN's split
 of the targets over CTAs when the queries are few."""
 import numpy as np
 import pytest
 
 import gtsam_points_b200 as g
-import gnc_oracle as go
 import registration_cases as rc
 import registration_oracle as ro
 from gtsam_points_b200 import capi
@@ -45,7 +44,7 @@ def test_gnc_matches_the_oracle(kitti, case):
     if kw.pop("swap", False):
         tgt, src, tf, sf = src, tgt, sf, tf
     assert (len(src) < len(tgt)) != case.startswith("swapped")
-    want = go.gnc(tgt.points, src.points, tf, sf, **kw)
+    want = ro.gnc(tgt.points, src.points, tf, sf, **kw)
     TF, SF = g.Features.from_array(tf), g.Features.from_array(sf)
     params = g.GNCParams(**kw)
     res, C = g.estimate_pose_gnc(tgt, src, TF, SF, params, correspondences=True)
@@ -112,7 +111,7 @@ def test_gnc_invalid_inputs(kitti):
     pairs = np.zeros((4, 2), dtype=np.int64)
     num = C.c_size_t()
     assert lib.b2_estimate_pose_gnc(tgt.h, src.h, TF.h, SF.h, C.byref(cp), C.byref(res), pairs.ctypes.data_as(C.POINTER(C.c_int64)), 4, C.byref(num)) == 1
-    assert num.value == len(go.gnc(tgt.points, src.points, tf, sf)["C"]) > 4
+    assert num.value == len(ro.gnc(tgt.points, src.points, tf, sf)["C"]) > 4
 
 
 def test_gnc_identity_cases():
@@ -124,7 +123,7 @@ def test_gnc_identity_cases():
     S = (Ti[:3, :3] @ P[perm].T).T + Ti[:3, 3]
     sf = np.roll(F[perm], 1, axis=0)  # wrong matches: no tuple keeps its edge ratios exactly
     kw = dict(reciprocal_check=False, tuple_check=True, max_num_tuples=10, tuple_thresh=1.0)
-    assert len(go.gnc(P, S, F, sf, num_threads=2, **kw)["C"]) == 0
+    assert len(ro.gnc(P, S, F, sf, num_threads=2, **kw)["C"]) == 0
     tgt, src = g.PointCloud(P), g.PointCloud(S)
     TF, SF = g.Features.from_array(F), g.Features.from_array(sf)
     res, C = g.estimate_pose_gnc(tgt, src, TF, SF, g.GNCParams(**kw), correspondences=True)

@@ -1,11 +1,9 @@
 """PFH and features at chosen points on the device (b2_features_create_pfh, b2_features_create_fpfh_at) against the CPU oracle
-(orc_pfh / orc_fpfh_at in tests/pfh_oracle.cpp), and RANSAC and GNC on PFH features."""
+(orc_pfh / orc_fpfh_at in tests/registration_oracle.cpp), and RANSAC and GNC on PFH features."""
 import numpy as np
 import pytest
 
 import gtsam_points_b200 as g
-import gnc_oracle as go
-import pfh_oracle as po
 import registration_cases as rc
 import registration_oracle as ro
 from gtsam_points_b200 import capi
@@ -49,7 +47,7 @@ def check_pfh(got, want, edge, nn, max_differ):
 def test_pfh_matches_the_oracle_on_kitti00_all_points(kitti):
     for cloud in kitti:
         got = g.estimate_pfh(cloud, 2.0).download()
-        want, edge, nn = po.pfh(cloud.points, cloud.normals, 2.0, 10000)
+        want, edge, nn = ro.pfh(cloud.points, cloud.normals, 2.0, 10000)
         assert got.shape == (len(cloud), 125)
         check_pfh(got, want, edge, nn, 20)
         assert np.array_equal(g.estimate_pfh(cloud, 2.0).download(), got)  # bit-reproducible
@@ -60,11 +58,11 @@ def test_pfh_and_fpfh_at_keypoints_match_the_oracle_on_kitti00(kitti):
     rng = np.random.default_rng(4)
     idx = rng.choice(len(tgt), 400, replace=False)
     got = g.estimate_pfh(tgt, 5.0, indices=idx).download()
-    want, edge, nn = po.pfh(tgt.points, tgt.normals, 5.0, 10000, indices=idx)
+    want, edge, nn = ro.pfh(tgt.points, tgt.normals, 5.0, 10000, indices=idx)
     check_pfh(got, want, edge, nn, 10)
     assert np.array_equal(g.estimate_pfh(tgt, 5.0, indices=idx).download(), got)
     f_got = g.estimate_fpfh(tgt, 5.0, indices=idx).download()
-    f_want, f_edge, _ = po.fpfh_at(tgt.points, tgt.normals, idx, 5.0, 10000)
+    f_want, f_edge, _ = ro.fpfh_at(tgt.points, tgt.normals, idx, 5.0, 10000)
     assert np.array_equal(f_got[~f_edge], f_want[~f_edge])
     assert np.array_equal(f_got, g.estimate_fpfh(tgt, 5.0).download()[idx])
 
@@ -80,7 +78,7 @@ def test_pfh_on_synthetic_scenes(seed):
         for max_nn in (10000, 16):
             rows[flags, max_nn] = g.estimate_pfh(cloud, 1.5, max_nn, tree=g.KdTree.from_cloud(cloud) if max_nn == 16 else None).download()
     for max_nn in (10000, 16):
-        want, edge, nn = po.pfh(P, N, 1.5, max_nn)
+        want, edge, nn = ro.pfh(P, N, 1.5, max_nn)
         assert np.array_equal(rows[capi.B2_CLOUD_DEFAULT, max_nn], rows[capi.B2_CLOUD_NO_REORDER, max_nn])
         got = rows[capi.B2_CLOUD_DEFAULT, max_nn]
         check_pfh(got, want, edge, nn, 5)
@@ -143,7 +141,7 @@ def test_pfh_rows_split_over_many_ctas():
     cloud = g.PointCloud(P, normals=Nr)
     idx = np.array([0, 1234, 3999])
     got = g.estimate_pfh(cloud, 5.0, 10000, indices=idx).download()
-    want, edge, nn = po.pfh(P, Nr, 5.0, 10000, indices=idx)
+    want, edge, nn = ro.pfh(P, Nr, 5.0, 10000, indices=idx)
     assert (nn == 4000).all()
     check_pfh(got, want, edge, nn, 3)
 
@@ -165,8 +163,8 @@ def test_registration_on_pfh(kitti):
     """PFH at 5 m feeds RANSAC (dof 6 and 4) and GNC.  With the oracle's PFH rows on both sides, the device follows the oracle chains;
     the device's own PFH rows then drive the same calls end to end.  Both meet the reference test's gate (0.5 m, 0.1 rad)."""
     tgt, src = kitti
-    tf, _, _ = po.pfh(tgt.points, tgt.normals, 5.0, 10000)
-    sf, _, _ = po.pfh(src.points, src.normals, 5.0, 10000)
+    tf, _, _ = ro.pfh(tgt.points, tgt.normals, 5.0, 10000)
+    sf, _, _ = ro.pfh(src.points, src.normals, 5.0, 10000)
     TF, SF = g.Features.from_array(tf), g.Features.from_array(sf)
     dev_tf, dev_sf = g.estimate_pfh(tgt, 5.0), g.estimate_pfh(src, 5.0)
     assert dev_tf.dim == 125 and len(dev_tf) == len(tgt)
@@ -187,7 +185,7 @@ def test_registration_on_pfh(kitti):
         assert oracle_err[0] <= 0.5 and oracle_err[1] <= 0.1  # the oracle chain meets the reference test's gate, so the device must too
         assert et <= 0.5 and er <= 0.1 and dev_err[0] <= 0.5 and dev_err[1] <= 0.1
     for dof in (6, 4):
-        want = go.gnc(tgt.points, src.points, tf, sf, dof=dof)
+        want = ro.gnc(tgt.points, src.points, tf, sf, dof=dof)
         res, C = g.estimate_pose_gnc(tgt, src, TF, SF, g.GNCParams(dof=dof), correspondences=True)
         assert np.array_equal(C, want["C"])
         assert np.abs(res.T_target_source - want["T_target_source"]).max() <= 1e-9

@@ -2,49 +2,31 @@
 gtsam_points_b200/cpp) compiles against the C ABI -- standalone and in its GTSAM-typed form against the header mocks
 (tests/cpp/mock_gtsam).  On a GPU box the driver (tests/cpp/test_ivox_cov.cpp) runs in the optimizer's call order and is checked
 against the restatement (tests/ivox_cov_np.py) with np_ref's GICP algebra."""
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "cpp", "test_ivox_cov.cpp")
-LIBDIR = os.path.join(ROOT, "gtsam_points_b200", "lib")
-MOCK = os.path.join(ROOT, "tests", "cpp", "mock_gtsam")
-
-
-def build_driver(tmp_path, mock_gtsam: bool):
-    exe = str(tmp_path / ("test_ivox_cov_gtsam" if mock_gtsam else "test_ivox_cov"))
-    cmd = ["/usr/bin/g++", "-std=c++17", "-O2", "-Wall", "-Wno-unused-variable", "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gtsam_points_b200", "cpp", "include")]
-    if mock_gtsam:
-        cmd += ["-I", MOCK]
-    cmd += [SRC, "-o", exe, "-L", LIBDIR, "-lb2points", f"-Wl,-rpath,{LIBDIR}"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    return exe
+import native
 
 
 @pytest.mark.parametrize("mock_gtsam", [False, True])
-def test_ivox_cov_adapter_compiles(tmp_path, mock_gtsam):
-    from gtsam_points_b200 import build
-
-    build.build()
-    exe = build_driver(tmp_path, mock_gtsam)
+def test_ivox_cov_adapter_compiles(mock_gtsam):
+    exe = native.adapter_driver("test_ivox_cov", mock_gtsam)
     syms = subprocess.run(["nm", "-C", exe], capture_output=True, text=True).stdout
     assert "gtsam_points_b200::iVoxCovarianceEstimationGPU" in syms
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("mock_gtsam", [False, True])
-def test_ivox_cov_driver_in_optimizer_call_order(tmp_path, mock_gtsam):
+def test_ivox_cov_driver_in_optimizer_call_order(mock_gtsam):
     import ivox_cov_np
     import ivox_np
     import np_ref
     from gtsam_points_b200 import synthetic as syn
     from test_ivox_cov_cpu import reduced, scene_frames
 
-    exe = build_driver(tmp_path, mock_gtsam)
+    exe = native.adapter_driver("test_ivox_cov", mock_gtsam)
     frames = scene_frames(3)
     ref = reduced(ivox_cov_np.IvoxCovNp(1.0))
     for p in frames[:2]:
@@ -81,14 +63,6 @@ def test_ivox_cov_driver_in_optimizer_call_order(tmp_path, mock_gtsam):
 
     pad44 = np.zeros((n, 4, 4))
     pad44[:, :3, :3] = sc
-    case = tmp_path / "case.bin"
-    with open(case, "wb") as f:
-        arrays = [frames[0], frames[1], frames[2], np.concatenate([sp, np.ones((n, 1))], 1), pad44, Ts, Ts2]
-        arrays += [vidx.astype(np.float64), ex["points"][valid], ex["normals"][valid], ex["covs"][valid], q, force, record(lin), np.array([err]), corr.astype(np.float64), record(lin2)]
-        for a in arrays:
-            a = np.ascontiguousarray(a, dtype=np.float64).ravel()
-            f.write(np.uint64(a.size).tobytes())
-            f.write(a.tobytes())
-    r = subprocess.run([exe, str(case)], capture_output=True, text=True, timeout=180)
-    assert r.returncode == 0, r.stdout + r.stderr
-    assert "OK" in r.stdout
+    arrays = [frames[0], frames[1], frames[2], np.concatenate([sp, np.ones((n, 1))], 1), pad44, Ts, Ts2]
+    arrays += [vidx.astype(np.float64), ex["points"][valid], ex["normals"][valid], ex["covs"][valid], q, force, record(lin), np.array([err]), corr.astype(np.float64), record(lin2)]
+    native.run_driver(exe, arrays, timeout=180)

@@ -2,35 +2,17 @@
 standalone and in their GTSAM-typed form against the header mocks (tests/cpp/mock_gtsam).  On a GPU box the driver
 (tests/cpp/test_ivox.cpp) runs in the optimizer's call order and is checked against the Python restatement of the iVox
 (tests/ivox_np.py) with np_ref's GICP algebra."""
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "cpp", "test_ivox.cpp")
-LIBDIR = os.path.join(ROOT, "gtsam_points_b200", "lib")
-MOCK = os.path.join(ROOT, "tests", "cpp", "mock_gtsam")
-
-
-def build_driver(tmp_path, mock_gtsam: bool):
-    exe = str(tmp_path / ("test_ivox_gtsam" if mock_gtsam else "test_ivox"))
-    cmd = ["/usr/bin/g++", "-std=c++17", "-O2", "-Wall", "-Wno-unused-variable", "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gtsam_points_b200", "cpp", "include")]
-    if mock_gtsam:
-        cmd += ["-I", MOCK]
-    cmd += [SRC, "-o", exe, "-L", LIBDIR, "-lb2points", f"-Wl,-rpath,{LIBDIR}"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    return exe
+import native
 
 
 @pytest.mark.parametrize("mock_gtsam", [False, True])
-def test_ivox_adapters_compile(tmp_path, mock_gtsam):
-    from gtsam_points_b200 import build
-
-    build.build()
-    exe = build_driver(tmp_path, mock_gtsam)
+def test_ivox_adapters_compile(mock_gtsam):
+    exe = native.adapter_driver("test_ivox", mock_gtsam)
     syms = subprocess.run(["nm", "-C", exe], capture_output=True, text=True).stdout
     assert "gtsam_points_b200::iVoxGPU" in syms
     if mock_gtsam:
@@ -39,12 +21,12 @@ def test_ivox_adapters_compile(tmp_path, mock_gtsam):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("mock_gtsam", [False, True])
-def test_ivox_driver_in_optimizer_call_order(tmp_path, mock_gtsam):
+def test_ivox_driver_in_optimizer_call_order(mock_gtsam):
     import ivox_np
     from gtsam_points_b200 import synthetic as syn
     from test_ivox_cpu import trajectory_frames
 
-    exe = build_driver(tmp_path, mock_gtsam)
+    exe = native.adapter_driver("test_ivox", mock_gtsam)
     frames = trajectory_frames(num_frames=3)
     ref = ivox_np.IvoxNp(1.0)
     ref.lru_horizon, ref.lru_clear_cycle = 10, 10
@@ -78,14 +60,6 @@ def test_ivox_driver_in_optimizer_call_order(tmp_path, mock_gtsam):
         m[:, :3, :3] = c
         return m
 
-    case = tmp_path / "case.bin"
-    with open(case, "wb") as f:
-        arrays = [frames[0][0], frames[0][1], frames[1][0], frames[1][1], frames[2][0], frames[2][1], pad4(sp), pad44(sc), Ts, Ts2]
-        arrays += [record(lin), np.array([err]), corr.astype(np.float64), q, knn, record(lin2)]
-        for a in arrays:
-            a = np.ascontiguousarray(a, dtype=np.float64).ravel()
-            f.write(np.uint64(a.size).tobytes())
-            f.write(a.tobytes())
-    r = subprocess.run([exe, str(case)], capture_output=True, text=True, timeout=180)
-    assert r.returncode == 0, r.stdout + r.stderr
-    assert "OK" in r.stdout
+    arrays = [frames[0][0], frames[0][1], frames[1][0], frames[1][1], frames[2][0], frames[2][1], pad4(sp), pad44(sc), Ts, Ts2]
+    arrays += [record(lin), np.array([err]), corr.astype(np.float64), q, knn, record(lin2)]
+    native.run_driver(exe, arrays, timeout=180)

@@ -2,47 +2,29 @@
 set_enable_surface_validation, point-to-plane IntegratedICPFactor over a target cloud with normals) compile against the C ABI --
 standalone and against the header mocks (tests/cpp/mock_gtsam).  On a GPU box the driver (tests/cpp/test_normals.cpp) is
 checked against the host restatement of surface validation (tests/normals_ref.py)."""
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "cpp", "test_normals.cpp")
-LIBDIR = os.path.join(ROOT, "gtsam_points_b200", "lib")
-MOCK = os.path.join(ROOT, "tests", "cpp", "mock_gtsam")
-
-
-def build_driver(tmp_path, mock_gtsam: bool):
-    exe = str(tmp_path / ("test_normals_gtsam" if mock_gtsam else "test_normals"))
-    cmd = ["/usr/bin/g++", "-std=c++17", "-O2", "-Wall", "-Wno-unused-variable", "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gtsam_points_b200", "cpp", "include")]
-    if mock_gtsam:
-        cmd += ["-I", MOCK]
-    cmd += [SRC, "-o", exe, "-L", LIBDIR, "-lb2points", f"-Wl,-rpath,{LIBDIR}"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    return exe
+import native
 
 
 @pytest.mark.parametrize("mock_gtsam", [False, True])
-def test_normals_adapters_compile(tmp_path, mock_gtsam):
-    from gtsam_points_b200 import build
-
-    build.build()
-    exe = build_driver(tmp_path, mock_gtsam)
+def test_normals_adapters_compile(mock_gtsam):
+    exe = native.adapter_driver("test_normals", mock_gtsam)
     syms = subprocess.run(["nm", "-C", exe], capture_output=True, text=True).stdout
     assert "b2_factor_set_enable_surface_validation" in syms and "b2_cloud_create_with_normals" in syms
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("mock_gtsam", [False, True])
-def test_normals_driver(tmp_path, mock_gtsam):
+def test_normals_driver(mock_gtsam):
     import normals_ref as nref
     import oracle_lib as orc
     from gtsam_points_b200 import synthetic as syn
 
-    exe = build_driver(tmp_path, mock_gtsam)
+    exe = native.adapter_driver("test_normals", mock_gtsam)
     tp, tc = syn.make_cloud(8000, stream=1, scale=0.25)
     sp, sc = syn.make_cloud(5000, stream=2, scale=0.25)
     nrm = nref.normals_from_covs(sp, sc)
@@ -66,12 +48,4 @@ def test_normals_driver(tmp_path, mock_gtsam):
         m[:, :3, :3] = c
         return m
 
-    case = tmp_path / "case.bin"
-    with open(case, "wb") as f:
-        for a in [pad4(tp, 1.0), pad44(tc), pad4(sp, 1.0), pad44(sc), pad4(nrm, 0.0), tn, T, np.array(inliers), val.correspondences()]:
-            a = np.ascontiguousarray(a, dtype=np.float64).ravel()
-            f.write(np.uint64(a.size).tobytes())
-            f.write(a.tobytes())
-    r = subprocess.run([exe, str(case)], capture_output=True, text=True, timeout=180)
-    assert r.returncode == 0, r.stdout + r.stderr
-    assert "OK" in r.stdout
+    native.run_driver(exe, [pad4(tp, 1.0), pad44(tc), pad4(sp, 1.0), pad44(sc), pad4(nrm, 0.0), tn, T, np.array(inliers), val.correspondences()], timeout=180)

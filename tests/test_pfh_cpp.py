@@ -1,35 +1,17 @@
 """The C++ adapters' PFH and keypoint feature path (estimate_pfh_gpu, the indices overloads, PFHEstimationParams) compiles against
 the C ABI -- standalone and against the header mocks (tests/cpp/mock_gtsam).  On a GPU box the driver (tests/cpp/test_pfh.cpp) is
 checked against the CPU registration oracle."""
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "cpp", "test_pfh.cpp")
-LIBDIR = os.path.join(ROOT, "gtsam_points_b200", "lib")
-MOCK = os.path.join(ROOT, "tests", "cpp", "mock_gtsam")
-
-
-def build_driver(tmp_path, mock_gtsam: bool):
-    exe = str(tmp_path / ("test_pfh_gtsam" if mock_gtsam else "test_pfh"))
-    cmd = ["/usr/bin/g++", "-std=c++17", "-O2", "-Wall", "-Wno-unused-variable", "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gtsam_points_b200", "cpp", "include")]
-    if mock_gtsam:
-        cmd += ["-I", MOCK]
-    cmd += [SRC, "-o", exe, "-L", LIBDIR, "-lb2points", f"-Wl,-rpath,{LIBDIR}"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    return exe
+import native
 
 
 @pytest.mark.parametrize("mock_gtsam", [False, True])
-def test_pfh_adapters_compile(tmp_path, mock_gtsam):
-    from gtsam_points_b200 import build
-
-    build.build()
-    exe = build_driver(tmp_path, mock_gtsam)
+def test_pfh_adapters_compile(mock_gtsam):
+    exe = native.adapter_driver("test_pfh", mock_gtsam)
     syms = subprocess.run(["nm", "-C", exe], capture_output=True, text=True).stdout
     for s in ("b2_features_create_pfh", "b2_features_create_fpfh_at", "b2_features_create_fpfh", "b2_features_download"):
         assert s in syms
@@ -37,26 +19,18 @@ def test_pfh_adapters_compile(tmp_path, mock_gtsam):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("mock_gtsam", [False, True])
-def test_pfh_driver(tmp_path, mock_gtsam):
+def test_pfh_driver(mock_gtsam):
     import registration_cases as rc
-    import pfh_oracle as po
+    import registration_oracle as ro
 
-    exe = build_driver(tmp_path, mock_gtsam)
+    exe = native.adapter_driver("test_pfh", mock_gtsam)
     P, N = rc.small_scene(700, seed=8, extent=8.0)
     idx = np.array([699, 3, 41, 3, 0, 512])
     radius = 1.5
-    pf, pe, _ = po.pfh(P, N, radius, 10000, indices=idx)
-    ff, fe, _ = po.fpfh_at(P, N, idx, radius, 10000)
+    pf, pe, _ = ro.pfh(P, N, radius, 10000, indices=idx)
+    ff, fe, _ = ro.fpfh_at(P, N, idx, radius, 10000)
 
     def pad(a, w):
         return np.concatenate([a, np.full((len(a), 1), w)], 1)
 
-    case = tmp_path / "case.bin"
-    with open(case, "wb") as f:
-        for a in [pad(P, 1.0), pad(N, 0.0), idx, pf, pe, ff, fe, [radius]]:
-            a = np.ascontiguousarray(a, dtype=np.float64).ravel()
-            f.write(np.uint64(a.size).tobytes())
-            f.write(a.tobytes())
-    res = subprocess.run([exe, str(case)], capture_output=True, text=True, timeout=300)
-    assert res.returncode == 0, res.stdout + res.stderr
-    assert "OK" in res.stdout
+    native.run_driver(exe, [pad(P, 1.0), pad(N, 0.0), idx, pf, pe, ff, fe, [radius]], timeout=300)

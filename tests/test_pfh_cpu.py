@@ -1,11 +1,10 @@
-"""The PFH oracle's PFH (orc_pfh) and FPFH at chosen points (orc_fpfh_at, tests/pfh_oracle.cpp) against plain numpy restatements of the formulas
+"""The registration oracle's PFH (orc_pfh) and FPFH at chosen points (orc_fpfh_at, tests/registration_oracle.cpp) against plain numpy restatements of the formulas
 include/b2points.h states for b2_features_create_pfh and b2_features_create_fpfh_at, on small scenes."""
 import math
 
 import numpy as np
 import pytest
 
-import pfh_oracle as po
 import registration_cases as rc
 import registration_oracle as ro
 from test_registration_cpu import np_fpfh
@@ -84,7 +83,7 @@ def scene(n=160, seed=3):
 @pytest.mark.parametrize("max_nn", [10000, 12])
 def test_oracle_pfh_matches_numpy(max_nn):
     P, N = scene()
-    got, edge, nn = po.pfh(P, N, 1.5, max_nn, num_threads=2)
+    got, edge, nn = ro.pfh(P, N, 1.5, max_nn, num_threads=2)
     want = np_pfh(P, N, 1.5, max_nn)
     assert np.array_equal(got, want)
     assert not edge.any()
@@ -99,7 +98,7 @@ def test_oracle_pfh_matches_numpy(max_nn):
 
 def test_oracle_pfh_follows_the_reference_pair_orientation():
     P, N = scene()
-    got, _, _ = po.pfh(P, N, 1.5, 10000, num_threads=2)
+    got, _, _ = ro.pfh(P, N, 1.5, 10000, num_threads=2)
     rev = np_pfh(P, N, 1.5, 10000, reverse=True)
     differ = np.nonzero((got != rev).any(axis=1))[0]
     assert TIE in differ and TIE + 1 in differ  # so the oracle's rows are those of (N[i], N[j])
@@ -109,18 +108,18 @@ def test_oracle_pfh_follows_the_reference_pair_orientation():
 def test_oracle_pfh_at_indices():
     P, N = scene()
     idx = np.array([7, ISOLATED, 3, 7, 0, 160, TIE + 1, 159])  # unsorted, a duplicate, the isolated and a coincident point
-    got, _, nn = po.pfh(P, N, 1.5, 10000, num_threads=2, indices=idx)
-    full, _, nn_full = po.pfh(P, N, 1.5, 10000, num_threads=2)
+    got, _, nn = ro.pfh(P, N, 1.5, 10000, num_threads=2, indices=idx)
+    full, _, nn_full = ro.pfh(P, N, 1.5, 10000, num_threads=2)
     assert np.array_equal(got, full[idx]) and np.array_equal(nn, nn_full[idx])
     assert np.array_equal(got, np_pfh(P, N, 1.5, 10000, indices=idx))
-    assert po.pfh(P, N, 1.5, 10000, indices=np.zeros(0, dtype=np.int64))[0].shape == (0, 125)
+    assert ro.pfh(P, N, 1.5, 10000, indices=np.zeros(0, dtype=np.int64))[0].shape == (0, 125)
 
 
 @pytest.mark.parametrize("max_nn", [10000, 12])
 def test_oracle_fpfh_at_indices(max_nn):
     P, N = scene()
     idx = np.array([9, 2, ISOLATED, 2, 5, TIE, 100])
-    got, edge, nn = po.fpfh_at(P, N, idx, 1.5, max_nn, num_threads=2)
+    got, edge, nn = ro.fpfh_at(P, N, idx, 1.5, max_nn, num_threads=2)
     full, edge_full, nn_full = ro.fpfh(P, N, 1.5, max_nn, num_threads=2)
     assert np.array_equal(got, full[idx]) and np.array_equal(edge, edge_full[idx]) and np.array_equal(nn, nn_full[idx])
     want, want_nn = np_fpfh(P, N, 1.5, max_nn)

@@ -1,38 +1,19 @@
 """The C++ adapters' map updates from device clouds (GaussianVoxelMapGPU::insert_cloud, iVoxGPU::insert_cloud, transform_gpu,
 merge_frames_gpu) compile against the C ABI -- standalone and against the header mocks (tests/cpp/mock_gtsam).  On a GPU box the
 driver (tests/cpp/test_posed_frames.cpp) checks them against the host-array path over the numpy-posed arrays."""
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
 import adversarial as adv
+import native
 import posed_ref
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "cpp", "test_posed_frames.cpp")
-LIBDIR = os.path.join(ROOT, "gtsam_points_b200", "lib")
-MOCK = os.path.join(ROOT, "tests", "cpp", "mock_gtsam")
-
-
-def build_driver(tmp_path, mock_gtsam: bool):
-    exe = str(tmp_path / ("test_posed_frames_gtsam" if mock_gtsam else "test_posed_frames"))
-    cmd = ["/usr/bin/g++", "-std=c++17", "-O2", "-Wall", "-Wno-unused-variable", "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gtsam_points_b200", "cpp", "include")]
-    if mock_gtsam:
-        cmd += ["-I", MOCK]
-    cmd += [SRC, "-o", exe, "-L", LIBDIR, "-lb2points", f"-Wl,-rpath,{LIBDIR}"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    return exe
 
 
 @pytest.mark.parametrize("mock_gtsam", [False, True])
-def test_posed_frames_adapters_compile(tmp_path, mock_gtsam):
-    from gtsam_points_b200 import build
-
-    build.build()
-    exe = build_driver(tmp_path, mock_gtsam)
+def test_posed_frames_adapters_compile(mock_gtsam):
+    exe = native.adapter_driver("test_posed_frames", mock_gtsam)
     syms = subprocess.run(["nm", "-C", exe], capture_output=True, text=True).stdout
     for s in ("b2_voxelmap_insert_cloud", "b2_ivox_insert_cloud", "b2_cloud_create_transformed", "b2_merge_frames_to_cloud"):
         assert s in syms
@@ -40,21 +21,13 @@ def test_posed_frames_adapters_compile(tmp_path, mock_gtsam):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("mock_gtsam", [False, True])
-def test_posed_frames_driver(tmp_path, mock_gtsam):
+def test_posed_frames_driver(mock_gtsam):
     from gtsam_points_b200 import synthetic as syn
 
-    exe = build_driver(tmp_path, mock_gtsam)
+    exe = native.adapter_driver("test_posed_frames", mock_gtsam)
     rng = np.random.default_rng(8)
     pts = rng.uniform(-8, 8, (4000, 3))
     covs = adv.spd(len(pts), 3)
     T = syn.random_pose(rng, 0.5, 3.0)
     q, qc, _ = posed_ref.transform(T, pts, covs)
-    case = tmp_path / "case.bin"
-    with open(case, "wb") as f:
-        for a in [pts, covs, T, q, qc]:
-            a = np.ascontiguousarray(a, dtype=np.float64).ravel()
-            f.write(np.uint64(a.size).tobytes())
-            f.write(a.tobytes())
-    r = subprocess.run([exe, str(case)], capture_output=True, text=True, timeout=180)
-    assert r.returncode == 0, r.stdout + r.stderr
-    assert "OK" in r.stdout
+    native.run_driver(exe, [pts, covs, T, q, qc], timeout=180)

@@ -7,29 +7,12 @@ import subprocess
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "cpp", "test_preprocess.cpp")
-LIBDIR = os.path.join(ROOT, "gtsam_points_b200", "lib")
-MOCK = os.path.join(ROOT, "tests", "cpp", "mock_gtsam")
-
-
-def build_driver(tmp_path, mock_gtsam: bool):
-    exe = str(tmp_path / ("test_preprocess_gtsam" if mock_gtsam else "test_preprocess"))
-    cmd = ["/usr/bin/g++", "-std=c++17", "-O2", "-Wall", "-Wno-unused-variable", "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gtsam_points_b200", "cpp", "include")]
-    if mock_gtsam:
-        cmd += ["-I", MOCK]
-    cmd += [SRC, "-o", exe, "-L", LIBDIR, "-lb2points", f"-Wl,-rpath,{LIBDIR}"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    return exe
+import native
 
 
 @pytest.mark.parametrize("mock_gtsam", [False, True])
-def test_preprocess_adapters_compile(tmp_path, mock_gtsam):
-    from gtsam_points_b200 import build
-
-    build.build()
-    exe = build_driver(tmp_path, mock_gtsam)
+def test_preprocess_adapters_compile(mock_gtsam):
+    exe = native.adapter_driver("test_preprocess", mock_gtsam)
     syms = subprocess.run(["nm", "-C", exe], capture_output=True, text=True).stdout
     for s in ("b2_cloud_create_voxelgrid", "b2_cloud_create_estimated", "b2_kdtree_create_from_cloud", "b2_cloud_download"):
         assert s in syms
@@ -37,12 +20,12 @@ def test_preprocess_adapters_compile(tmp_path, mock_gtsam):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("mock_gtsam", [False, True])
-def test_preprocess_driver(tmp_path, mock_gtsam):
+def test_preprocess_driver(mock_gtsam):
     import voxelgrid_oracle as vo
     from gtsam_points_b200 import synthetic as syn
 
-    exe = build_driver(tmp_path, mock_gtsam)
-    k00 = np.load(os.path.join(ROOT, "tests", "golden", "kitti00_pair.npz"))
+    exe = native.adapter_driver("test_preprocess", mock_gtsam)
+    k00 = np.load(os.path.join(native.ROOT, "tests", "golden", "kitti00_pair.npz"))
     tp, sp = k00["frame0"], k00["frame1"]
     res = 0.25
     want = vo.voxelgrid_sampling(tp, res)[0]
@@ -51,12 +34,4 @@ def test_preprocess_driver(tmp_path, mock_gtsam):
     def pad4(p):
         return np.concatenate([p, np.ones((len(p), 1))], 1)
 
-    case = tmp_path / "case.bin"
-    with open(case, "wb") as f:
-        for a in [pad4(tp), pad4(sp), np.array([res]), want, delta]:
-            a = np.ascontiguousarray(a, dtype=np.float64).ravel()
-            f.write(np.uint64(a.size).tobytes())
-            f.write(a.tobytes())
-    r = subprocess.run([exe, str(case)], capture_output=True, text=True, timeout=180)
-    assert r.returncode == 0, r.stdout + r.stderr
-    assert "OK" in r.stdout
+    native.run_driver(exe, [pad4(tp), pad4(sp), np.array([res]), want, delta], timeout=180)

@@ -1,35 +1,17 @@
 """The C++ adapters' global registration path (FeaturesGPU, estimate_fpfh_gpu, estimate_pose_ransac_gpu) compiles against the C ABI --
 standalone and against the header mocks (tests/cpp/mock_gtsam).  On a GPU box the driver (tests/cpp/test_registration.cpp) is checked
 against the CPU registration oracle."""
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "cpp", "test_registration.cpp")
-LIBDIR = os.path.join(ROOT, "gtsam_points_b200", "lib")
-MOCK = os.path.join(ROOT, "tests", "cpp", "mock_gtsam")
-
-
-def build_driver(tmp_path, mock_gtsam: bool):
-    exe = str(tmp_path / ("test_registration_gtsam" if mock_gtsam else "test_registration"))
-    cmd = ["/usr/bin/g++", "-std=c++17", "-O2", "-Wall", "-Wno-unused-variable", "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gtsam_points_b200", "cpp", "include")]
-    if mock_gtsam:
-        cmd += ["-I", MOCK]
-    cmd += [SRC, "-o", exe, "-L", LIBDIR, "-lb2points", f"-Wl,-rpath,{LIBDIR}"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    return exe
+import native
 
 
 @pytest.mark.parametrize("mock_gtsam", [False, True])
-def test_registration_adapters_compile(tmp_path, mock_gtsam):
-    from gtsam_points_b200 import build
-
-    build.build()
-    exe = build_driver(tmp_path, mock_gtsam)
+def test_registration_adapters_compile(mock_gtsam):
+    exe = native.adapter_driver("test_registration", mock_gtsam)
     syms = subprocess.run(["nm", "-C", exe], capture_output=True, text=True).stdout
     for s in ("b2_features_create", "b2_features_create_fpfh", "b2_estimate_pose_ransac", "b2_features_download"):
         assert s in syms
@@ -37,13 +19,13 @@ def test_registration_adapters_compile(tmp_path, mock_gtsam):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("mock_gtsam", [False, True])
-def test_registration_driver(tmp_path, mock_gtsam):
+def test_registration_driver(mock_gtsam):
     import normals_ref
     import registration_cases as rc
     import registration_oracle as ro
     import voxelgrid_oracle as vo
 
-    exe = build_driver(tmp_path, mock_gtsam)
+    exe = native.adapter_driver("test_registration", mock_gtsam)
     d = rc.kitti00()
     tgt = vo.voxelgrid_sampling(d["frame0"], 0.5)[0]
     src = vo.voxelgrid_sampling(d["frame1"], 0.5)[0]
@@ -60,12 +42,4 @@ def test_registration_driver(tmp_path, mock_gtsam):
     def pad(a, w):
         return np.concatenate([a, np.full((len(a), 1), w)], 1)
 
-    case = tmp_path / "case.bin"
-    with open(case, "wb") as f:
-        for a in [pad(tgt, 1.0), pad(tn, 0.0), pad(src, 1.0), pad(sn, 0.0), tf, sf, np.concatenate([te, se]).astype(np.float64), want]:
-            a = np.ascontiguousarray(a, dtype=np.float64).ravel()
-            f.write(np.uint64(a.size).tobytes())
-            f.write(a.tobytes())
-    res = subprocess.run([exe, str(case)], capture_output=True, text=True, timeout=300)
-    assert res.returncode == 0, res.stdout + res.stderr
-    assert "OK" in res.stdout
+    native.run_driver(exe, [pad(tgt, 1.0), pad(tn, 0.0), pad(src, 1.0), pad(sn, 0.0), tf, sf, np.concatenate([te, se]).astype(np.float64), want], timeout=300)

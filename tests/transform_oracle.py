@@ -1,22 +1,21 @@
 """ctypes binding of tests/transform_oracle.cpp, the CPU oracle's transform(frame, T) -- TEST INFRASTRUCTURE ONLY.
 
-The library (the oracle's sources plus orc_transform) is compiled on first use into a temporary directory (the source tree may be
-read-only) by the compiler and flags that oracle/Makefile builds liboracle.so with, read from the Makefile itself.
+The library (the oracle's sources plus orc_transform) is compiled on first use by tests/native.py, with the compiler and flags that
+oracle/Makefile builds liboracle.so with, read from the Makefile itself.
 """
-import atexit
 import ctypes as C
+import functools
 import os
 import shlex
-import shutil
 import subprocess
-import tempfile
 
 import numpy as np
+
+import native
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "transform_oracle.cpp")
 ORACLE_DIR = os.path.join(os.path.dirname(HERE), "oracle")
-_LIB = None
 
 
 def oracle_compile_command():
@@ -26,22 +25,17 @@ def oracle_compile_command():
     return shlex.split(out.strip())
 
 
+@functools.cache
 def lib():
-    global _LIB
-    if _LIB is None:
-        tmp = tempfile.mkdtemp(prefix="b2_transform_oracle_")
-        atexit.register(shutil.rmtree, tmp, True)
-        so = os.path.join(tmp, "libtransform_oracle.so")
-        subprocess.check_call(oracle_compile_command() + ["-shared", "-o", so, SRC])
-        L = C.CDLL(so)
-        vp, dp = C.c_void_p, C.POINTER(C.c_double)
-        L.orc_cloud_create.restype = vp
-        L.orc_cloud_create.argtypes = [dp, dp, C.c_size_t]
-        L.orc_cloud_destroy.argtypes = [vp]
-        L.orc_cloud_set_normals.argtypes = [vp, dp]
-        L.orc_transform.argtypes = [dp, vp, dp, dp, dp]
-        _LIB = L
-    return _LIB
+    cxx, *flags = oracle_compile_command()
+    L = native.shared_library([SRC], flags + ["-shared"], cxx)
+    vp, dp = C.c_void_p, C.POINTER(C.c_double)
+    L.orc_cloud_create.restype = vp
+    L.orc_cloud_create.argtypes = [dp, dp, C.c_size_t]
+    L.orc_cloud_destroy.argtypes = [vp]
+    L.orc_cloud_set_normals.argtypes = [vp, dp]
+    L.orc_transform.argtypes = [dp, vp, dp, dp, dp]
+    return L
 
 
 def _dp(a):

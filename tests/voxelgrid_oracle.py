@@ -1,37 +1,25 @@
-"""ctypes binding of tests/voxelgrid_oracle.cpp, the CPU restatement of voxelgrid_sampling -- TEST INFRASTRUCTURE ONLY.
-
-The library is compiled on first use into a temporary directory (the source tree may be read-only), with the CPU oracle's
-flags: -O3 -fopenmp -ffp-contract=off.
+"""ctypes binding of tests/voxelgrid_oracle.cpp, the CPU restatement of voxelgrid_sampling -- TEST INFRASTRUCTURE ONLY.  The library
+is compiled on first use by tests/native.py with the CPU oracles' flags.
 """
-import atexit
 import ctypes as C
+import functools
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, "voxelgrid_oracle.cpp")
-FLAGS = ["-O3", "-std=c++17", "-fopenmp", "-fPIC", "-ffp-contract=off", "-Wall", "-shared"]
-_LIB = None
+import native
+
+SRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "voxelgrid_oracle.cpp")
 
 
+@functools.cache
 def lib():
-    global _LIB
-    if _LIB is None:
-        tmp = tempfile.mkdtemp(prefix="b2_voxelgrid_oracle_")
-        atexit.register(shutil.rmtree, tmp, True)
-        so = os.path.join(tmp, "libvoxelgrid_oracle.so")
-        subprocess.check_call(["/usr/bin/g++"] + FLAGS + ["-o", so, SRC])
-        L = C.CDLL(so)
-        dp = C.POINTER(C.c_double)
-        L.orc_voxelgrid_sampling.restype = C.c_size_t
-        L.orc_voxelgrid_sampling.argtypes = [C.c_double, dp, C.c_int, dp, C.c_int, dp, C.c_int, C.c_size_t, C.c_int, dp, dp, dp]
-        L.orc_voxelgrid_max_threads.restype = C.c_int
-        _LIB = L
-    return _LIB
+    L = native.shared_library([SRC], native.ORACLE_FLAGS)
+    dp = C.POINTER(C.c_double)
+    L.orc_voxelgrid_sampling.restype = C.c_size_t
+    L.orc_voxelgrid_sampling.argtypes = [C.c_double, dp, C.c_int, dp, C.c_int, dp, C.c_int, C.c_size_t, C.c_int, dp, dp, dp]
+    L.orc_voxelgrid_max_threads.restype = C.c_int
+    return L
 
 
 def max_threads():

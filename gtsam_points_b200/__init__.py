@@ -19,6 +19,25 @@ from .factors import (  # noqa: F401
     pose_inverse,
 )
 from .registration import Features, GNCParams, RANSACParams, RegistrationResult, estimate_fpfh, estimate_pfh, estimate_pose_gnc, estimate_pose_ransac  # noqa: F401
-from .types import Context, GaussianVoxelMapGPU, KdTree, PointCloud, default_context, estimate_covariances, estimate_normals, iVox, iVoxCovarianceEstimation, merge_frames_gpu, overlap_gpu, transform_gpu, voxelgrid_sampling  # noqa: F401
+from .types import (  # noqa: F401
+    Context,
+    GaussianVoxelMapGPU,
+    KdTree,
+    PointCloud,
+    default_context,
+    estimate_covariances,
+    estimate_normals,
+    find_inlier_points,
+    iVox,
+    iVoxCovarianceEstimation,
+    merge_frames_gpu,
+    overlap_gpu,
+    random_sampling,
+    randomgrid_sampling,
+    remove_outliers,
+    sample,
+    transform_gpu,
+    voxelgrid_sampling,
+)
 
 __version__ = "0.1.0"

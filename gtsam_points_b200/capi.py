@@ -89,6 +89,10 @@ SIGNATURES = {
     "b2_cloud_create_voxelgrid": (C.c_int, [_vp, C.c_double, _dp, C.c_int, _dp, C.c_int, _dp, C.c_int, C.c_size_t, C.c_uint, _pp]),
     "b2_cloud_create_estimated": (C.c_int, [_vp, _vp, C.c_int, _dp, C.c_int, C.c_uint, _pp]),
     "b2_cloud_create_transformed": (C.c_int, [_vp, _dp, C.c_uint, _pp]),
+    "b2_cloud_create_sampled": (C.c_int, [_vp, _lp, C.c_size_t, C.c_uint, _pp]),
+    "b2_cloud_create_random_sampled": (C.c_int, [_vp, C.c_double, C.c_uint64, C.c_uint, _lp, _pp]),
+    "b2_cloud_create_randomgrid": (C.c_int, [_vp, C.c_double, C.c_double, C.c_uint64, C.c_uint, _lp, _pp]),
+    "b2_cloud_create_inliers": (C.c_int, [_vp, _vp, C.c_int, C.c_double, C.c_uint, _dp, _dp, _lp, _pp]),
     "b2_cloud_destroy": (C.c_int, [_vp]),
     "b2_cloud_get_info": (C.c_int, [_vp, C.POINTER(CloudInfo)]),
     "b2_voxelmap_create_from_points": (C.c_int, [_vp, C.c_double, _dp, C.c_int, _dp, C.c_int, C.c_size_t, _pp]),

@@ -407,6 +407,49 @@ inline PointCloudGPU::Ptr transform_gpu(const PointCloudGPU::ConstPtr& cloud, co
   return PointCloudGPU::adopt(out, cloud->context());
 }
 
+// Frame filtering of a device cloud into a new device cloud (types/point_cloud_cpu.hpp), with the reference's argument order: each
+// result is the cloud b2_cloud_create makes of the downloaded rows it selects (see include/b2points.h).  Where the reference takes a
+// std::mt19937&, these take the seed of the library's counter-based stream; the distribution is the same.
+// sample(frame, indices) (point_cloud_cpu_funcs.cpp:27-75)
+inline PointCloudGPU::Ptr sample_gpu(const PointCloudGPU::ConstPtr& frame, const std::vector<int>& indices, unsigned flags = B2_CLOUD_DEFAULT) {
+  const std::vector<std::int64_t> idx(indices.begin(), indices.end());
+  b2_cloud* out = nullptr;
+  check(b2_cloud_create_sampled(frame->handle(), idx.data(), idx.size(), flags, &out), "b2_cloud_create_sampled");
+  return PointCloudGPU::adopt(out, frame->context());
+}
+// random_sampling(frame, sampling_rate, mt) (point_cloud_cpu_funcs.cpp:77-93)
+inline PointCloudGPU::Ptr random_sampling_gpu(const PointCloudGPU::ConstPtr& frame, double sampling_rate, std::uint64_t seed, unsigned flags = B2_CLOUD_DEFAULT) {
+  b2_cloud* out = nullptr;
+  check(b2_cloud_create_random_sampled(frame->handle(), sampling_rate, seed, flags, nullptr, &out), "b2_cloud_create_random_sampled");
+  return PointCloudGPU::adopt(out, frame->context());
+}
+// randomgrid_sampling(frame, voxel_resolution, sampling_rate, mt) (point_cloud_cpu_funcs.cpp:297-456); the device pass has no thread count
+inline PointCloudGPU::Ptr randomgrid_sampling_gpu(const PointCloudGPU::ConstPtr& frame, double voxel_resolution, double sampling_rate, std::uint64_t seed,
+                                                  unsigned flags = B2_CLOUD_DEFAULT) {
+  b2_cloud* out = nullptr;
+  check(b2_cloud_create_randomgrid(frame->handle(), voxel_resolution, sampling_rate, seed, flags, nullptr, &out), "b2_cloud_create_randomgrid");
+  return PointCloudGPU::adopt(out, frame->context());
+}
+// remove_outliers(frame, k, std_thresh) (point_cloud_cpu_funcs.cpp:576-650); tree: null, or a KdTreeGPU built from this frame
+inline PointCloudGPU::Ptr remove_outliers_gpu(const PointCloudGPU::ConstPtr& frame, int k = 10, double std_thresh = 1.0, const KdTreeGPU* tree = nullptr,
+                                              unsigned flags = B2_CLOUD_DEFAULT) {
+  b2_cloud* out = nullptr;
+  check(b2_cloud_create_inliers(frame->handle(), tree ? tree->handle() : nullptr, k, std_thresh, flags, nullptr, nullptr, nullptr, &out), "b2_cloud_create_inliers");
+  return PointCloudGPU::adopt(out, frame->context());
+}
+// find_inlier_points(frame, neighbors, k, std_thresh) (point_cloud_cpu_funcs.cpp:576-613) with the k-NN search on the device: the
+// caller indices remove_outliers_gpu keeps, ascending
+inline std::vector<int> find_inlier_points_gpu(const PointCloudGPU::ConstPtr& frame, int k = 10, double std_thresh = 1.0, const KdTreeGPU* tree = nullptr) {
+  std::vector<std::int64_t> idx(std::max<std::size_t>(frame->size(), 1));
+  b2_cloud* out = nullptr;
+  check(b2_cloud_create_inliers(frame->handle(), tree ? tree->handle() : nullptr, k, std_thresh, B2_CLOUD_DEFAULT, nullptr, nullptr, idx.data(), &out), "b2_cloud_create_inliers");
+  b2_cloud_info info{};
+  const b2_status st = b2_cloud_get_info(out, &info);
+  b2_cloud_destroy(out);
+  check(st, "b2_cloud_get_info");
+  return std::vector<int>(idx.begin(), idx.begin() + info.num_points);
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // Global registration (features/fpfh_estimation.hpp, registration/ransac.hpp, registration/graduated_non_convexity.hpp): features,
 // FPFH, RANSAC and GNC on the device

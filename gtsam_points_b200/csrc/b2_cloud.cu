@@ -277,24 +277,14 @@ b2_status average_voxels(const DeviceBuffer& keys, const DeviceBuffer& vals, con
   *m = 0;
   if (count == 0) return B2_OK;
   const size_t n = in.n;
-  DeviceBuffer keys2, vals2, flags, incl, starts, tmp;
+  DeviceBuffer keys2, vals2, incl, starts, tmp;
   B2_TRY(keys2.alloc(n * sizeof(unsigned long long)));
   B2_TRY(vals2.alloc(n * sizeof(uint32_t)));
   B2_TRY(cub_run(tmp, st, [&](void* t, size_t& b) {
     return cub::DeviceRadixSort::SortPairs(t, b, keys.as<const unsigned long long>(), keys2.as<unsigned long long>(), vals.as<const uint32_t>(), vals2.as<uint32_t>(),
                                            static_cast<int>(n), 0, 64, st);
   }));
-  B2_TRY(flags.alloc(count * sizeof(uint32_t)));
-  B2_TRY(incl.alloc(count * sizeof(uint32_t)));
-  B2_TRY(starts.alloc((count + 1) * sizeof(uint32_t)));
-  const unsigned grid = static_cast<unsigned>((count + 255) / 256);
-  key_heads_kernel<<<grid, 256, 0, st>>>(keys2.as<const unsigned long long>(), count, flags.as<uint32_t>());
-  B2_CUDA(cudaGetLastError());
-  B2_TRY(cub_run(tmp, st, [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, flags.as<const uint32_t>(), incl.as<uint32_t>(), static_cast<int>(count), st); }));
-  key_starts_kernel<<<grid, 256, 0, st>>>(flags.as<const uint32_t>(), incl.as<const uint32_t>(), count, starts.as<uint32_t>());
-  B2_CUDA(cudaGetLastError());
-  B2_CUDA(cudaMemcpyAsync(m, incl.as<uint32_t>() + (count - 1), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-  B2_CUDA(cudaStreamSynchronize(st));
+  B2_TRY(key_segments(keys2.as<const unsigned long long>(), count, st, incl, starts, m));
   const size_t v = *m;
   B2_TRY(out_p.alloc(v * 3 * sizeof(double)));
   if (in.covs) B2_TRY(out_c.alloc(v * 9 * sizeof(double)));
@@ -514,6 +504,22 @@ b2_status assemble_cloud(b2_ctx* ctx, const RawCloud& raw, unsigned flags, const
   B2_CUDA(cudaStreamSynchronize(st));
 
   *out = c.release();
+  return B2_OK;
+}
+
+b2_status key_segments(const unsigned long long* sorted_keys, size_t count, cudaStream_t st, DeviceBuffer& incl, DeviceBuffer& starts, uint32_t* num_segments) {
+  DeviceBuffer flags, tmp;
+  B2_TRY(flags.alloc(count * sizeof(uint32_t)));
+  B2_TRY(incl.alloc(count * sizeof(uint32_t)));
+  B2_TRY(starts.alloc((count + 1) * sizeof(uint32_t)));
+  const unsigned grid = static_cast<unsigned>((count + 255) / 256);
+  key_heads_kernel<<<grid, 256, 0, st>>>(sorted_keys, count, flags.as<uint32_t>());
+  B2_CUDA(cudaGetLastError());
+  B2_TRY(cub_run(tmp, st, [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, flags.as<const uint32_t>(), incl.as<uint32_t>(), static_cast<int>(count), st); }));
+  key_starts_kernel<<<grid, 256, 0, st>>>(flags.as<const uint32_t>(), incl.as<const uint32_t>(), count, starts.as<uint32_t>());
+  B2_CUDA(cudaGetLastError());
+  B2_CUDA(cudaMemcpyAsync(num_segments, incl.as<uint32_t>() + (count - 1), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
   return B2_OK;
 }
 

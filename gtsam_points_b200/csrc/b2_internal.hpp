@@ -311,6 +311,9 @@ constexpr unsigned long long kNoKey = ~0ull;
 // Voxel keys of n >= 1 AoS points (stride 3 or 4) on the grid of 1 / inv_res: keys (kNoKey: cannot be keyed) and vals (the caller
 // index) of n entries each, *num_kept = the keyed points.  Synchronises the stream.
 b2_status voxel_keys(const double* pts, int pstride, size_t n, double inv_res, cudaStream_t st, DeviceBuffer& keys, DeviceBuffer& vals, unsigned int* num_kept);
+// The segments of equal keys among count >= 1 sorted keys: incl[p] = 1 + the segment of position p, starts[s] = the first position
+// of segment s (starts[num_segments] = count), *num_segments on the host.  Synchronises the stream.
+b2_status key_segments(const unsigned long long* sorted_keys, size_t count, cudaStream_t st, DeviceBuffer& incl, DeviceBuffer& starts, uint32_t* num_segments);
 
 // ---- radius search (b2_kdtree.cu), the two passes of b2_kdtree_radius_search over device queries ------------------------------
 // Pass 1 for nq >= 1 queries (device, AoS, stride 3 or 4) of a tree with n > 0 points: d_raw and h_raw (nq + 1 entries each) get the
@@ -321,6 +324,20 @@ b2_status radius_count(const b2_kdtree* t, const double* d_q, int stride, size_t
 // [1, 2^31 - 1]); d_kept: device, nq + 1 entries.  Synchronises the tree's stream.
 b2_status radius_fill(const b2_kdtree* t, const double* d_q, int stride, size_t nq, double r2, const unsigned long long* d_raw, unsigned long long raw_total,
                       const unsigned long long* d_kept, long long* d_out_index, double* d_out_sq);
+
+// ---- ordered statistics (b2_voxelmap.cu): iVoxCovarianceEstimation's eigenvalue statistics and the outlier threshold ----------
+// P records of 4 doubles (v0, v1, v2, w); a record with w == 0 is skipped.  Chunk c sums the records [c * kStatChunk, (c + 1) *
+// kStatChunk) in position order into (count, sum v0..v2, sum v0^2..v2^2), one addition after another; then one thread sums the
+// chunk sums in chunk order.  part: (stats_chunks(P) + 1) x 7 doubles, the total at part + 7 * stats_chunks(P).  P >= 1; asynchronous.
+constexpr int kStatChunk = 256;
+inline size_t stats_chunks(size_t P) { return (P + kStatChunk - 1) / kStatChunk; }
+b2_status ordered_stats(const double* stats, size_t P, double* part, cudaStream_t st);
+
+// ---- mean k-NN distances (b2_kdtree.cu): statistical outlier removal -----------------------------------------------------------
+// For every point i of a tree with n >= k >= 1 points, over its k nearest stored points (itself included) in ascending distance:
+// d_i = (((s_0 + s_1) + ...) + s_{k-1}) / k with s_j = sqrt of the squared distance of the k-NN.  Written as the ordered_stats
+// record of caller index i: (d_i, 0, 0, 1), stats n x 4.  Asynchronous on the tree's stream.
+b2_status launch_mean_knn_dists(const b2_kdtree* t, int k, double* stats);
 
 // A caller's pose (16 doubles, row-major 4x4) is usable: not NULL, every entry finite.  `who` names the entry point.
 inline b2_status check_pose(const double* T, const char* who) {

@@ -288,6 +288,29 @@ __global__ void __launch_bounds__(kKnnWarps * 32) covariance_kernel(KdTreeView v
   if (NORMALS) store_normal_of(reg, 3, qx, qy, qz, out_normals + static_cast<size_t>(leaf_index[i]) * 3);
 }
 
+// remove_outliers' mean neighbour distance (point_cloud_cpu_funcs.cpp:576-591) for the tree's own points, n >= k: the covariance
+// kernel's leaf-order queries and k-NN list, then d = (((s_0 + s_1) + ...) + s_{k-1}) / k over s_j = sqrt(sq_j) in ascending
+// distance, stored as the ordered_stats record (d, 0, 0, 1) of the point's caller index.
+__global__ void __launch_bounds__(kKnnWarps * 32) mean_knn_dist_kernel(KdTreeView view, size_t n, int k, const uint32_t* __restrict__ leaf_index,
+                                                                       double* __restrict__ stats /* n x 4, caller order */) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double* sdist;
+  int* sidx;
+  knn_scratch(k, warp, lane, sdist, sidx);
+  const size_t i = (blockIdx.x * static_cast<size_t>(kKnnWarps) + warp) * 32 + lane;
+  const bool active = i < n;
+  const double3 q = active ? leaf_point(view, i) : make_double3(0.0, 0.0, 0.0);
+  kdtree_knn_warp(view, q.x, q.y, q.z, active, k, 1.7976931348623157e308, sdist, sidx);
+  if (!active) return;
+  double sum = 0.0;
+  for (int j = 0; j < k; j++) sum = __dadd_rn(sum, __dsqrt_rn(sdist[j * 32]));
+  double* out = stats + static_cast<size_t>(leaf_index[i]) * 4;
+  out[0] = __ddiv_rn(sum, static_cast<double>(k));
+  out[1] = 0.0;
+  out[2] = 0.0;
+  out[3] = 1.0;
+}
+
 // estimate_normals(points, covs, n) (normal_estimation.cpp:18-50): one thread per point, caller order throughout
 __global__ void normals_from_covs_kernel(const double* __restrict__ pts, int pstride, const double* __restrict__ covs, int cstride, size_t n, double* __restrict__ out_normals) {
   const size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
@@ -595,6 +618,16 @@ b2_status radius_fill(const b2_kdtree* t, const double* d_q, int stride, size_t 
                                                                           d_out_sq);
   B2_CUDA(cudaGetLastError());
   B2_CUDA(cudaStreamSynchronize(st));
+  return B2_OK;
+}
+
+b2_status launch_mean_knn_dists(const b2_kdtree* t, int k, double* stats) {
+  const size_t n = t->n;
+  const size_t smem = knn_smem_bytes(k);
+  B2_CUDA(cudaFuncSetAttribute(reinterpret_cast<const void*>(mean_knn_dist_kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  mean_knn_dist_kernel<<<static_cast<unsigned>((n + kKnnWarps * 32 - 1) / (kKnnWarps * 32)), kKnnWarps * 32, smem, t->ctx->stream>>>(t->view(), n, k, t->d_leaf_index.as<const uint32_t>(),
+                                                                                                                               stats);
+  B2_CUDA(cudaGetLastError());
   return B2_OK;
 }
 

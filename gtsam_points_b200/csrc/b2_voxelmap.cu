@@ -589,7 +589,6 @@ b2_status check_insert_cloud(const b2_voxelmap& vm, const b2_cloud* frame, const
 
 constexpr unsigned long long kValidBit = 1ull << 63;                // IncrementalCovarianceContainer::VALID_BIT
 constexpr unsigned long long kBirthdayMask = (kValidBit >> 1) - 1;  // ::BIRTHDAY_MASK
-constexpr int kStatChunk = 256;                                     // positions per partial sum of the eigenvalue statistics
 
 struct CovEstParams {
   int k, min_k;                             // num_neighbors, min_num_neighbors
@@ -665,8 +664,9 @@ __global__ void cov_est_kernel(const IvoxView iv, size_t P, CovEstParams prm, un
   flags[p] = f | kValidBit;
 }
 
-// The statistics of one insert in a fixed order: partial c sums positions [c * kStatChunk, (c + 1) * kStatChunk) in position order
-// (count, sum, sum of squares), then one thread sums the partials in order.  out: count, sum[3], sum_sq[3].
+// The statistics of one insert in a fixed order (ordered_stats, which statistical outlier removal shares): partial c sums positions
+// [c * kStatChunk, (c + 1) * kStatChunk) in position order (count, sum, sum of squares), then one thread sums the partials in order.
+// out: count, sum[3], sum_sq[3].
 __global__ void eig_stats_partial_kernel(const double* __restrict__ stats, size_t P, size_t chunks, double* __restrict__ part) {
   const size_t c = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
   if (c >= chunks) return;
@@ -754,7 +754,7 @@ b2_status cov_est_pass(b2_ivox* iv) {
   b2_eig_stats fresh;
   if (P > 0) {
     const IvoxView view{vm->table(), vm->d_records.as<const double>(), vm->d_counts.as<const uint32_t>(), vm->slots, iv->neighbor_mode};
-    const size_t chunks = (P + kStatChunk - 1) / kStatChunk;
+    const size_t chunks = stats_chunks(P);
     if (iv->d_stats.bytes() < P * 4 * sizeof(double)) B2_TRY(iv->d_stats.alloc(P * 4 * sizeof(double)));
     if (iv->d_stats_part.bytes() < (chunks + 1) * 7 * sizeof(double)) B2_TRY(iv->d_stats_part.alloc((chunks + 1) * 7 * sizeof(double)));
     double* part = iv->d_stats_part.as<double>();
@@ -764,9 +764,7 @@ b2_status cov_est_pass(b2_ivox* iv) {
                                                                          iv->d_stats.as<double>());
     B2_CUDA(cudaGetLastError());
     B2_CUDA(cudaEventRecord(iv->phase_ev[2], st));
-    eig_stats_partial_kernel<<<static_cast<unsigned>((chunks + 127) / 128), 128, 0, st>>>(iv->d_stats.as<const double>(), P, chunks, part);
-    eig_stats_total_kernel<<<1, 1, 0, st>>>(part, chunks, total);
-    B2_CUDA(cudaGetLastError());
+    B2_TRY(ordered_stats(iv->d_stats.as<const double>(), P, part, st));
     double h[7];
     B2_CUDA(cudaMemcpyAsync(h, total, sizeof(h), cudaMemcpyDeviceToHost, st));
     B2_CUDA(cudaEventRecord(iv->phase_ev[3], st));
@@ -857,6 +855,15 @@ b2_status check_cov_est(const b2_ivox* iv, const char* who) {
 }
 
 }  // namespace
+
+b2_status ordered_stats(const double* stats, size_t P, double* part, cudaStream_t st) {
+  const size_t chunks = stats_chunks(P);
+  eig_stats_partial_kernel<<<static_cast<unsigned>((chunks + 127) / 128), 128, 0, st>>>(stats, P, chunks, part);
+  eig_stats_total_kernel<<<1, 1, 0, st>>>(part, chunks, part + chunks * 7);
+  B2_CUDA(cudaGetLastError());
+  return B2_OK;
+}
+
 }  // namespace b2
 
 using namespace b2;

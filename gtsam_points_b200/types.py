@@ -565,6 +565,77 @@ def voxelgrid_sampling(points, resolution: float, covs=None, normals=None, ctx: 
     return PointCloud._from_handle(h, ctx)
 
 
+def _lptr(a: np.ndarray):
+    return a.ctypes.data_as(C.POINTER(C.c_int64))
+
+
+def sample(cloud: PointCloud, indices, flags: int = capi.B2_CLOUD_DEFAULT) -> PointCloud:
+    """sample(frame, indices) (point_cloud_cpu_funcs.cpp:27-75) of a device cloud into a new device cloud: row r is the input's caller
+    index indices[r] (duplicates allowed; an index outside [0, n) raises).  The result is the cloud b2_cloud_create makes of the same
+    downloaded rows under `flags`; no point data leaves the device (b2_cloud_create_sampled)."""
+    idx = np.ascontiguousarray(indices, dtype=np.int64).ravel()
+    h = C.c_void_p()
+    capi.check(capi.lib().b2_cloud_create_sampled(cloud.h, _lptr(idx), len(idx), int(flags), C.byref(h)))
+    return PointCloud._from_handle(h, cloud.ctx)
+
+
+def _random_sampled(cloud: PointCloud, rate: float, seed: int, flags: int):
+    """(new cloud, K) of b2_cloud_create_random_sampled."""
+    out = np.zeros(max(len(cloud), 1), dtype=np.int64)
+    h = C.c_void_p()
+    capi.check(capi.lib().b2_cloud_create_random_sampled(cloud.h, float(rate), int(seed) & (2**64 - 1), int(flags), _lptr(out), C.byref(h)))
+    res = PointCloud._from_handle(h, cloud.ctx)
+    return res, out[: len(res)].copy()
+
+
+def random_sampling(cloud: PointCloud, rate: float, seed: int = 5489, flags: int = capi.B2_CLOUD_DEFAULT) -> PointCloud:
+    """random_sampling(frame, rate, mt) (point_cloud_cpu_funcs.cpp:77-93) on the device: rate >= 0.99 keeps every point, else the
+    int(n * rate) points with the smallest SplitMix64 priorities of `seed` (include/b2points.h), in caller order."""
+    return _random_sampled(cloud, rate, seed, flags)[0]
+
+
+def _randomgrid(cloud: PointCloud, resolution: float, rate: float, seed: int, flags: int):
+    """(new cloud, K) of b2_cloud_create_randomgrid."""
+    out = np.zeros(max(len(cloud), 1), dtype=np.int64)
+    h = C.c_void_p()
+    capi.check(capi.lib().b2_cloud_create_randomgrid(cloud.h, float(resolution), float(rate), int(seed) & (2**64 - 1), int(flags), _lptr(out), C.byref(h)))
+    res = PointCloud._from_handle(h, cloud.ctx)
+    return res, out[: len(res)].copy()
+
+
+def randomgrid_sampling(cloud: PointCloud, resolution: float, rate: float, seed: int = 5489, flags: int = capi.B2_CLOUD_DEFAULT) -> PointCloud:
+    """randomgrid_sampling(frame, resolution, rate, mt) (point_cloud_cpu_funcs.cpp:297-456) on the device: in every voxel of
+    `resolution` at most ceil(rate n / V) points by priority, at most int(n rate 1.2) in all, in caller order.  See
+    b2_cloud_create_randomgrid for the three deliberate differences from the reference."""
+    return _randomgrid(cloud, resolution, rate, seed, flags)[0]
+
+
+def _inliers(cloud: PointCloud, k: int, std_thresh: float, tree, flags: int):
+    """(new cloud, K, mean neighbour distances in caller order, threshold) of b2_cloud_create_inliers."""
+    n = len(cloud)
+    idx = np.zeros(max(n, 1), dtype=np.int64)
+    dists = np.zeros(max(n, 1))
+    thresh = np.zeros(1)
+    h = C.c_void_p()
+    capi.check(capi.lib().b2_cloud_create_inliers(cloud.h, None if tree is None else tree.h, int(k), float(std_thresh), int(flags), capi.dptr(dists), capi.dptr(thresh),
+                                                  _lptr(idx), C.byref(h)))
+    res = PointCloud._from_handle(h, cloud.ctx)
+    return res, idx[: len(res)].copy(), dists[:n].copy(), float(thresh[0])
+
+
+def remove_outliers(cloud: PointCloud, k: int = 10, std_thresh: float = 1.0, tree: "KdTree | None" = None, flags: int = capi.B2_CLOUD_DEFAULT) -> PointCloud:
+    """remove_outliers(frame, k, std_thresh) (point_cloud_cpu_funcs.cpp:576-650) on the device: keeps the points whose mean distance to
+    their k nearest neighbours (themselves included) is below mean + std_thresh * stddev of those distances.  tree: None builds one;
+    else a KdTree.from_cloud(cloud)."""
+    return _inliers(cloud, k, std_thresh, tree, flags)[0]
+
+
+def find_inlier_points(cloud: PointCloud, k: int = 10, std_thresh: float = 1.0, tree: "KdTree | None" = None) -> np.ndarray:
+    """find_inlier_points (point_cloud_cpu_funcs.cpp:576-613) with its k-NN on the device: the caller indices remove_outliers keeps,
+    ascending (int64)."""
+    return _inliers(cloud, k, std_thresh, tree, capi.B2_CLOUD_DEFAULT)[1]
+
+
 class KdTree:
     """NearestNeighborSearch over a point set: exact k-NN and radius search on the device."""
 

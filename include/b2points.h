@@ -397,6 +397,70 @@ B2_API b2_status b2_cloud_create_estimated(const b2_cloud* cloud, const b2_kdtre
                                            unsigned flags, b2_cloud** out);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Frame filtering of a device cloud into a NEW device cloud on the input's context (types/point_cloud_cpu.hpp; src/gtsam_points/
+ * types/point_cloud_cpu_funcs.cpp): sample, random_sampling, randomgrid_sampling and remove_outliers / find_inlier_points.
+ * Rules common to the four entry points:
+ *   output:   each call selects a list K of input caller indices.  The new cloud is exactly the cloud that
+ *             b2_cloud_create_with_normals(rows, 3, covs, 9, normals, 3, |K|, flags) makes of b2_cloud_download's rows at K: the same
+ *             stored values, storage types, Morton order and info.  New caller index r is K[r].  Covariances and normals come along
+ *             iff the input has them.  Every flag applies as for b2_cloud_create, B2_CLOUD_NO_REORDER included.  The rows are
+ *             gathered and assembled on the device; no point data goes to the host.
+ *   K:        depends only on caller indices and stored values, so a cloud made with and without B2_CLOUD_NO_REORDER gives the same K
+ *             and the same bits.  out_indices (where taken) may be NULL; else it is a host array with room for n entries (n = the
+ *             input's size) and receives K -- clouds carry no times or intensities, so this is how a caller samples side arrays.
+ *   edges:    an empty input gives an empty cloud.  Every argument check runs before any device work.
+ * The random stream of the two random samplers: each point has two 64-bit priorities, s = 0 and 1, with i its caller index and
+ * arithmetic mod 2^64 (SplitMix64):
+ *     z = seed + (2 i + s + 1) * 0x9E3779B97F4A7C15;  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;  z = (z ^ (z >> 27)) * 0x94D049BB133111EB;
+ *     h_s(i) = z ^ (z >> 31)
+ * (seed 0: h_0(0) = 0xe220a8397b1dcdaf, h_1(0) = 0x6e789e6aa1b965f4; seed 5489: h_0(7) = 0xf22dd99f91e8d40a, h_1(7) = 0x6f93c0157c1b6d3c).
+ * No two priorities are equal (the multiplier is odd and each step a bijection).  "The m smallest by h_s" is the first m points in
+ * ascending (h_s(i), i): a uniformly random subset of m without replacement.
+ * ---------------------------------------------------------------------------------------------------------- */
+/* sample(frame, indices) (point_cloud_cpu_funcs.cpp:27-75): K = indices in the given order, duplicates allowed.  An index outside
+ * [0, n) is B2_ERR_INVALID_ARGUMENT; num_indices == 0 gives an empty cloud. */
+B2_API b2_status b2_cloud_create_sampled(const b2_cloud* cloud, const int64_t* indices, size_t num_indices, unsigned flags, b2_cloud** out);
+/* random_sampling(frame, sampling_rate, mt) (point_cloud_cpu_funcs.cpp:77-93).  sampling_rate: finite and >= 0.  rate >= 0.99 gives every
+ * point (the reference returns a clone); else m = (size_t)((double)n * rate) and K = the m smallest by h_0, in ascending caller index
+ * (the reference sorts its sample the same way).  Deliberate difference: the draws are the stream above, not std::mt19937 /
+ * std::shuffle; the distribution is the same. */
+B2_API b2_status b2_cloud_create_random_sampled(const b2_cloud* cloud, double sampling_rate, uint64_t seed, unsigned flags, int64_t* out_indices,
+                                                b2_cloud** out);
+/* randomgrid_sampling(frame, voxel_resolution, sampling_rate, mt) (point_cloud_cpu_funcs.cpp:297-456).  resolution: positive and finite;
+ * sampling_rate: finite and >= 0; rate >= 0.99 gives every point.  Otherwise:
+ *   keys:  those of b2_cloud_create_voxelgrid (c = fast_floor(x * (1 / resolution)) + 2^20, 21 bits per axis); a point out of range
+ *          is never kept.  V = the number of occupied voxels; V == 0 gives an empty cloud.
+ *   ppv = (size_t)ceil((rate * (double)n) / (double)V), with n counting every input point (the reference's frame->size()); in each
+ *          voxel the min(count, ppv) smallest by h_0 are kept.
+ *   cap = (size_t)(((double)n * rate) * 1.2); if more than cap points are kept, the cap smallest of them by h_1 stay -- a second
+ *          stream, since capping by h_0 would favour dense voxels, whose minima are smaller.
+ *   K in ascending caller index.
+ * Deliberate differences from the reference: (a) the draws are the stream above, not std::mt19937 / std::sample: the distribution is
+ * the same, and the result does not depend on threads (the reference seeds one engine per thread and places blocks with an atomic
+ * fetch_add, so its multi-threaded output depends on the schedule); (b) a voxel is sampled whole -- the reference cuts the sorted
+ * run into blocks of 1024, so a voxel whose run crosses a block boundary is sampled as two groups (voxel-grid difference (b));
+ * (c) V is the number of occupied voxels -- the reference counts key transitions, V - 1 when no point is dropped, and divides by
+ * zero when every point shares one voxel. */
+B2_API b2_status b2_cloud_create_randomgrid(const b2_cloud* cloud, double resolution, double sampling_rate, uint64_t seed, unsigned flags,
+                                            int64_t* out_indices, b2_cloud** out);
+/* remove_outliers(frame, k, std_thresh) (point_cloud_cpu_funcs.cpp:576-650); out_indices is find_inlier_points.  1 <= k <= B2_KNN_MAX_K,
+ * std_thresh finite.  tree: NULL builds a temporary one, else it must come from b2_kdtree_create_from_cloud(cloud)
+ * (B2_ERR_INVALID_ARGUMENT).  0 < n < k is B2_ERR_INVALID_ARGUMENT (the reference reads neighbors[-1] there).
+ *   d_i = (((s_0 + s_1) + ...) + s_{k-1}) / k with s_j = sqrt(sq_j) over point i's k nearest stored points (itself included) in
+ *         ascending distance, sq the k-NN's ((dx dx + dy dy) + dz dz).  The sequence of distances is unique, so ties in index do not
+ *         change d_i: any exact k-NN gives the same bits.
+ *   S = sum of d_i, Q = sum of d_i d_i, each in iVoxCovarianceEstimation's order: chunks of 256 caller indices, each summed in index
+ *         order, then the chunk sums in chunk order.
+ *   mean = S / n, var = Q / n - mean mean, thresh = mean + sqrt(var) std_thresh; K = the points with d_i < thresh, ascending.
+ * Every operation is rounded on its own, in the order written (no FMA).  As in the reference: a negative rounded var gives a NaN
+ * threshold and no inliers, and a cloud whose d_i are all equal (a lattice) keeps no point, since the test is strict.
+ * out_mean_dists (n entries, caller order) and out_thresh may each be NULL; an empty cloud gives thresh NaN (0 / 0).
+ * Deliberate differences: (a) the reference sums S and Q sequentially, so a point within rounding of the threshold can land on the
+ * other side; (b) its norm of a Vector4d difference is an Eigen reduction whose order depends on the SIMD width. */
+B2_API b2_status b2_cloud_create_inliers(const b2_cloud* cloud, const b2_kdtree* tree, int k, double std_thresh, unsigned flags, double* out_mean_dists,
+                                         double* out_thresh, int64_t* out_indices, b2_cloud** out);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Global registration: FPFH features, exact feature-space nearest neighbours, RANSAC and GNC pose estimation
  * (include/gtsam_points/features/fpfh_estimation.hpp, src/gtsam_points/features/fpfh_estimation.cpp:196-327,
  *  include/gtsam_points/registration/ransac.hpp, registration/impl/ransac_impl.hpp, src/gtsam_points/registration/alignment.cpp,

@@ -46,6 +46,19 @@ B2_FPFH_DIM = 33
 B2_PFH_DIM = 125
 
 
+class MinCutParamsC(C.Structure):
+    _fields_ = [("distance_sigma", C.c_double), ("angle_sigma", C.c_double), ("foreground_mask_radius", C.c_double), ("background_mask_radius", C.c_double),
+                ("foreground_weight", C.c_double), ("background_weight", C.c_double), ("k_neighbors", C.c_int32), ("reserved", C.c_int32)]
+
+
+class MinCutResultC(C.Structure):
+    _fields_ = [("source_index", C.c_int64), ("sink_index", C.c_int64), ("max_flow", C.c_double), ("max_flow_q", C.c_int64), ("cluster_size", C.c_uint64),
+                ("flags", C.c_int32), ("reserved", C.c_int32)]
+
+
+B2_MIN_CUT_NO_SEED, B2_MIN_CUT_FEW_NEIGHBORS, B2_MIN_CUT_NO_SINK = 1, 2, 4
+
+
 class FeaturesInfo(C.Structure):
     _fields_ = [("num_features", C.c_uint64), ("dim", C.c_int32), ("reserved", C.c_int32), ("device_bytes", C.c_uint64)]
 
@@ -153,6 +166,11 @@ SIGNATURES = {
     "b2_features_nearest": (C.c_int, [_vp, _vp, _lp, _dp]),
     "b2_estimate_pose_ransac": (C.c_int, [_vp, _vp, _vp, _vp, C.POINTER(RansacParams), C.POINTER(RegistrationResultC), _ip]),
     "b2_estimate_pose_gnc": (C.c_int, [_vp, _vp, _vp, _vp, C.POINTER(GncParams), C.POINTER(RegistrationResultC), _lp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "b2_region_growing_create": (C.c_int, [_vp, _vp, _dp, C.c_double, C.c_double, C.c_double, C.c_int, _pp]),
+    "b2_region_growing_update": (C.c_int, [_vp, C.c_int, _ip]),
+    "b2_region_growing_get": (C.c_int, [_vp, C.POINTER(C.c_uint64), _lp]),
+    "b2_region_growing_destroy": (C.c_int, [_vp]),
+    "b2_min_cut": (C.c_int, [_vp, _vp, C.c_int64, _dp, C.POINTER(MinCutParamsC), C.POINTER(MinCutResultC), _lp, _lp]),
     "b2_vgicp_factor_create": (C.c_int, [_vp, _vp, _vp, _pp]),
     "b2_gicp_factor_create": (C.c_int, [_vp, _vp, _vp, _vp, _pp]),
     "b2_icp_factor_create": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int, _dp, _pp]),

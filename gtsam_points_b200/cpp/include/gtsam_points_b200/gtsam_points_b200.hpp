@@ -451,6 +451,100 @@ inline std::vector<int> find_inlier_points_gpu(const PointCloudGPU::ConstPtr& fr
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
+// Region growing (segmentation/region_growing.hpp) on a device cloud with normals.  The whole visit order is computed on the device
+// by region_growing_init_gpu; region_growing_update_gpu reveals it as the reference's steps would, flag and dilation included (see
+// b2_region_growing_create).  Only max_steps may change between init and update: other changed parameters throw
+// std::invalid_argument, since the stored order depends on them.
+// ---------------------------------------------------------------------------------------------------------------------
+struct RegionGrowingParams {
+  double distance_threshold = 0.5;
+  double angle_threshold = 10.0 * 3.14159265358979323846 / 180.0;  // 10 degrees, M_PI
+  double dilation_radius = 0.5;
+  int max_cluster_size = 1000000;
+  int max_steps = 1000000;
+  int num_threads = 1;  // accepted for the reference's signature; the device pass has no thread count
+};
+
+struct RegionGrowingContextGPU {
+  std::vector<std::size_t> cluster_indices;
+  std::shared_ptr<b2_region_growing> handle;
+  RegionGrowingParams params;  // as given to init
+};
+
+inline RegionGrowingContextGPU region_growing_init_gpu(const PointCloudGPU::ConstPtr& points, const KdTreeGPU* search, const std::array<double, 3>& seed_point,
+                                                       const RegionGrowingParams& params = RegionGrowingParams()) {
+  b2_region_growing* rg = nullptr;
+  check(b2_region_growing_create(points->handle(), search ? search->handle() : nullptr, seed_point.data(), params.distance_threshold, params.angle_threshold,
+                                 params.dilation_radius, params.max_cluster_size, &rg),
+        "b2_region_growing_create");
+  RegionGrowingContextGPU ctx;
+  ctx.handle.reset(rg, [](b2_region_growing* h) { b2_region_growing_destroy(h); });
+  ctx.params = params;
+  return ctx;
+}
+
+// region_growing_update: returns true when converged; context.cluster_indices is refreshed
+inline bool region_growing_update_gpu(RegionGrowingContextGPU& context, const RegionGrowingParams& params) {
+  const RegionGrowingParams& p0 = context.params;
+  if (params.distance_threshold != p0.distance_threshold || params.angle_threshold != p0.angle_threshold || params.dilation_radius != p0.dilation_radius ||
+      params.max_cluster_size != p0.max_cluster_size)
+    throw std::invalid_argument("region_growing_update_gpu: only max_steps may change after region_growing_init_gpu");
+  int converged = 0;
+  check(b2_region_growing_update(context.handle.get(), params.max_steps, &converged), "b2_region_growing_update");
+  std::uint64_t size = 0;
+  check(b2_region_growing_get(context.handle.get(), &size, nullptr), "b2_region_growing_get");
+  std::vector<std::int64_t> idx(size);
+  check(b2_region_growing_get(context.handle.get(), &size, idx.data()), "b2_region_growing_get");
+  context.cluster_indices.assign(idx.begin(), idx.end());
+  return converged != 0;
+}
+
+// region_growing_update with the parameters given to init
+inline bool region_growing_update_gpu(RegionGrowingContextGPU& context) { return region_growing_update_gpu(context, context.params); }
+
+// min_cut (segmentation/min_cut.hpp) on a device cloud with normals: the minimal minimum-cut source set (see b2_min_cut for the
+// network, the integer capacities and the differences from the reference)
+struct MinCutParams {
+  double distance_sigma = 0.25;
+  double angle_sigma = 10.0 * 3.14159265358979323846 / 180.0;
+  double foreground_mask_radius = 0.2;
+  double background_mask_radius = 3.0;
+  double foreground_weight = 0.2;
+  double background_weight = 0.2;
+  int k_neighbors = 20;
+  int num_threads = 1;  // accepted for the reference's signature
+};
+
+struct MinCutResult {
+  std::size_t source_index = static_cast<std::size_t>(-1);
+  std::size_t sink_index = static_cast<std::size_t>(-1);
+  double max_flow = 0.0;
+  int flags = 0;  // B2_MIN_CUT_NO_SEED / _FEW_NEIGHBORS / _NO_SINK: the reference's warnings
+  std::vector<std::size_t> cluster_indices;
+};
+
+inline MinCutResult min_cut_gpu_(const PointCloudGPU::ConstPtr& points, const KdTreeGPU* search, std::int64_t source, const double* seed, const MinCutParams& params) {
+  const b2_min_cut_params p{params.distance_sigma, params.angle_sigma, params.foreground_mask_radius, params.background_mask_radius, params.foreground_weight,
+                            params.background_weight, params.k_neighbors, 0};
+  b2_min_cut_result info{};
+  std::vector<std::int64_t> idx(std::max<std::size_t>(points->size(), 1));
+  check(b2_min_cut(points->handle(), search ? search->handle() : nullptr, source, seed, &p, &info, idx.data(), nullptr), "b2_min_cut");
+  MinCutResult r;
+  r.source_index = static_cast<std::size_t>(info.source_index);
+  r.sink_index = static_cast<std::size_t>(info.sink_index);
+  r.max_flow = info.max_flow;
+  r.flags = info.flags;
+  r.cluster_indices.assign(idx.begin(), idx.begin() + info.cluster_size);
+  return r;
+}
+inline MinCutResult min_cut_gpu(const PointCloudGPU::ConstPtr& points, const KdTreeGPU* search, std::size_t source_pt_index, const MinCutParams& params = MinCutParams()) {
+  return min_cut_gpu_(points, search, static_cast<std::int64_t>(source_pt_index), nullptr, params);
+}
+inline MinCutResult min_cut_gpu(const PointCloudGPU::ConstPtr& points, const KdTreeGPU* search, const std::array<double, 3>& source_pt, const MinCutParams& params = MinCutParams()) {
+  return min_cut_gpu_(points, search, -1, source_pt.data(), params);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
 // Global registration (features/fpfh_estimation.hpp, registration/ransac.hpp, registration/graduated_non_convexity.hpp): features,
 // FPFH, RANSAC and GNC on the device
 // ---------------------------------------------------------------------------------------------------------------------

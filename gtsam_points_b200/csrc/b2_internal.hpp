@@ -325,6 +325,18 @@ b2_status radius_count(const b2_kdtree* t, const double* d_q, int stride, size_t
 b2_status radius_fill(const b2_kdtree* t, const double* d_q, int stride, size_t nq, double r2, const unsigned long long* d_raw, unsigned long long raw_total,
                       const unsigned long long* d_kept, long long* d_out_index, double* d_out_sq);
 
+// ---- radius neighbourhoods (b2_registration.cu): FPFH, PFH and region growing -------------------------------------------------
+// Radius neighbourhoods of nq >= 1 queries in CSR form: row q is b2_kdtree_radius_search's list of d_q[q] (device, nq x 3) --
+// (distance, caller index) order -- truncated to its first max_nn entries.  off: nq + 1 offsets, on the host and on the device.
+struct Neighbourhoods {
+  std::vector<unsigned long long> off;
+  DeviceBuffer d_off, d_nbr, d_sq;
+};
+// Fills nb for a tree with n > 0 points; r2 = radius^2.  Synchronises the stream.
+b2_status radius_neighbourhoods(const b2_kdtree* tree, const double* d_q, size_t nq, double r2, size_t max_nn, cudaStream_t st, Neighbourhoods& nb);
+// flags[idx[k]] = 1 for k < m (mark_kernel); asynchronous
+b2_status launch_mark(size_t m, const long long* idx, unsigned char* flags, cudaStream_t st);
+
 // ---- ordered statistics (b2_voxelmap.cu): iVoxCovarianceEstimation's eigenvalue statistics and the outlier threshold ----------
 // P records of 4 doubles (v0, v1, v2, w); a record with w == 0 is skipped.  Chunk c sums the records [c * kStatChunk, (c + 1) *
 // kStatChunk) in position order into (count, sum v0..v2, sum v0^2..v2^2), one addition after another; then one thread sums the
@@ -338,6 +350,9 @@ b2_status ordered_stats(const double* stats, size_t P, double* part, cudaStream_
 // d_i = (((s_0 + s_1) + ...) + s_{k-1}) / k with s_j = sqrt of the squared distance of the k-NN.  Written as the ordered_stats
 // record of caller index i: (d_i, 0, 0, 1), stats n x 4.  Asynchronous on the tree's stream.
 b2_status launch_mean_knn_dists(const b2_kdtree* t, int k, double* stats);
+// b2_kdtree_knn's k nearest neighbours (1 <= k <= B2_KNN_MAX_K) of nq device queries (AoS, stride 3 or 4) into device arrays
+// d_idx / d_sq (nq x k, caller indices, -1 / max_sq beyond the number found).  Asynchronous on the tree's stream.
+b2_status launch_knn(const b2_kdtree* t, const double* d_q, int stride, size_t nq, int k, double max_sq, long long* d_idx, double* d_sq);
 
 // A caller's pose (16 doubles, row-major 4x4) is usable: not NULL, every entry finite.  `who` names the entry point.
 inline b2_status check_pose(const double* T, const char* who) {

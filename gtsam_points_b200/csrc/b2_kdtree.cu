@@ -621,6 +621,16 @@ b2_status radius_fill(const b2_kdtree* t, const double* d_q, int stride, size_t 
   return B2_OK;
 }
 
+b2_status launch_knn(const b2_kdtree* t, const double* d_q, int stride, size_t nq, int k, double max_sq, long long* d_idx, double* d_sq) {
+  if (nq == 0) return B2_OK;
+  const size_t smem = knn_smem_bytes(k);
+  B2_CUDA(cudaFuncSetAttribute(reinterpret_cast<const void*>(knn_kernel), cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  knn_kernel<<<static_cast<unsigned>((nq + kKnnWarps * 32 - 1) / (kKnnWarps * 32)), kKnnWarps * 32, smem, t->ctx->stream>>>(t->view(), d_q, stride, nq, k, max_sq,
+                                                                                                                        t->d_leaf_index.as<const uint32_t>(), d_idx, d_sq);
+  B2_CUDA(cudaGetLastError());
+  return B2_OK;
+}
+
 b2_status launch_mean_knn_dists(const b2_kdtree* t, int k, double* stats) {
   const size_t n = t->n;
   const size_t smem = knn_smem_bytes(k);

@@ -744,12 +744,7 @@ b2_status check_features(const b2_features* f, const char* who) {
   return B2_OK;
 }
 
-// Radius neighbourhoods of nq >= 1 queries in CSR form: row q is b2_kdtree_radius_search's list of d_q[q] (device, nq x 3) --
-// (distance, caller index) order -- truncated to its first max_nn entries.  off: nq + 1 offsets, on the host and on the device.
-struct Neighbourhoods {
-  std::vector<unsigned long long> off;
-  DeviceBuffer d_off, d_nbr, d_sq;
-};
+}  // namespace
 
 b2_status radius_neighbourhoods(const b2_kdtree* tree, const double* d_q, size_t nq, double r2, size_t max_nn, cudaStream_t st, Neighbourhoods& nb) {
   std::vector<unsigned long long> raw;
@@ -782,6 +777,14 @@ b2_status radius_neighbourhoods(const b2_kdtree* tree, const double* d_q, size_t
   }
   return B2_OK;
 }
+
+b2_status launch_mark(size_t m, const long long* idx, unsigned char* flags, cudaStream_t st) {
+  if (m > 0) mark_kernel<<<grid_for(m, 256), 256, 0, st>>>(m, idx, flags);
+  B2_CUDA(cudaGetLastError());
+  return B2_OK;
+}
+
+namespace {
 
 // PFH rows of the neighbourhoods nb (nq rows) into out (nq x 125): the pair numbering and CTA chunks of pfh_kernel, built on the
 // host from the neighbour counts, then the counts and their conversion in place.

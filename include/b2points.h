@@ -461,6 +461,100 @@ B2_API b2_status b2_cloud_create_inliers(const b2_cloud* cloud, const b2_kdtree*
                                          double* out_thresh, int64_t* out_indices, b2_cloud** out);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Segmentation: region growing on a device cloud with normals (include/gtsam_points/segmentation/region_growing.hpp,
+ * segmentation/impl/region_growing_impl.hpp).  region_growing_init is b2_region_growing_create, region_growing_update is
+ * b2_region_growing_update, and RegionGrowingContext::cluster_indices is b2_region_growing_get.
+ * The reference's semantics, with p, n the stored points and normals (b2_cloud_download's) and M = max_cluster_size:
+ *   seed:      the nearest point to seed_point (b2_kdtree_knn1 with max_sq_dist = DBL_MAX; among equidistant points which one is not
+ *              specified).  None (an empty cloud) gives an empty, converged context.
+ *   queue:     FIFO, starting with the seed.  A step pops until it meets a point i not yet visited (stale entries cost no step),
+ *              visits i -- appends it to the cluster -- and pushes, in list order, every j of b2_kdtree_radius_search's list of p_i
+ *              (squared distance < distance_threshold^2, sorted by (distance, index), the first M) that is not yet visited and
+ *              has NOT (n_i . n_j < cos(angle_threshold)), with the dot ((n_i0 n_j0 + n_i1 n_j1) + n_i2 n_j2) and the cosine
+ *              computed by the host's std::cos.  A step that starts with an empty queue does nothing; one that starts with more
+ *              than M points in the cluster clears the queue (so a cluster can reach M + 1 points).
+ *   update:    if the queue is empty, returns converged at once.  Otherwise at most max_steps steps (none for max_steps <= 0),
+ *              stopping when the queue runs empty; if it is then empty and dilation_radius > 0 the cluster is replaced by the
+ *              ascending union of the radius lists (dilation_radius, no count limit) of its points.  converged = the queue is
+ *              empty.  As in the reference, the last visit can leave stale entries in the queue: converged is then 0 and the
+ *              dilation waits for the next update, whose first step drains them.
+ * How it is computed: the visit order O is the BFS order of the graph i -> j (j accepted in i's list), each level sorted by
+ * (rank of the discovering point, position in its list); create computes O on the device, level-synchronously, with the number of
+ * pushes of every visit (the accepted j ranked after i), which fixes the step that empties the queue.  create also computes the
+ * dilation set; update only advances a cursor over O, and get reads the cluster back.  The result is bit-reproducible and does not
+ * depend on the cloud's storage order.
+ * Deliberate differences from the reference:
+ *   (a) the dot product is rounded in the order above; the reference's Vector4d dot is an Eigen reduction whose order depends on
+ *       the SIMD width, so a pair within rounding of the angle threshold can be decided the other way;
+ *   (b) a cloud without normals is B2_ERR_INVALID_ARGUMENT (the reference prints a warning and reports convergence);
+ *   (c) the parameters are fixed at create: the reference takes them again on every update call.
+ *   (d) the truncated radius list is the first M by (distance, index): the reference's kd-tree promises no order for which points
+ *       enter when max_num_neighbors cuts the list, and this choice fixes the visit order and the cap's behaviour.
+ * Memory: the radius lists of up to 65536 points are held at once, so a radius that covers thousands of points of a dense cloud
+ * needs that many 16-byte entries per point on the device.
+ * ---------------------------------------------------------------------------------------------------------- */
+typedef struct b2_region_growing b2_region_growing; /* the visit order, dilation set and step cursor of one region growing */
+/* tree: NULL builds a temporary one, else it must come from b2_kdtree_create_from_cloud(cloud).  seed_point: host, 3 finite doubles.
+ * distance_threshold finite and >= 0; angle_threshold and dilation_radius finite; max_cluster_size >= 0 (the reference's defaults:
+ * 0.5, 10 degrees, 0.5 and 1000000).  Every argument is checked before any device work.  The context does not need the cloud or
+ * the tree afterwards. */
+B2_API b2_status b2_region_growing_create(const b2_cloud* cloud, const b2_kdtree* tree, const double seed_point[3], double distance_threshold,
+                                          double angle_threshold, double dilation_radius, int max_cluster_size, b2_region_growing** out);
+/* region_growing_update with params.max_steps = max_steps; converged (may be NULL) receives its return value as 0 / 1 */
+B2_API b2_status b2_region_growing_update(b2_region_growing* rg, int max_steps, int* converged);
+/* cluster_indices: *size = its length; indices (host, may be NULL) receives them: the visited points in visit order, or after
+ * the dilation the dilation set in ascending order */
+B2_API b2_status b2_region_growing_get(const b2_region_growing* rg, uint64_t* size, int64_t* indices);
+B2_API b2_status b2_region_growing_destroy(b2_region_growing* rg);
+
+/* min_cut(points, search, source_pt_index | source_pt, params) (segmentation/min_cut.hpp, impl/min_cut_impl.hpp) on a device cloud
+ * with normals.  The network, with p, n the stored points and normals and s the source point:
+ *   k-NN arcs: for every point i and each of its k nearest points j (itself included; fewer where the cloud has fewer), an arc i -> j
+ *       of weight w = exp(-d2 * (1 / sd^2)) * exp(-a * a * (1 / sa^2)), d2 the k-NN squared distance, a = acos(|n_i . n_j|) with
+ *       the dot ((..) + ..) + ..;  background: t = the first point (by index) with |p_i - p_s| > background_mask_radius, and every
+ *       other such point an arc to t of background_weight;  foreground arcs (into s) carry no flow and are left out.  No point
+ *       farther than the background radius gives the reference's default result: source = sink = -1, flow 0, no cluster, and
+ *       flags B2_MIN_CUT_NO_SINK.
+ *   capacities: q = llround(w * 2^32) in int64; info->max_flow_q = the maximum flow in these units, max_flow = max_flow_q / 2^32.
+ *   result: the points reachable from s in the residual network of a maximum flow -- the minimal minimum-cut source set, which is
+ *       unique, in ascending order.  The reference reports Boykov-Kolmogorov's source-coloured vertices, which are this set: its
+ *       source tree is closed under residual arcs when the algorithm ends (reasoned from the algorithm, not measured).
+ * How: one device k-NN pass, the capacities in a kernel, the arcs sorted and merged into a CSR network on the device (parallel arcs
+ * i -> j and j -> i become one arc pair; merging changes neither the flow value nor the set), then phase one of a lock-free
+ * push-relabel with 64-bit integer atomics and global relabels by device BFS, run on the REVERSED network from t to s: the nodes
+ * that can still reach s are then the minimal source set of the original network.  Every capacity is clamped to one more than the
+ * source's out-capacity, which changes no minimum cut.
+ * Arguments: source_index >= 0 picks the source; source_index < 0 takes the nearest point to seed_point (3 finite doubles;
+ * B2_MIN_CUT_NO_SEED in flags if there is none).  sigmas positive and finite; weights finite and in [0, 2^30]; radii >= 0;
+ * 1 <= k_neighbors <= B2_KNN_MAX_K; n < 2^24.  tree: NULL or from b2_kdtree_create_from_cloud(cloud).  out_indices: NULL or room
+ * for n entries.  out_capacities: NULL or n * k entries, the quantised k-NN capacities q in row order (-1: no neighbour).
+ * Deliberate differences from the reference: (a) integer capacities: a cut within one quantum of another can come out differently;
+ * (b) a NaN weight (|n_i . n_j| rounded above 1) gives capacity 0 -- as far as can be told without Boost, Boykov-Kolmogorov never
+ * uses an arc whose residual does not compare > 0, so such an arc carries nothing there either (an inference, not a measurement);
+ * (c) each k-NN row is b2_kdtree_knn's, reordered by (squared distance, index); which of several points tied at the k-th distance
+ * enters the row is the tree's choice (the reference makes no promise there either); (d) the distance to s is
+ * sqrt((dx dx + dy dy) + dz dz), where the reference's Vector4d norm is an Eigen reduction; (e) a cloud without normals is
+ * B2_ERR_INVALID_ARGUMENT, and the seed form's and short rows' warnings are flags, not messages on stderr. */
+#define B2_MIN_CUT_NO_SEED 1
+#define B2_MIN_CUT_FEW_NEIGHBORS 2
+#define B2_MIN_CUT_NO_SINK 4
+typedef struct b2_min_cut_params {
+  double distance_sigma, angle_sigma, foreground_mask_radius, background_mask_radius, foreground_weight, background_weight;
+  int32_t k_neighbors;
+  int32_t reserved;
+} b2_min_cut_params;
+typedef struct b2_min_cut_result {
+  int64_t source_index, sink_index;
+  double max_flow;
+  int64_t max_flow_q;
+  uint64_t cluster_size;
+  int32_t flags;
+  int32_t reserved;
+} b2_min_cut_result;
+B2_API b2_status b2_min_cut(const b2_cloud* cloud, const b2_kdtree* tree, int64_t source_index, const double* seed_point, const b2_min_cut_params* params,
+                            b2_min_cut_result* info, int64_t* out_indices, int64_t* out_capacities);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Global registration: FPFH features, exact feature-space nearest neighbours, RANSAC and GNC pose estimation
  * (include/gtsam_points/features/fpfh_estimation.hpp, src/gtsam_points/features/fpfh_estimation.cpp:196-327,
  *  include/gtsam_points/registration/ransac.hpp, registration/impl/ransac_impl.hpp, src/gtsam_points/registration/alignment.cpp,

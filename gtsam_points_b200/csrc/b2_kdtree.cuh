@@ -163,47 +163,61 @@ __device__ __forceinline__ double jsqrt(double a) {
   else return sqrt(a);
 }
 
-// cyclic Jacobi eigen-decomposition of a symmetric 3x3 (ascending eigenvalues, eigenvectors in the columns of V): the same
-// rotation sequence as the CPU oracle's restatement, robust for the rank-deficient covariances of planar neighbourhoods
-// (covariance estimation, normals) and of the 3-point alignment's cross-covariance (RANSAC).  Rounded: see jmul.
-template <bool Rounded = false>
-__device__ __forceinline__ void jacobi_eigen3(double A[3][3], double w[3], double V[3][3]) {
+// cyclic Jacobi sweeps over a symmetric N x N until the off-diagonal sum of squares is at most 1e-32 times the diagonal's (at most
+// 64 sweeps): A ends (nearly) diagonal, with the eigenvalues on its diagonal and the eigenvectors in the columns of V, unsorted.
+// Pairs (p, q) in row order; the off-diagonal and diagonal sums run over the upper triangle in row order.  Rounded: see jmul.
+template <int N, bool Rounded>
+__device__ __forceinline__ void jacobi_sweeps(double A[N][N], double V[N][N]) {
 #pragma unroll
-  for (int i = 0; i < 3; i++)
+  for (int i = 0; i < N; i++)
 #pragma unroll
-    for (int j = 0; j < 3; j++) V[i][j] = i == j ? 1.0 : 0.0;
+    for (int j = 0; j < N; j++) V[i][j] = i == j ? 1.0 : 0.0;
   for (int sweep = 0; sweep < 64; sweep++) {
-    const double off = jadd<Rounded>(jadd<Rounded>(jmul<Rounded>(A[0][1], A[0][1]), jmul<Rounded>(A[0][2], A[0][2])), jmul<Rounded>(A[1][2], A[1][2]));
-    const double diag = jadd<Rounded>(jadd<Rounded>(jmul<Rounded>(A[0][0], A[0][0]), jmul<Rounded>(A[1][1], A[1][1])), jmul<Rounded>(A[2][2], A[2][2]));
+    double off = jmul<Rounded>(A[0][1], A[0][1]), diag = jmul<Rounded>(A[0][0], A[0][0]);
+#pragma unroll
+    for (int p = 0; p < N - 1; p++)
+#pragma unroll
+      for (int q = p + 1; q < N; q++)
+        if (p + q > 1) off = jadd<Rounded>(off, jmul<Rounded>(A[p][q], A[p][q]));
+#pragma unroll
+    for (int p = 1; p < N; p++) diag = jadd<Rounded>(diag, jmul<Rounded>(A[p][p], A[p][p]));
     if (off <= jmul<Rounded>(1e-32, diag) || off == 0.0) break;
 #pragma unroll
-    for (int p = 0; p < 2; p++)
+    for (int p = 0; p < N - 1; p++)
 #pragma unroll
-      for (int q = p + 1; q < 3; q++) {
+      for (int q = p + 1; q < N; q++) {
         if (A[p][q] == 0.0) continue;
         const double theta = jdiv<Rounded>(jsub<Rounded>(A[q][q], A[p][p]), jmul<Rounded>(2.0, A[p][q]));
         const double t = jdiv<Rounded>(theta >= 0.0 ? 1.0 : -1.0, jadd<Rounded>(fabs(theta), jsqrt<Rounded>(jadd<Rounded>(jmul<Rounded>(theta, theta), 1.0))));
         const double c = jdiv<Rounded>(1.0, jsqrt<Rounded>(jadd<Rounded>(jmul<Rounded>(t, t), 1.0))), sn = jmul<Rounded>(t, c);
 #pragma unroll
-        for (int k = 0; k < 3; k++) {
+        for (int k = 0; k < N; k++) {
           const double akp = A[k][p], akq = A[k][q];
           A[k][p] = jsub<Rounded>(jmul<Rounded>(c, akp), jmul<Rounded>(sn, akq));
           A[k][q] = jadd<Rounded>(jmul<Rounded>(sn, akp), jmul<Rounded>(c, akq));
         }
 #pragma unroll
-        for (int k = 0; k < 3; k++) {
+        for (int k = 0; k < N; k++) {
           const double apk = A[p][k], aqk = A[q][k];
           A[p][k] = jsub<Rounded>(jmul<Rounded>(c, apk), jmul<Rounded>(sn, aqk));
           A[q][k] = jadd<Rounded>(jmul<Rounded>(sn, apk), jmul<Rounded>(c, aqk));
         }
 #pragma unroll
-        for (int k = 0; k < 3; k++) {
+        for (int k = 0; k < N; k++) {
           const double vkp = V[k][p], vkq = V[k][q];
           V[k][p] = jsub<Rounded>(jmul<Rounded>(c, vkp), jmul<Rounded>(sn, vkq));
           V[k][q] = jadd<Rounded>(jmul<Rounded>(sn, vkp), jmul<Rounded>(c, vkq));
         }
       }
   }
+}
+
+// Jacobi eigen-decomposition of a symmetric 3x3 (ascending eigenvalues, eigenvectors in the columns of V): the same rotation
+// sequence as the CPU oracle's restatement, robust for the rank-deficient covariances of planar neighbourhoods (covariance
+// estimation, normals).  Rounded: see jmul.
+template <bool Rounded = false>
+__device__ __forceinline__ void jacobi_eigen3(double A[3][3], double w[3], double V[3][3]) {
+  jacobi_sweeps<3, Rounded>(A, V);
   // ascending order (3-element sorting network on (w, column))
   w[0] = A[0][0], w[1] = A[1][1], w[2] = A[2][2];
   auto swap_cols = [&](int a, int b) {

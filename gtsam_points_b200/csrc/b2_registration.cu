@@ -369,40 +369,52 @@ struct HypothesisParams {
   int num_taboo;
 };
 
-// The rotation maximising sum t_i . R s_i over centred point sets, from H = sum (t_i - mt)(s_i - ms)^T, det R = +1: the top two
-// eigenvectors v1, v2 of H^T H, u_k = H v_k normalised (u2 made orthogonal to u1), R = u1 v1^T + u2 v2^T + (u1 x u2)(v1 x v2)^T.
-// That is U diag(1, 1, det U det V) V^T of the SVD of H, the reference's reflection fix (alignment.cpp:10-37); it needs rank H >= 2.
+// The rotation maximising sum t_i . R s_i over centred point sets, from H = sum (t_i - mt)(s_i - ms)^T, det R = +1, by Horn's
+// quaternion: q = the eigenvector of the largest eigenvalue of the symmetric 4x4 N below (Jacobi, every operation rounded; the
+// first largest diagonal entry), normalised, and R = R(q).  With s1 >= s2 >= s3 the singular values of H and d = det U det V, N's
+// eigenvalues are +-s1 +- s2 +- d s3 with an even number of minus signs, so the top one, s1 + s2 + d s3, is 2 (s2 + d s3) above
+// the next: R errs by O(eps s1 / (s2 + d s3)) (the eigenvectors of H^T H would err by O(eps (s1 / s2)^2)).  R(q) is
+// U diag(1, 1, d) V^T of the SVD of H, the reference's reflection fix (alignment.cpp:10-37), wherever that is unique
+// (s2 + d s3 > 0).  Otherwise (collinear or coincident points) it is still an optimal rotation, finite and proper, mapping the
+// source line onto the target line; R = I for H = 0.
 __device__ void rotation_se3(const double H[3][3], double R[3][3]) {
-  double M[3][3];
+  const double tr = __dadd_rn(__dadd_rn(H[0][0], H[1][1]), H[2][2]);
+  double N[4][4] = {
+      {tr, __dsub_rn(H[2][1], H[1][2]), __dsub_rn(H[0][2], H[2][0]), __dsub_rn(H[1][0], H[0][1])},
+      {0.0, __dsub_rn(__dsub_rn(H[0][0], H[1][1]), H[2][2]), __dadd_rn(H[0][1], H[1][0]), __dadd_rn(H[0][2], H[2][0])},
+      {0.0, 0.0, __dsub_rn(__dsub_rn(H[1][1], H[0][0]), H[2][2]), __dadd_rn(H[1][2], H[2][1])},
+      {0.0, 0.0, 0.0, __dsub_rn(__dsub_rn(H[2][2], H[0][0]), H[1][1])},
+  };
 #pragma unroll
-  for (int a = 0; a < 3; a++)
+  for (int a = 1; a < 4; a++)
 #pragma unroll
-    for (int b = 0; b < 3; b++) M[a][b] = __dadd_rn(__dadd_rn(__dmul_rn(H[0][a], H[0][b]), __dmul_rn(H[1][a], H[1][b])), __dmul_rn(H[2][a], H[2][b]));
-  double w[3], V[3][3];
-  jacobi_eigen3(M, w, V);
-  const double v1[3] = {V[0][2], V[1][2], V[2][2]}, v2[3] = {V[0][1], V[1][1], V[2][1]};
-  double u1[3], u2[3], u3[3], v3[3];
+    for (int b = 0; b < a; b++) N[a][b] = N[b][a];
+  double V[4][4];
+  jacobi_sweeps<4, true>(N, V);
+  // the column of the first largest diagonal entry, selected with constant indices so that N and V stay in registers
+  double top = N[0][0], q[4] = {V[0][0], V[1][0], V[2][0], V[3][0]};
 #pragma unroll
-  for (int a = 0; a < 3; a++) {
-    const double h[3] = {H[a][0], H[a][1], H[a][2]};
-    u1[a] = dot3(h, v1);
-    u2[a] = dot3(h, v2);
-  }
-  const double n1 = __dsqrt_rn(dot3(u1, u1));
+  for (int a = 1; a < 4; a++)
+    if (N[a][a] > top) {
+      top = N[a][a];
 #pragma unroll
-  for (int a = 0; a < 3; a++) u1[a] = __ddiv_rn(u1[a], n1);
-  const double p = dot3(u1, u2);
+      for (int b = 0; b < 4; b++) q[b] = V[b][a];
+    }
+  const double n = __dsqrt_rn(__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(q[0], q[0]), __dmul_rn(q[1], q[1])), __dmul_rn(q[2], q[2])), __dmul_rn(q[3], q[3])));
 #pragma unroll
-  for (int a = 0; a < 3; a++) u2[a] = __dsub_rn(u2[a], __dmul_rn(p, u1[a]));
-  const double n2 = __dsqrt_rn(dot3(u2, u2));
-#pragma unroll
-  for (int a = 0; a < 3; a++) u2[a] = __ddiv_rn(u2[a], n2);
-  cross3(u1, u2, u3);
-  cross3(v1, v2, v3);
-#pragma unroll
-  for (int a = 0; a < 3; a++)
-#pragma unroll
-    for (int b = 0; b < 3; b++) R[a][b] = __dadd_rn(__dadd_rn(__dmul_rn(u1[a], v1[b]), __dmul_rn(u2[a], v2[b])), __dmul_rn(u3[a], v3[b]));
+  for (int a = 0; a < 4; a++) q[a] = __ddiv_rn(q[a], n);
+  const double w = q[0], x = q[1], y = q[2], z = q[3];
+  const double xx = __dmul_rn(x, x), yy = __dmul_rn(y, y), zz = __dmul_rn(z, z);
+  const double xy = __dmul_rn(x, y), xz = __dmul_rn(x, z), yz = __dmul_rn(y, z), wx = __dmul_rn(w, x), wy = __dmul_rn(w, y), wz = __dmul_rn(w, z);
+  R[0][0] = __dsub_rn(1.0, __dmul_rn(2.0, __dadd_rn(yy, zz)));
+  R[0][1] = __dmul_rn(2.0, __dsub_rn(xy, wz));
+  R[0][2] = __dmul_rn(2.0, __dadd_rn(xz, wy));
+  R[1][0] = __dmul_rn(2.0, __dadd_rn(xy, wz));
+  R[1][1] = __dsub_rn(1.0, __dmul_rn(2.0, __dadd_rn(xx, zz)));
+  R[1][2] = __dmul_rn(2.0, __dsub_rn(yz, wx));
+  R[2][0] = __dmul_rn(2.0, __dsub_rn(xz, wy));
+  R[2][1] = __dmul_rn(2.0, __dadd_rn(yz, wx));
+  R[2][2] = __dsub_rn(1.0, __dmul_rn(2.0, __dadd_rn(xx, yy)));
 }
 
 // The planar rotation about z maximising sum t_i . R s_i, from H the top-left 2x2 of sum (t_i - mt)(s_i - ms)^T:

@@ -672,7 +672,12 @@ typedef struct b2_registration_result {
  *        sqrt((d0 d0 + d1 d1) + d2 d2) of the target / source points; above poly_error_thresh rejects [-2];
  *     4. T from the 3-point (dof 6) or 2-point (dof 4) alignment of the sampled source points onto their target points: the
  *        rotation maximising sum t_i . R s_i about the centroids (means ((a + b) + c) / 3, (a + b) / 2), with det R = +1 -- for dof 4
- *        the planar rotation about z, row and column 2 of R exactly e_z -- and t = mean_t - R mean_s;
+ *        the planar rotation about z, row and column 2 of R exactly e_z -- and t = mean_t - R mean_s.  With H = sum (t_i - mean_t)
+ *        (s_i - mean_s)^T (summed over the points in order), dof 6 takes Horn's quaternion: the unit eigenvector q of the largest
+ *        eigenvalue of the symmetric 4x4 N(H) (cyclic Jacobi, every operation rounded, the first largest diagonal entry), R = R(q);
+ *        its error grows as eps s1 / (s2 + d s3) with the singular values s of H and d = det U det V, as an SVD's does.  dof 4
+ *        takes (c, s) = (H00 + H11, H10 - H01) / its norm, or R = I when that norm is 0.  Collinear samples (rank-1 H) give a
+ *        proper rotation mapping the source line onto the target line, and H = 0 gives R = I;
  *     5. within taboo_thresh_rot (rotation angle of taboo^-1 T) and taboo_thresh_trans (translation distance) of a taboo pose
  *        rejects it [-3];
  *     6. count = the source points p with T p (b2_cloud_create_transformed's arithmetic) in a voxel of inlier_voxel_resolution
@@ -727,8 +732,8 @@ typedef struct b2_gnc_params {
  *        w = 1 if i = j = 0, else w = (mu / (mu + e)) * (mu / (mu + e));  num_inliers = #(e < (2 max_corr_dist)^2);
  *        sums (below): W = sum w, mt = (sum w t) / W, ms = (sum w s) / W, then in a second pass H = sum (w (t - mt)) (s - ms)^T
  *        (the top-left 2x2 for dof 4);
- *        R from H as b2_estimate_pose_ransac's step 4 computes it (dof 6: the top two eigenvectors of H^T H; dof 4: the planar
- *        (c, s)), t = mt - R ms, and T = [R | t].
+ *        R from H as b2_estimate_pose_ransac's step 4 computes it (dof 6: Horn's quaternion; dof 4: the planar (c, s)),
+ *        t = mt - R ms, and T = [R | t].
  *      After each outer iteration mu = mu / div_factor; the loop stops once mu < max_corr_dist.
  *   7. result: T, num_inliers of the last inner iteration (errors measured before that iteration's alignment),
  *      inlier_rate = num_inliers / |C|, hypothesis = -1.  |C| == 0, max_iterations == 0 or inner_iterations == 0 give the identity
@@ -746,7 +751,8 @@ typedef struct b2_gnc_params {
  * unstable (this can matter only without the reciprocal check, on the swapped side); (f) edge lengths and mu use the order above,
  * not Eigen's reduction; (g) num_threads has no meaning; (h) the reference tests `j == 0` inside its per-pair loop, whose index
  * shadows the inner-iteration counter, so there only pair 0 has weight 1 in the first outer iteration -- here, as the method
- * intends, the whole first alignment is unweighted.  With fewer than two non-collinear pairs R is ill-determined (dof 6). */
+ * intends, the whole first alignment is unweighted.  With fewer than two non-collinear pairs R is ill-determined (dof 6): it is then
+ * one of the optimal rotations (step 4 of b2_estimate_pose_ransac). */
 B2_API b2_status b2_estimate_pose_gnc(const b2_cloud* target, const b2_cloud* source, const b2_features* target_features, const b2_features* source_features,
                                       const b2_gnc_params* params, b2_registration_result* out, int64_t* out_correspondences, size_t capacity,
                                       size_t* out_num_correspondences);

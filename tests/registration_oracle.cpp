@@ -77,74 +77,74 @@ int pfh_bin(const double* f, bool* edge) {
   return feature_bin(f, 0, kPfhBins, edge) + kPfhBins * feature_bin(f, 1, kPfhBins, nullptr) + kPfhBins * kPfhBins * feature_bin(f, 2, kPfhBins, nullptr);
 }
 
-// Jacobi eigen-decomposition of a symmetric 3x3 (ascending eigenvalues, eigenvectors in the columns of V)
-void jacobi_eigen3(double A[3][3], double w[3], double V[3][3]) {
-  for (int i = 0; i < 3; i++)
-    for (int j = 0; j < 3; j++) V[i][j] = i == j ? 1.0 : 0.0;
+// cyclic Jacobi sweeps over a symmetric 4x4 (the device's jacobi_sweeps<4, true>): eigenvalues on the diagonal of A, eigenvectors in
+// the columns of V, unsorted
+void jacobi_sweeps4(double A[4][4], double V[4][4]) {
+  for (int i = 0; i < 4; i++)
+    for (int j = 0; j < 4; j++) V[i][j] = i == j ? 1.0 : 0.0;
   for (int sweep = 0; sweep < 64; sweep++) {
-    const double off = A[0][1] * A[0][1] + A[0][2] * A[0][2] + A[1][2] * A[1][2];
-    const double diag = A[0][0] * A[0][0] + A[1][1] * A[1][1] + A[2][2] * A[2][2];
+    double off = A[0][1] * A[0][1], diag = A[0][0] * A[0][0];
+    for (int p = 0; p < 3; p++)
+      for (int q = p + 1; q < 4; q++)
+        if (p + q > 1) off = off + A[p][q] * A[p][q];
+    for (int p = 1; p < 4; p++) diag = diag + A[p][p] * A[p][p];
     if (off <= 1e-32 * diag || off == 0.0) break;
-    for (int p = 0; p < 2; p++)
-      for (int q = p + 1; q < 3; q++) {
+    for (int p = 0; p < 3; p++)
+      for (int q = p + 1; q < 4; q++) {
         if (A[p][q] == 0.0) continue;
         const double theta = (A[q][q] - A[p][p]) / (2.0 * A[p][q]);
         const double t = (theta >= 0.0 ? 1.0 : -1.0) / (std::fabs(theta) + std::sqrt(theta * theta + 1.0));
         const double c = 1.0 / std::sqrt(t * t + 1.0), sn = t * c;
-        for (int k = 0; k < 3; k++) {
+        for (int k = 0; k < 4; k++) {
           const double akp = A[k][p], akq = A[k][q];
           A[k][p] = c * akp - sn * akq;
           A[k][q] = sn * akp + c * akq;
         }
-        for (int k = 0; k < 3; k++) {
+        for (int k = 0; k < 4; k++) {
           const double apk = A[p][k], aqk = A[q][k];
           A[p][k] = c * apk - sn * aqk;
           A[q][k] = sn * apk + c * aqk;
         }
-        for (int k = 0; k < 3; k++) {
+        for (int k = 0; k < 4; k++) {
           const double vkp = V[k][p], vkq = V[k][q];
           V[k][p] = c * vkp - sn * vkq;
           V[k][q] = sn * vkp + c * vkq;
         }
       }
   }
-  w[0] = A[0][0], w[1] = A[1][1], w[2] = A[2][2];
-  auto swap_cols = [&](int a, int b) {
-    if (w[b] < w[a]) {
-      std::swap(w[a], w[b]);
-      for (int i = 0; i < 3; i++) std::swap(V[i][a], V[i][b]);
-    }
-  };
-  swap_cols(0, 1);
-  swap_cols(1, 2);
-  swap_cols(0, 1);
 }
 
-// The rotation from H = sum (t_i - mt)(s_i - ms)^T maximising sum t_i . R s_i, det R = +1 (the device's rotation_se3);
-// *degenerate: H has rank < 2, so R is ill-determined
+// The rotation from H = sum (t_i - mt)(s_i - ms)^T maximising sum t_i . R s_i, det R = +1 (the device's rotation_se3: Horn's
+// quaternion, the top eigenvector of the 4x4 N); *degenerate: the top eigenvalue of N lies within 2e-4 of its size above the next,
+// i.e. s2 + d s3 <~ 1e-4 s1 for the singular values s of H, so R is ill-determined
 void rotation_se3(const double H[3][3], double R[3][3], bool* degenerate) {
-  double M[3][3];
-  for (int a = 0; a < 3; a++)
-    for (int b = 0; b < 3; b++) M[a][b] = (H[0][a] * H[0][b] + H[1][a] * H[1][b]) + H[2][a] * H[2][b];
-  double w[3], V[3][3];
-  jacobi_eigen3(M, w, V);
-  *degenerate = !(w[1] > 1e-8 * w[2]);
-  const double v1[3] = {V[0][2], V[1][2], V[2][2]}, v2[3] = {V[0][1], V[1][1], V[2][1]};
-  double u1[3], u2[3], u3[3], v3[3];
-  for (int a = 0; a < 3; a++) {
-    u1[a] = dot3(H[a], v1);
-    u2[a] = dot3(H[a], v2);
-  }
-  const double n1 = std::sqrt(dot3(u1, u1));
-  for (double& x : u1) x = x / n1;
-  const double p = dot3(u1, u2);
-  for (int a = 0; a < 3; a++) u2[a] = u2[a] - p * u1[a];
-  const double n2 = std::sqrt(dot3(u2, u2));
-  for (double& x : u2) x = x / n2;
-  cross3(u1, u2, u3);
-  cross3(v1, v2, v3);
-  for (int a = 0; a < 3; a++)
-    for (int b = 0; b < 3; b++) R[a][b] = (u1[a] * v1[b] + u2[a] * v2[b]) + u3[a] * v3[b];
+  const double tr = (H[0][0] + H[1][1]) + H[2][2];
+  double N[4][4] = {
+      {tr, H[2][1] - H[1][2], H[0][2] - H[2][0], H[1][0] - H[0][1]},
+      {0.0, (H[0][0] - H[1][1]) - H[2][2], H[0][1] + H[1][0], H[0][2] + H[2][0]},
+      {0.0, 0.0, (H[1][1] - H[0][0]) - H[2][2], H[1][2] + H[2][1]},
+      {0.0, 0.0, 0.0, (H[2][2] - H[0][0]) - H[1][1]},
+  };
+  for (int a = 1; a < 4; a++)
+    for (int b = 0; b < a; b++) N[a][b] = N[b][a];
+  double V[4][4];
+  jacobi_sweeps4(N, V);
+  int k = 0;
+  for (int a = 1; a < 4; a++) k = N[a][a] > N[k][k] ? a : k;
+  double second = -INFINITY;
+  for (int a = 0; a < 4; a++)
+    if (a != k) second = std::max(second, N[a][a]);
+  *degenerate = !(N[k][k] - second > 2e-4 * N[k][k]);
+  double q[4];
+  for (int a = 0; a < 4; a++) q[a] = V[a][k];
+  const double n = std::sqrt(((q[0] * q[0] + q[1] * q[1]) + q[2] * q[2]) + q[3] * q[3]);
+  for (double& v : q) v = v / n;
+  const double w = q[0], x = q[1], y = q[2], z = q[3];
+  const double xx = x * x, yy = y * y, zz = z * z, xy = x * y, xz = x * z, yz = y * z, wx = w * x, wy = w * y, wz = w * z;
+  const double R9[3][3] = {{1.0 - 2.0 * (yy + zz), 2.0 * (xy - wz), 2.0 * (xz + wy)},
+                           {2.0 * (xy + wz), 1.0 - 2.0 * (xx + zz), 2.0 * (yz - wx)},
+                           {2.0 * (xz - wy), 2.0 * (yz + wx), 1.0 - 2.0 * (xx + yy)}};
+  std::memcpy(R, R9, sizeof(R9));
 }
 
 // The planar rotation about z from the top-left 2x2 of H (the device's rotation_4dof)
@@ -223,6 +223,16 @@ int64_t nearest(const double* q, const double* T, size_t nt, int D, double* out_
 extern "C" {
 
 int orc_reg_max_threads() { return omp_get_max_threads(); }
+
+// One RANSAC hypothesis' alignment of the ns = 3 (dof 6) or 2 (dof 4) source points s (ns x 3) onto the target points t: T (rows of
+// [R | t], 12), *degenerate as in orc_ransac.
+void orc_align(int ns, const double* t, const double* s, double* T, unsigned char* degenerate) {
+  const double* tp[3] = {t, t + 3, t + 6};
+  const double* sp[3] = {s, s + 3, s + 6};
+  bool deg = false;
+  align(ns, tp, sp, T, &deg);
+  *degenerate = deg;
+}
 
 // FPFH of n points (pts, nrm: n x 3) over brute-force radius neighbours; out n x 33; edge[i] = 1 if a pair entering row i (a pair
 // of i or of one of its neighbours) has some nf * 11 within 1e-9 of an integer.  num_neighbors[i] = |N_i|.

@@ -29,6 +29,8 @@ def lib():
     L.orc_gnc.restype = None
     L.orc_gnc.argtypes = [_dp, C.c_size_t, _dp, C.c_size_t, _dp, _dp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int,
                           C.c_int, C.c_int, C.c_uint64, C.c_int, _lp, _lp, _lp, _lp, _ip, _ip, _lp, _lp, _bp, _dp]
+    L.orc_align.restype = None
+    L.orc_align.argtypes = [C.c_int, _dp, _dp, _dp, _bp]
     for fn in (L.orc_pfh, L.orc_fpfh_at):
         fn.restype = None
         fn.argtypes = [_dp, _dp, C.c_size_t, _lp, C.c_size_t, C.c_double, C.c_size_t, C.c_int, _dp, _bp, _lp]
@@ -90,6 +92,18 @@ def ransac(target, source, target_features, source_features, max_iterations=5000
                      status.ctypes.data_as(_ip), T.ctypes.data_as(_dp), slack.ctypes.data_as(_ip), deg.ctypes.data_as(_bp), res.ctypes.data_as(_dp))
     return dict(samples=samples[:K], targets=targets[:K], status=status[:K], T=T[:K].reshape(K, 3, 4), slack=slack[:K], degenerate=deg[:K].astype(bool),
                 T_target_source=res[:16].reshape(4, 4), inlier_rate=res[16], num_inliers=int(res[17]), hypothesis=int(res[18]))
+
+
+def align(target, source):
+    """One RANSAC hypothesis' alignment of 3 (dof 6) or 2 (dof 4) source points onto their target points, as
+    b2_estimate_pose_ransac's step 4 computes it -> (T 3 x 4, degenerate)."""
+    tp, sp = _f64(target, 3), _f64(source, 3)
+    ns = len(tp)
+    assert ns in (2, 3) and len(sp) == ns
+    T = np.zeros(12)
+    deg = np.zeros(1, dtype=np.uint8)
+    lib().orc_align(ns, tp.ctypes.data_as(_dp), sp.ctypes.data_as(_dp), T.ctypes.data_as(_dp), deg.ctypes.data_as(_bp))
+    return T.reshape(3, 4), bool(deg[0])
 
 
 def gnc(target, source, target_features, source_features, max_init_samples=5000, reciprocal_check=True, tuple_check=False, max_num_tuples=1000,

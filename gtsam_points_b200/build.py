@@ -16,7 +16,7 @@ LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(HERE, "build")
 LIB = os.path.join(LIBDIR, "libb2points.so")
 
-SOURCES = ["b2_context.cu", "b2_cloud.cu", "b2_voxelmap.cu", "b2_kdtree.cu", "b2_factors.cu", "b2_registration.cu", "b2_filter.cu", "b2_segmentation.cu"]
+SOURCES = ["b2_context.cu", "b2_cloud.cu", "b2_voxelmap.cu", "b2_kdtree.cu", "b2_factors.cu", "b2_registration.cu", "b2_filter.cu", "b2_segmentation.cu", "b2_occupancy.cu"]
 HEADERS = ["b2_internal.hpp", "b2_device.cuh", "b2_kdtree.cuh", "b2_factor_kernel_ws.cuh", os.path.join("..", "..", "include", "b2points.h")]
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

@@ -59,6 +59,10 @@ class MinCutResultC(C.Structure):
 B2_MIN_CUT_NO_SEED, B2_MIN_CUT_FEW_NEIGHBORS, B2_MIN_CUT_NO_SINK = 1, 2, 4
 
 
+class OccGridInfo(C.Structure):
+    _fields_ = [("resolution", C.c_double), ("num_occupied_cells", C.c_uint64), ("num_blocks", C.c_uint64), ("device_bytes", C.c_uint64)]
+
+
 class FeaturesInfo(C.Structure):
     _fields_ = [("num_features", C.c_uint64), ("dim", C.c_int32), ("reserved", C.c_int32), ("device_bytes", C.c_uint64)]
 
@@ -171,6 +175,14 @@ SIGNATURES = {
     "b2_region_growing_get": (C.c_int, [_vp, C.POINTER(C.c_uint64), _lp]),
     "b2_region_growing_destroy": (C.c_int, [_vp]),
     "b2_min_cut": (C.c_int, [_vp, _vp, C.c_int64, _dp, C.POINTER(MinCutParamsC), C.POINTER(MinCutResultC), _lp, _lp]),
+    "b2_occgrid_create": (C.c_int, [_vp, C.c_double, _pp]),
+    "b2_occgrid_destroy": (C.c_int, [_vp]),
+    "b2_occgrid_get_info": (C.c_int, [_vp, C.POINTER(OccGridInfo)]),
+    "b2_occgrid_insert": (C.c_int, [_vp, _vp, _dp]),
+    "b2_occgrid_overlap": (C.c_int, [_vp, _vp, _dp, C.c_size_t, C.POINTER(C.c_uint64), C.POINTER(C.c_uint8)]),
+    "b2_occgrid_free_rays": (C.c_int, [_vp, _vp, _dp]),
+    "b2_occgrid_download": (C.c_int, [_vp, _ip]),
+    "b2_raycast": (C.c_int, [_vp, _dp, _dp, C.c_size_t, C.c_double, C.POINTER(C.c_uint64), C.c_size_t, _ip]),
     "b2_vgicp_factor_create": (C.c_int, [_vp, _vp, _vp, _pp]),
     "b2_gicp_factor_create": (C.c_int, [_vp, _vp, _vp, _vp, _pp]),
     "b2_icp_factor_create": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int, _dp, _pp]),

@@ -545,6 +545,80 @@ inline MinCutResult min_cut_gpu(const PointCloudGPU::ConstPtr& points, const KdT
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
+// Occupancy (ann/fast_occupancy_grid.hpp, util/voxel_raycaster.hpp): FastOccupancyGrid on device clouds and VoxelRaycaster rows.
+// Poses are row-major 4x4 (the matrix of an Eigen::Isometry3d); see b2_occgrid_* / b2_raycast for the keying and the differences.
+// ---------------------------------------------------------------------------------------------------------------------
+class FastOccupancyGridGPU {
+public:
+  using Ptr = std::shared_ptr<FastOccupancyGridGPU>;
+  using ConstPtr = std::shared_ptr<const FastOccupancyGridGPU>;
+  static Mat4 identity() { return Mat4{1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1}; }
+  explicit FastOccupancyGridGPU(double resolution, Context::Ptr ctx = Context::default_context()) : ctx_(ctx) {
+    check(b2_occgrid_create(ctx_->get(), resolution, &grid_), "b2_occgrid_create");
+  }
+  ~FastOccupancyGridGPU() { b2_occgrid_destroy(grid_); }
+  FastOccupancyGridGPU(const FastOccupancyGridGPU&) = delete;
+
+  void insert(const PointCloudGPU& points, const Mat4& pose = identity()) { check(b2_occgrid_insert(grid_, points.handle(), pose.data()), "b2_occgrid_insert"); }
+  // Clears the occupied cells crossed by the rays from pose's translation to the posed points (end voxels excluded); call before insert
+  void free_rays(const PointCloudGPU& points, const Mat4& pose = identity()) {
+    check(b2_occgrid_free_rays(grid_, points.handle(), pose.data()), "b2_occgrid_free_rays");
+  }
+  int calc_overlap(const PointCloudGPU& points, const Mat4& pose = identity()) const { return static_cast<int>(calc_overlaps(points, {pose})[0]); }
+  // count / n; 0 for an empty cloud
+  double calc_overlap_rate(const PointCloudGPU& points, const Mat4& pose = identity()) const {
+    return points.size() ? calc_overlap(points, pose) / static_cast<double>(points.size()) : 0.0;
+  }
+  std::vector<unsigned char> get_overlaps(const PointCloudGPU& points, const Mat4& pose = identity()) const {
+    std::uint64_t count = 0;
+    std::vector<unsigned char> flags(points.size());
+    check(b2_occgrid_overlap(grid_, points.handle(), pose.data(), 1, &count, flags.data()), "b2_occgrid_overlap");
+    return flags;
+  }
+  // calc_overlap under every pose, one launch
+  std::vector<std::uint64_t> calc_overlaps(const PointCloudGPU& points, const std::vector<Mat4>& poses) const {
+    if (poses.empty()) return {};
+    std::vector<double> Ts;
+    for (const Mat4& T : poses) Ts.insert(Ts.end(), T.begin(), T.end());
+    std::vector<std::uint64_t> counts(poses.size());
+    check(b2_occgrid_overlap(grid_, points.handle(), Ts.data(), poses.size(), counts.data(), nullptr), "b2_occgrid_overlap");
+    return counts;
+  }
+  int num_occupied_cells() const {
+    b2_occgrid_info info{};
+    check(b2_occgrid_get_info(grid_, &info), "b2_occgrid_get_info");
+    return static_cast<int>(info.num_occupied_cells);
+  }
+  // The occupied cells, ascending key order (z, then y, then x)
+  std::vector<std::array<int, 3>> occupied_cells() const {
+    std::vector<std::array<int, 3>> cells(num_occupied_cells());
+    check(b2_occgrid_download(grid_, cells.empty() ? nullptr : cells[0].data()), "b2_occgrid_download");
+    return cells;
+  }
+  b2_occgrid* handle() const { return grid_; }
+
+private:
+  Context::Ptr ctx_;
+  b2_occgrid* grid_ = nullptr;
+};
+
+// VoxelRaycaster(start, end, voxel_size) for every row: row i of the result is the sequence from begin() up to, not including, end_voxel()
+inline std::vector<std::vector<std::array<int, 3>>> raycast_gpu(const std::vector<std::array<double, 3>>& starts, const std::vector<std::array<double, 3>>& ends,
+                                                                double voxel_size, Context::Ptr ctx = Context::default_context()) {
+  if (starts.size() != ends.size()) throw std::invalid_argument("raycast_gpu: starts and ends differ in size");
+  const std::size_t n = starts.size();
+  std::vector<std::uint64_t> off(n + 1);
+  const double* s = n ? starts[0].data() : nullptr;
+  const double* e = n ? ends[0].data() : nullptr;
+  check(b2_raycast(ctx->get(), s, e, n, voxel_size, off.data(), 0, nullptr), "b2_raycast");
+  std::vector<std::array<int, 3>> coords(off[n]);
+  if (off[n]) check(b2_raycast(ctx->get(), s, e, n, voxel_size, off.data(), coords.size(), coords[0].data()), "b2_raycast");
+  std::vector<std::vector<std::array<int, 3>>> rows(n);
+  for (std::size_t i = 0; i < n; i++) rows[i].assign(coords.begin() + off[i], coords.begin() + off[i + 1]);
+  return rows;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
 // Global registration (features/fpfh_estimation.hpp, registration/ransac.hpp, registration/graduated_non_convexity.hpp): features,
 // FPFH, RANSAC and GNC on the device
 // ---------------------------------------------------------------------------------------------------------------------

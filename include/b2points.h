@@ -555,6 +555,70 @@ B2_API b2_status b2_min_cut(const b2_cloud* cloud, const b2_kdtree* tree, int64_
                             b2_min_cut_result* info, int64_t* out_indices, int64_t* out_capacities);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Occupancy grid and voxel ray traversal (include/gtsam_points/ann/fast_occupancy_grid.hpp, ann/impl/fast_occupancy_grid_impl.hpp,
+ * src/gtsam_points/ann/fast_occupancy_grid.cpp; include/gtsam_points/util/voxel_raycaster.hpp, src/gtsam_points/util/voxel_raycaster.cpp).
+ * FastOccupancyGrid on device clouds: a set of occupied cells of edge `resolution`, stored as the reference stores it (8^3-cell blocks
+ * of 512-bit bitmaps in an open-addressed table).
+ *   posing:   T is 16 doubles, row-major, every entry finite (B2_ERR_INVALID_ARGUMENT otherwise); NULL uses the stored points as they
+ *             are.  A point is posed as transform() poses it, ((T_r0 x + T_r1 y) + T_r2 z) + T_r3 on the stored values (the values
+ *             b2_cloud_download returns), so float32-compact and Morton-ordered clouds give the results of their downloaded rows.
+ *   keying:   the cell of q is c = floor(q * (1 / resolution)) per axis, the key voxelgrid_sampling, merge_frames and RANSAC use.  A
+ *             point whose c is outside [-2^20, 2^20 - 1] on some axis, or whose posed coordinates are not finite, cannot be keyed: it
+ *             is never inserted, never overlaps and gets flag 0.
+ *   results:  insert adds cells, free_rays removes them, overlap tests membership.  Every result is independent of thread order;
+ *             download and num_occupied_cells are bit-reproducible.  calc_overlap_rate = count / n in double.
+ *   devices:  the cloud must live on the grid's device (B2_ERR_INVALID_ARGUMENT otherwise); its context may differ, and the work
+ *             runs on the grid's stream.  Every check runs before the grid changes.
+ * Deliberate differences from the reference:
+ *   (a) key range: the reference adds 2^20 to c and divides by 8 with C's truncation, so a coordinate outside [-2^20, 2^20 - 1]
+ *       lands in a wrong block or indexes a bitset out of bounds; here such a point is dropped.  Inside the range the cells agree.
+ *   (b) an empty cloud has overlap rate 0 (b2_overlap's convention); the reference computes 0 / 0.
+ *   (c) b2_raycast rejects a non-finite endpoint or a voxel coordinate outside int32, where the reference loops or has undefined
+ *       behaviour.
+ *   (d) additions: overlap under num_poses poses in one call, and free_rays (the reference has no single function for it). */
+typedef struct b2_occgrid b2_occgrid;
+typedef struct b2_occgrid_info {
+  double resolution;
+  uint64_t num_occupied_cells;
+  uint64_t num_blocks;    /* table slots holding a block; a block emptied by free_rays keeps its slot, as in the reference */
+  uint64_t device_bytes;
+} b2_occgrid_info;
+/* FastOccupancyGrid(resolution): resolution > 0 and finite */
+B2_API b2_status b2_occgrid_create(b2_ctx* ctx, double resolution, b2_occgrid** out);
+B2_API b2_status b2_occgrid_destroy(b2_occgrid* grid);
+B2_API b2_status b2_occgrid_get_info(const b2_occgrid* grid, b2_occgrid_info* info);
+/* insert(points, pose): the cell of every keyed point of `cloud` posed by T becomes occupied.  The table grows before the launch to
+ * hold every block the insert can add, so no cell is ever dropped. */
+B2_API b2_status b2_occgrid_insert(b2_occgrid* grid, const b2_cloud* cloud, const double* T);
+/* calc_overlap / get_overlaps for num_poses >= 1 poses in one call.  Ts: num_poses x 16 doubles, or NULL (every pose the stored
+ * points as they are).  out_counts[j] (always written) = the number of points p with the cell of T_j p occupied; out_flags (NULL, or
+ * num_poses x n bytes) row j = those hits as 0 / 1 per point in the cloud's CALLER order. */
+B2_API b2_status b2_occgrid_overlap(const b2_occgrid* grid, const b2_cloud* cloud, const double* Ts, size_t num_poses, uint64_t* out_counts, uint8_t* out_flags);
+/* Free-space clearing, a composition of the reference's two primitives: for every point p of `cloud`, FastOccupancyBlock::set_free
+ * on every voxel of VoxelRaycaster(o, T p, resolution) from begin() up to, not including, end_voxel() -- b2_raycast's row of
+ * (o, T p) -- where o = T's translation (T[3], T[7], T[11]) taken as is (0 for T == NULL).  A cell outside the key range, or in a
+ * block the grid does not have, is left alone: clearing never creates a block.  Rays whose end point cannot be keyed are skipped.
+ * o's voxel coordinate must lie in int32 (B2_ERR_INVALID_ARGUMENT).  Clearing is idempotent, so the result is order-free.  The
+ * usual scan update is free_rays followed by insert of the same scan and pose. */
+B2_API b2_status b2_occgrid_free_rays(b2_occgrid* grid, const b2_cloud* cloud, const double* T);
+/* The occupied cells, num_occupied_cells x 3 int32 coordinates c, in ascending key order (x | y << 21 | z << 42 of c + 2^20: z, then
+ * y, then x).  out_coords may be NULL for an empty grid. */
+B2_API b2_status b2_occgrid_download(const b2_occgrid* grid, int32_t* out_coords);
+/* VoxelRaycaster(start_i, end_i, voxel_size) for n rays (starts, ends: host, n x 3): row i is the iterator's sequence from begin()
+ * up to, not including, end_voxel().  out_offsets (n + 1, always written) is CSR as in b2_kdtree_radius_search; out_coords NULL
+ * counts only, else it needs capacity >= offsets[n] entries x 3 int32 (B2_ERR_INVALID_ARGUMENT otherwise, offsets still written).
+ * The arithmetic, every operation rounded on its own, with inv = 1.0 / voxel_size and per axis a:
+ *   c_a = fast_floor(s_a * inv), e_a = fast_floor(end_a * inv), d_a = end_a - s_a, step_a = sign(d_a);
+ *   axis a is valid iff |d_a| > 1e-9; t_delta_a = voxel_size / |d_a|, t_max_a = ((c_a + (step_a > 0)) * voxel_size - s_a) / d_a
+ *   (both +inf on an invalid axis);
+ *   while c != e: emit c; m = t_x < t_y && t_x < t_z ? x : (t_y < t_z ? y : z); stop if t_max_m > 1.0 + 1e-9; c_m += step_m;
+ *   t_max_m += t_delta_m; stop if c passed e on some axis in the direction of its step.
+ * So a ray whose start voxel is its end voxel gives an empty row.  A non-finite endpoint coordinate, or one whose voxel coordinate
+ * floor(x * inv) lies outside int32, is B2_ERR_INVALID_ARGUMENT (the offsets are then unspecified). */
+B2_API b2_status b2_raycast(b2_ctx* ctx, const double* starts, const double* ends, size_t n, double voxel_size, uint64_t* out_offsets, size_t capacity,
+                            int32_t* out_coords);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Global registration: FPFH features, exact feature-space nearest neighbours, RANSAC and GNC pose estimation
  * (include/gtsam_points/features/fpfh_estimation.hpp, src/gtsam_points/features/fpfh_estimation.cpp:196-327,
  *  include/gtsam_points/registration/ransac.hpp, registration/impl/ransac_impl.hpp, src/gtsam_points/registration/alignment.cpp,

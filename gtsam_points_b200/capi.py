@@ -187,6 +187,7 @@ SIGNATURES = {
     "b2_gicp_factor_create": (C.c_int, [_vp, _vp, _vp, _vp, _pp]),
     "b2_icp_factor_create": (C.c_int, [_vp, _vp, _vp, _vp, C.c_int, _dp, _pp]),
     "b2_gicp_ivox_factor_create": (C.c_int, [_vp, _vp, _vp, _pp]),
+    "b2_icp_ivox_factor_create": (C.c_int, [_vp, _vp, _vp, C.c_int, _pp]),
     "b2_factor_destroy": (C.c_int, [_vp]),
     "b2_factor_set_max_correspondence_distance": (C.c_int, [_vp, C.c_double]),
     "b2_factor_set_correspondence_update_tolerance": (C.c_int, [_vp, C.c_double, C.c_double]),

@@ -1385,10 +1385,21 @@ public:
   IntegratedICPFactor(Key target_key, Key source_key, const std::shared_ptr<const TargetFrame>& target, const std::shared_ptr<const SourceFrame>& source, Context::Ptr ctx = Context::default_context())
   : IntegratedICPFactor(target_key, source_key, PointCloudGPU::from_frame(target, ctx), PointCloudGPU::from_frame(source, ctx),
                         std::make_shared<KdTreeGPU>(reinterpret_cast<const double*>(target->points), 4, target->size(), ctx)) {}
+  // IntegratedICPFactor_<iVox, PointCloud> / <iVoxCovarianceEstimation, PointCloud> (src/gtsam_points/factors/integrated_icp_factor.cpp:9-10):
+  // the iVox is target and search structure at once; correspondences are iVox indices; after the map changes the factor
+  // re-associates before it reads them.  Point-to-plane takes the normals an iVoxCovarianceEstimationGPU estimates.
+  IntegratedICPFactor(Key target_key, Key source_key, const iVoxGPU::ConstPtr& target, const PointCloudGPU::ConstPtr& source, bool use_point_to_plane = false)
+  : IntegratedMatchingCostFactorB200(target_key, source_key), source_(source), ivox_(target), plane_(use_point_to_plane) {
+    init(nullptr);
+  }
+  IntegratedICPFactor(const FixedPose& fixed_target_pose, Key source_key, const iVoxGPU::ConstPtr& target, const PointCloudGPU::ConstPtr& source, bool use_point_to_plane = false)
+  : IntegratedMatchingCostFactorB200(pose_matrix(fixed_target_pose), source_key), source_(source), ivox_(target), plane_(use_point_to_plane) {
+    init(nullptr);
+  }
 
   void print(const std::string& s = "", const KeyFormatter& keyFormatter = &default_key_format) const override {
     print_keys(s, plane_ ? "IntegratedPointToPlaneICPFactor" : "IntegratedICPFactor", keyFormatter);
-    std::cout << "|target|=" << target_->size() << "pts, |source|=" << source_->size() << "pts" << std::endl;
+    std::cout << "|target|=" << (ivox_ ? ivox_->size() : target_->size()) << "pts, |source|=" << source_->size() << "pts" << std::endl;
   }
   void set_num_threads(int) {}
   void set_max_correspondence_distance(double dist) { check(b2_factor_set_max_correspondence_distance(factor_, dist), "b2_factor_set_max_correspondence_distance"); }
@@ -1398,16 +1409,29 @@ public:
   // NonlinearFactor::clone: a new factor over the same (shared) target, source and search tree
   FactorBasePtr clone() const override {
     const double* nrm = normals_.empty() ? nullptr : normals_.data();
-    if (is_binary_) return FactorBasePtr(new IntegratedICPFactor(this->keys()[0], this->keys()[1], target_, source_, tree_, plane_, nrm));
-    IntegratedICPFactor* f = new IntegratedICPFactor(this->keys()[0], this->keys()[0], target_, source_, tree_, plane_, nrm);
+    auto make = [&](Key target_key, Key source_key) {
+      return ivox_ ? new IntegratedICPFactor(target_key, source_key, ivox_, source_, plane_) : new IntegratedICPFactor(target_key, source_key, target_, source_, tree_, plane_, nrm);
+    };
+    if (is_binary_) return FactorBasePtr(make(this->keys()[0], this->keys()[1]));
+    IntegratedICPFactor* f = make(this->keys()[0], this->keys()[0]);
     f->is_binary_ = false;
     f->fixed_target_pose_ = fixed_target_pose_;
     f->keys_.erase(f->keys_.begin());
     return FactorBasePtr(f);
   }
+  iVoxGPU::ConstPtr get_target_ivox() const { return ivox_; }
 
 private:
   void init(const double* target_normals) {
+    if (ivox_) {
+      // integrated_icp_factor_impl.hpp:36-50: an empty iVox has no points; a plain iVox keeps no normals (b2_icp_ivox_factor_create)
+      if (!source_ || ivox_->num_voxels() == 0 || (plane_ && !std::dynamic_pointer_cast<const iVoxCovarianceEstimationGPU>(ivox_))) {
+        std::cerr << "error: target frame doesn't have required attributes for icp" << std::endl;
+        abort();
+      }
+      check(b2_icp_ivox_factor_create(source_->context()->get(), ivox_->handle(), source_->handle(), plane_ ? 1 : 0, &factor_), "b2_icp_ivox_factor_create");
+      return;
+    }
     if (!source_ || !target_ || !tree_ || (plane_ && target_normals == nullptr && !target_->has_normals())) {
       std::cerr << "error: target frame doesn't have required attributes for icp" << std::endl;  // integrated_icp_factor_impl.hpp:36-50
       abort();
@@ -1417,8 +1441,26 @@ private:
   }
   PointCloudGPU::ConstPtr target_, source_;
   KdTreeGPU::ConstPtr tree_;
+  iVoxGPU::ConstPtr ivox_;
   bool plane_;
   std::vector<double> normals_;
+};
+
+// IntegratedPointToPlaneICPFactor_ (include/gtsam_points/factors/integrated_icp_factor.hpp:147-175): IntegratedICPFactor with
+// use_point_to_plane = true, on a kd-tree target with normals or on an iVoxCovarianceEstimationGPU.
+class IntegratedPointToPlaneICPFactor : public IntegratedICPFactor {
+public:
+  using shared_ptr = std::shared_ptr<IntegratedPointToPlaneICPFactor>;
+  IntegratedPointToPlaneICPFactor(Key target_key, Key source_key, const PointCloudGPU::ConstPtr& target, const PointCloudGPU::ConstPtr& source,
+                                  const KdTreeGPU::ConstPtr& target_tree, const double* target_normals = nullptr)
+  : IntegratedICPFactor(target_key, source_key, target, source, target_tree, true, target_normals) {}
+  IntegratedPointToPlaneICPFactor(const FixedPose& fixed_target_pose, Key source_key, const PointCloudGPU::ConstPtr& target, const PointCloudGPU::ConstPtr& source,
+                                  const KdTreeGPU::ConstPtr& target_tree, const double* target_normals = nullptr)
+  : IntegratedICPFactor(fixed_target_pose, source_key, target, source, target_tree, true, target_normals) {}
+  IntegratedPointToPlaneICPFactor(Key target_key, Key source_key, const iVoxGPU::ConstPtr& target, const PointCloudGPU::ConstPtr& source)
+  : IntegratedICPFactor(target_key, source_key, target, source, true) {}
+  IntegratedPointToPlaneICPFactor(const FixedPose& fixed_target_pose, Key source_key, const iVoxGPU::ConstPtr& target, const PointCloudGPU::ConstPtr& source)
+  : IntegratedICPFactor(fixed_target_pose, source_key, target, source, true) {}
 };
 
 // estimate_covariances (include/gtsam_points/features/covariance_estimation.hpp:41-66) on the device: k nearest neighbours over a

@@ -87,6 +87,10 @@ template <>
 struct KindTraits<B2_FACTOR_ICP_PLANE> : Traits<TreeProbeWarps, Search::Tree, false, 2> {};
 template <>
 struct KindTraits<B2_FACTOR_GICP_IVOX> : Traits<TreeProbeWarps, Search::Ivox, true, 0> {};
+template <>
+struct KindTraits<B2_FACTOR_ICP_IVOX> : Traits<TreeProbeWarps, Search::Ivox, false, 1> {};
+template <>
+struct KindTraits<B2_FACTOR_ICP_PLANE_IVOX> : Traits<TreeProbeWarps, Search::Ivox, false, 2> {};
 // VGICP with surface validation.  A probe lane also holds its points' normals from the coordinate load to the rejection test.  With
 // two points per lane that does not fit the 88 probe registers for launches over sets (ptxas: 120 - 144 bytes of stack), and the
 // accumulate warps cannot give any up (below 168 they spill).  One point per lane fits with 0 spill bytes in every instantiation.
@@ -701,6 +705,18 @@ validated_vgicp_kernel(const FactorDesc* __restrict__ descs, const uint32_t* __r
                        const double* __restrict__ poses_eval, double* __restrict__ partials, unsigned int* __restrict__ counters, double* __restrict__ out,
                        const __grid_constant__ DoneSignal sig, const __grid_constant__ PoseArg pose, const uint32_t* __restrict__ frozen_flags) {
   factor_kernel_body<PT, CT, B2_FACTOR_VGICP_VALIDATED, MODE, SINGLE>(descs, tile_factor, num_tiles, poses_lin, poses_eval, partials, counters, out, sig, pose, frozen_flags);
+}
+
+// The kernel of ICP and point-to-plane ICP on an iVox (KIND B2_FACTOR_ICP_IVOX / B2_FACTOR_ICP_PLANE_IVOX).  `factor_kernel`'s body
+// under a name of its own, for the same reason as validated_vgicp_kernel: the suite pins the set of `factor_kernel` instantiations,
+// and tests these apart.
+template <typename PT, typename CT, int KIND, int MODE, bool SINGLE = false>
+__global__ void __launch_bounds__(KindTraits<KIND>::kThreads, 1)
+ivox_icp_kernel(const FactorDesc* __restrict__ descs, const uint32_t* __restrict__ tile_factor, uint32_t num_tiles, const double* __restrict__ poses_lin,
+                const double* __restrict__ poses_eval, double* __restrict__ partials, unsigned int* __restrict__ counters, double* __restrict__ out,
+                const __grid_constant__ DoneSignal sig, const __grid_constant__ PoseArg pose, const uint32_t* __restrict__ frozen_flags) {
+  static_assert(KIND == B2_FACTOR_ICP_IVOX || KIND == B2_FACTOR_ICP_PLANE_IVOX, "iVox ICP kinds only");
+  factor_kernel_body<PT, CT, KIND, MODE, SINGLE>(descs, tile_factor, num_tiles, poses_lin, poses_eval, partials, counters, out, sig, pose, frozen_flags);
 }
 
 }  // namespace ws

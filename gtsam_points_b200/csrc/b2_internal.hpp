@@ -459,6 +459,11 @@ struct b2_ivox {
   // never passes the strict '<' of ivox_nn1), rebuilt after every insert.
   b2::DeviceBuffer d_valid_records;
   const b2::DeviceBuffer& search_records() const { return cov_est ? d_valid_records : map.d_records; }
+  // The plane view, the records point-to-plane ICP searches: the valid view's points, the estimated normal in slots 3..5, zeros
+  // in 6..8, count 1.  Written with the valid view once a point-to-plane factor has been created on the map (ivox_enable_plane_view);
+  // never dropped after that.  A cache of the map's state, so building it leaves a const map's contents as they were.
+  mutable bool plane_view = false;
+  mutable b2::DeviceBuffer d_plane_records;
   b2::DeviceBuffer d_stats, d_stats_part;  // per-insert scratch of the statistics, grown on demand
   // CUDA events at the boundaries of the last insert's phases: start, base insert, estimation pass, statistics, removal + valid view
   cudaEvent_t phase_ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
@@ -487,12 +492,24 @@ struct b2_features {
 
 // B2_FACTOR_VGICP_VALIDATED names a kernel instantiation only (a VGICP factor with surface validation on, launch_kind below);
 // b2_factor::kind never holds it.
-enum b2_factor_kind { B2_FACTOR_VGICP = 0, B2_FACTOR_GICP = 1, B2_FACTOR_ICP = 2, B2_FACTOR_ICP_PLANE = 3, B2_FACTOR_GICP_IVOX = 4, B2_FACTOR_VGICP_VALIDATED = 5 };
+enum b2_factor_kind {
+  B2_FACTOR_VGICP = 0,
+  B2_FACTOR_GICP = 1,
+  B2_FACTOR_ICP = 2,
+  B2_FACTOR_ICP_PLANE = 3,
+  B2_FACTOR_GICP_IVOX = 4,
+  B2_FACTOR_VGICP_VALIDATED = 5,
+  B2_FACTOR_ICP_IVOX = 6,        // point-to-point ICP on an iVox (its search records)
+  B2_FACTOR_ICP_PLANE_IVOX = 7,  // point-to-plane ICP on an iVoxCovarianceEstimation (its plane view)
+};
+
+// Turns on a covariance-estimating iVox's plane view and writes it from the map's current state.  Synchronous.
+b2_status ivox_enable_plane_view(const b2_ivox* iv);
 
 struct b2_factor {
   b2_ctx* ctx = nullptr;
   b2_factor_kind kind = B2_FACTOR_VGICP;
-  const b2_voxelmap* voxelmap = nullptr;  // VGICP: the target map; iVox GICP: the iVox's voxel-keyed map
+  const b2_voxelmap* voxelmap = nullptr;  // VGICP: the target map; iVox factors: the iVox's voxel-keyed map
   const b2_ivox* ivox = nullptr;
   const b2_cloud* target = nullptr;
   const b2_kdtree* tree = nullptr;
@@ -509,7 +526,7 @@ struct b2_factor {
   b2::DeviceBuffer d_target_records;  // double: kd-tree factors' target records in leaf order (Nt x 10)
   b2::DeviceBuffer d_lin_pose;        // 16 doubles: the linearization point, written by the linearize kernel's epilogue
   bool linearized = false;
-  uint64_t corr_gen = 0;  // iVox GICP: map generation the stored correspondences were associated against
+  uint64_t corr_gen = 0;  // iVox factors: map generation the stored correspondences were associated against
   double lin_delta[16] = {0};
   b2_factor_set* self_set = nullptr;  // lazily created set of size 1 for the single-factor entry points
 };

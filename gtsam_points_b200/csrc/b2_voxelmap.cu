@@ -721,12 +721,49 @@ __global__ void remove_old_invalid_kernel(size_t V, int slots, unsigned long lon
   keep[v] = out > 0 ? 1u : 0u;
 }
 
-// The valid view: the records with the point of every slot that is not valid at +inf.
-__global__ void valid_view_kernel(size_t P, const double* __restrict__ records, const unsigned long long* __restrict__ flags, double* __restrict__ view) {
+// The valid view: the records with the point of every slot that is not valid at +inf.  PLANE: also the plane view (b2_ivox::
+// d_plane_records), the same points with the slot's normal in 3..5, zeros in 6..8 and count 1.
+template <bool PLANE>
+__global__ void valid_view_kernel(size_t P, const double* __restrict__ records, const unsigned long long* __restrict__ flags, double* __restrict__ view,
+                                  const double* __restrict__ normals, double* __restrict__ plane) {
   const size_t p = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
   if (p >= P) return;
   const bool valid = flags[p] & kValidBit;
   for (int k = 0; k < kRecordDoubles; k++) view[p * kRecordDoubles + k] = (k < 3 && !valid) ? CUDART_INF : records[p * kRecordDoubles + k];
+  if (PLANE) {
+    for (int k = 0; k < kRecordDoubles; k++)
+      plane[p * kRecordDoubles + k] = k < 3 ? (valid ? records[p * kRecordDoubles + k] : CUDART_INF) : k < 6 ? normals[p * 3 + (k - 3)] : k < 9 ? 0.0 : 1.0;
+  }
+}
+
+// The valid view and, if the map has one, the plane view of the map's current point slots, (re)allocated to the map's capacity.
+// The generation is bumped when a view that factors may already read moves; the plane view's first allocation is read by none.
+b2_status write_views(const b2_ivox* iv_const) {
+  b2_ivox* iv = const_cast<b2_ivox*>(iv_const);  // only the views (caches of the state) change; see b2_ivox::plane_view
+  b2_voxelmap* vm = &iv->map;
+  cudaStream_t st = vm->ctx->stream;
+  const size_t Pv = vm->num_voxels * static_cast<size_t>(std::max(vm->slots, 0));
+  const size_t want = std::max<size_t>(vm->capacity * std::max(vm->slots, 1) * kRecordDoubles * sizeof(double), sizeof(double));
+  const bool valid_moves = iv->d_valid_records.bytes() != want;
+  const bool plane_moves = iv->plane_view && iv->d_plane_records.bytes() != want;
+  if (valid_moves || plane_moves) {
+    const bool plane_read = iv->d_plane_records.bytes() > 0;
+    B2_CUDA(cudaStreamSynchronize(st));
+    if (valid_moves) B2_TRY(iv->d_valid_records.alloc(want));
+    if (plane_moves) B2_TRY(iv->d_plane_records.alloc(want));
+    if (valid_moves || plane_read) vm->generation++;  // factor sets refresh their descriptors
+  }
+  if (Pv > 0) {
+    const unsigned grid = static_cast<unsigned>((Pv + 255) / 256);
+    if (iv->plane_view)
+      valid_view_kernel<true><<<grid, 256, 0, st>>>(Pv, vm->d_records.as<const double>(), vm->d_flags.as<const unsigned long long>(), iv->d_valid_records.as<double>(),
+                                                    vm->d_normals.as<const double>(), iv->d_plane_records.as<double>());
+    else
+      valid_view_kernel<false><<<grid, 256, 0, st>>>(Pv, vm->d_records.as<const double>(), vm->d_flags.as<const unsigned long long>(), iv->d_valid_records.as<double>(),
+                                                     nullptr, nullptr);
+    B2_CUDA(cudaGetLastError());
+  }
+  return B2_OK;
 }
 
 // Everything IncrementalCovarianceVoxelMap::insert does after the base insert (which insert_batch has run): birthdays, thresholds
@@ -793,18 +830,7 @@ b2_status cov_est_pass(b2_ivox* iv) {
     if (dropped) B2_TRY(rebuild_table(vm));
   }
 
-  const size_t Pv = vm->num_voxels * static_cast<size_t>(std::max(vm->slots, 0));
-  const size_t want = std::max<size_t>(vm->capacity * std::max(vm->slots, 1) * kRecordDoubles * sizeof(double), sizeof(double));
-  if (iv->d_valid_records.bytes() != want) {
-    B2_CUDA(cudaStreamSynchronize(st));
-    B2_TRY(iv->d_valid_records.alloc(want));
-    vm->generation++;  // the view moved: factor sets refresh their descriptors
-  }
-  if (Pv > 0) {
-    valid_view_kernel<<<static_cast<unsigned>((Pv + 255) / 256), 256, 0, st>>>(Pv, vm->d_records.as<const double>(), vm->d_flags.as<const unsigned long long>(),
-                                                                              iv->d_valid_records.as<double>());
-    B2_CUDA(cudaGetLastError());
-  }
+  B2_TRY(write_views(iv));
   B2_CUDA(cudaEventRecord(iv->phase_ev[4], st));
   B2_CUDA(cudaStreamSynchronize(st));
   return B2_OK;
@@ -867,6 +893,19 @@ b2_status ordered_stats(const double* stats, size_t P, double* part, cudaStream_
 }  // namespace b2
 
 using namespace b2;
+
+b2_status ivox_enable_plane_view(const b2_ivox* iv) {
+  if (iv->plane_view) return B2_OK;
+  B2_CUDA(cudaSetDevice(iv->map.ctx->device));
+  iv->plane_view = true;
+  const b2_status s = write_views(iv);
+  if (s != B2_OK) {
+    iv->plane_view = false;
+    return s;
+  }
+  B2_CUDA(cudaStreamSynchronize(iv->map.ctx->stream));
+  return B2_OK;
+}
 
 extern "C" {
 
@@ -1252,7 +1291,7 @@ b2_status b2_ivox_get_info(const b2_ivox* iv, b2_ivox_info* info) {
   info->num_voxels = vm->num_voxels;
   info->num_points = 0;
   info->resolution = vm->resolution;
-  info->device_bytes = vm->device_bytes();
+  info->device_bytes = vm->device_bytes() + iv->d_plane_records.bytes();
   if (vm->num_voxels > 0) {
     std::vector<uint32_t> cnt(vm->num_voxels);
     B2_CUDA(cudaSetDevice(vm->ctx->device));

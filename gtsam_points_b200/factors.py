@@ -229,10 +229,24 @@ class IntegratedICPFactor(IntegratedMatchingCostFactor):
     """IntegratedICPFactor(target_key, source_key, target, source[, target_tree][, use_point_to_plane]) or
     (fixed_target_pose, source_key, ...): include/gtsam_points/factors/integrated_icp_factor.hpp:27-145.  Point-to-plane
     needs target normals: those of the target PointCloud, which is then read on the device, or an `normals` attribute (n x 3) of
-    any other target object.  Neither cloud needs covariances."""
+    any other target object.  Neither cloud needs covariances.
+
+    `target` may also be an iVox, which is then target and search structure at once (IntegratedICPFactor_<iVox, PointCloud>,
+    src/gtsam_points/factors/integrated_icp_factor.cpp:9-10): correspondences are iVox indices voxel_id << 32 | point_id, and a
+    factor whose map changed since its last linearize re-associates.  Point-to-plane needs an iVoxCovarianceEstimation target,
+    whose valid points and estimated normals it uses; a plain iVox keeps no normals."""
 
     def __init__(self, a0, a1, target: PointCloud, source: PointCloud, target_tree: KdTree | None = None, use_point_to_plane: bool = False, ctx: Context | None = None):
         super().__init__(a0, a1)
+        if isinstance(target, iVox):
+            if source is None:
+                raise ValueError("error: source frame doesn't have required attributes for icp")
+            self.ctx = ctx or source.ctx
+            self.target, self.source, self.target_tree, self.use_point_to_plane = target, source, target, bool(use_point_to_plane)
+            h = C.c_void_p()
+            capi.check(capi.lib().b2_icp_ivox_factor_create(self.ctx.h, target.h, source.h, 1 if use_point_to_plane else 0, C.byref(h)))
+            self.h = h
+            return
         normals = getattr(target, "normals", None)
         if target is None or (use_point_to_plane and normals is None):
             raise ValueError("error: target frame doesn't have required attributes for icp")

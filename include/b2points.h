@@ -288,7 +288,7 @@ B2_API b2_status b2_ivox_knn(const b2_ivox* ivox, const double* queries, int que
  * ann/incremental_covariance_container.{hpp,cpp}): an iVox that estimates each stored point's covariance and normal from the
  * map's own neighbourhood as frames arrive, the map of frame-to-map odometry with no separate covariance step.  It is a b2_ivox:
  * b2_ivox_set_lru, _set_neighbor_voxel_mode, _set_insertion_setting, _clear, _insert, _insert_cloud, _get_info, _download, _knn
- * and b2_gicp_ivox_factor_create apply.  Input covariances are ignored.  Each stored point has a flags word (birthday = the
+ * b2_gicp_ivox_factor_create and b2_icp_ivox_factor_create apply.  Input covariances are ignored.  Each stored point has a flags word (birthday = the
  * lru_counter of its first estimation pass, bit 63 = VALID), a normal and a covariance, both zero until first estimated.
  *
  * One insert (incremental_covariance_voxelmap.cpp:69-196), in this order:
@@ -333,7 +333,8 @@ B2_API b2_status b2_ivox_knn_force(const b2_ivox* ivox, const double* queries, i
 B2_API b2_status b2_ivox_download_state(const b2_ivox* ivox, int32_t* coords, int32_t* counts, double* points, uint64_t* flags, double* normals, double* covs);
 /* Device time of the last insert's phases by CUDA events on the map's stream, in ms: ms[0] the base insert (segmentation, cells,
  * LRU sweep, table), ms[1] the estimation pass, ms[2] the statistics (reduction and its D2H), ms[3] the removal of old invalid
- * points and the valid view.  B2_ERR_INVALID_STATE before the first insert. */
+ * points and the valid view (with the plane view, once a point-to-plane factor has been created on the map).  B2_ERR_INVALID_STATE
+ * before the first insert. */
 B2_API b2_status b2_ivox_insert_timings(const b2_ivox* ivox, double* ms);
 /* The ring of eigenvalue statistics (eig_stats), oldest first: counts 10, sums 10 x 3, sums_sq 10 x 3. */
 B2_API b2_status b2_ivox_eig_stats(const b2_ivox* ivox, uint64_t* counts, double* sums, double* sums_sq);
@@ -840,6 +841,22 @@ B2_API b2_status b2_icp_factor_create(b2_ctx* ctx, const b2_cloud* target_cloud,
  * (insert, clear, neighbour mode) the factor's stored correspondences count as absent: the next linearize re-associates, an
  * error() before it associates at the evaluation pose. */
 B2_API b2_status b2_gicp_ivox_factor_create(b2_ctx* ctx, const b2_ivox* target, const b2_cloud* source, b2_factor** out);
+/* IntegratedICPFactor_<iVox, PointCloud> and IntegratedICPFactor_<iVoxCovarianceEstimation, PointCloud>
+ * (src/gtsam_points/factors/integrated_icp_factor.cpp:9-10, impl/integrated_icp_factor_impl.hpp:131-248): ICP with the iVox as target
+ * and search structure.  The search is b2_gicp_ivox_factor_create's (the iVox 1-NN in the map's neighbour voxel mode; on an
+ * iVoxCovarianceEstimation only valid points are found), the arithmetic b2_icp_factor_create's: r = mu_B - T p weighted with the
+ * identity, or, when use_point_to_plane != 0, with M = diag(n_x^2, n_y^2, n_z^2) for the target point's normal n.  Neither the map nor
+ * the source needs covariances.  Correspondences are voxel << 32 | slot; after the map changes they count as absent, as for
+ * b2_gicp_ivox_factor_create.
+ * Errors (B2_ERR_INVALID_ARGUMENT, before any device work): an empty map, or point-to-plane on a map without normals, "error: target
+ * frame doesn't have required attributes for icp"; a source without points, "error: source frame doesn't have required attributes
+ * for icp"; handles on different devices.
+ * Point-to-plane keeps a plane view in the map, built by the first such factor created on it and rewritten by every later insert
+ * (counted in b2_ivox_info::device_bytes and in the last phase of b2_ivox_insert_timings).
+ * Deliberate differences: (a) a plain iVox keeps no normals, so point-to-plane needs an iVoxCovarianceEstimation target; (b) the
+ * normals are those of the map's estimation pass, from the library's Jacobi solver and not oriented -- their sign does not matter,
+ * since M = diag(n^2). */
+B2_API b2_status b2_icp_ivox_factor_create(b2_ctx* ctx, const b2_ivox* target, const b2_cloud* source, int use_point_to_plane, b2_factor** out);
 B2_API b2_status b2_factor_destroy(b2_factor* f);
 /* IntegratedGICPFactor_::set_max_correspondence_distance (integrated_gicp_factor.hpp:98-101); default 1.0 */
 B2_API b2_status b2_factor_set_max_correspondence_distance(b2_factor* f, double dist);
@@ -847,7 +864,9 @@ B2_API b2_status b2_factor_set_max_correspondence_distance(b2_factor* f, double 
  * whose pose lies within (angle [rad], trans [m]) of the pose of the last correspondence update KEEPS those correspondences and
  * linearizes them at the new pose; otherwise it re-associates.  Default 0 / 0 = always re-associate.  Honoured by the entry
  * points that receive HOST poses (b2_factor_linearize, b2_factor_set_linearize, *_issue_linearize); the device-pose variants
- * cannot see the pose and always re-associate.  Set it before the factor joins a user-built set.  kd-tree factors only. */
+ * cannot see the pose and always re-associate.  Set it before the factor joins a user-built set.  Honoured by the GICP, ICP and
+ * point-to-plane ICP factors on kd-trees and on iVox targets (b2_gicp_factor_create, b2_icp_factor_create, b2_gicp_ivox_factor_create,
+ * b2_icp_ivox_factor_create); not by VGICP.  On an iVox target a map change re-associates regardless. */
 B2_API b2_status b2_factor_set_correspondence_update_tolerance(b2_factor* f, double angle, double trans);
 /* IntegratedVGICPFactorGPU::set_enable_surface_validation (include/gtsam_points/factors/integrated_vgicp_factor_gpu.hpp:88;
  * include/gtsam_points/cuda/kernels/lookup_voxels.cuh:42-50,86): when on, a source point whose normal n faces away from the

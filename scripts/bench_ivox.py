@@ -7,10 +7,12 @@ A synthetic scene (synthetic.make_cloud) is scanned along a trajectory, N points
   * linearize and error of an iVox GICP factor: kernel time by CUDA events on the context's stream, and end to end;
   * the alternative a kd-tree user has: rebuild a device kd-tree (and the GICP target cloud) over the same map points,
     then linearize -- end to end, and its linearize kernel;
-  * the oracle's kd-tree GICP over the same map points on the host cores (tree build + linearize).
+  * the oracle's kd-tree GICP over the same map points on the host cores (tree build + linearize);
+  * with --factor icp, also linearize and error of a point-to-point ICP factor on the same map and frame (icp_* keys), next to
+    GICP in the same run.
 Medians over the timed frames; map size at the end.  Prints the card name, power limit and max SM clock of the same run.
 
-  python scripts/bench_ivox.py [--frames 12] [--sizes 20000 120000]
+  python scripts/bench_ivox.py [--frames 12] [--sizes 20000 120000] [--factor gicp|icp]
 """
 import argparse
 import ctypes as C
@@ -62,12 +64,24 @@ def wall_ms(fn):
     return (time.perf_counter() - t) * 1e3
 
 
-def run(n, count, threads):
+def factor_times(stream, fac, delta, d_out):
+    """(linearize kernel, linearize end to end, error kernel, error end to end) in ms; the factor has been linearized once."""
+    lin_k = kernel_ms(stream, lambda: capi.check(capi.lib().b2_factor_issue_linearize(fac.h, capi.dptr(delta), C.c_void_p(d_out.data_ptr()))))
+    lin_e = wall_ms(lambda: fac.linearize({1: delta}))
+    err_k = kernel_ms(stream, lambda: capi.check(capi.lib().b2_factor_issue_error(fac.h, capi.dptr(delta), C.c_void_p(d_out.data_ptr()))))
+    err_e = wall_ms(lambda: fac.error({1: delta}))
+    return lin_k, lin_e, err_k, err_e
+
+
+def run(n, count, threads, factor="gicp"):
     stream = torch.cuda.current_stream()
     ctx = g.Context(0, stream.cuda_stream)
     ivox = g.iVox(1.0, ctx=ctx)
     d_out = torch.zeros(capi.B2_LINEARIZED_DOUBLES, dtype=torch.float64, device="cuda")
     rec = {k: [] for k in ("insert_ms", "lin_kernel_ms", "lin_e2e_ms", "err_kernel_ms", "err_e2e_ms", "kd_rebuild_lin_e2e_ms", "kd_lin_kernel_ms", "host_oracle_ms")}
+    icp_keys = ("icp_lin_kernel_ms", "icp_lin_e2e_ms", "icp_err_kernel_ms", "icp_err_e2e_ms")
+    if factor == "icp":
+        rec.update({k: [] for k in icp_keys})
     fr = frames(n, count)
     for f, (p, c, T) in enumerate(fr):
         R, t = T[:3, :3], T[:3, 3]
@@ -79,10 +93,11 @@ def run(n, count, threads):
             delta = np.ascontiguousarray(T @ syn.random_pose(np.random.default_rng(f), 0.01, 0.1))
             fac = g.IntegratedGICPFactor(np.eye(4), 1, ivox, src, ctx=ctx)
             fac.linearize({1: delta})  # first call builds the factor's launch set
-            lin_k = kernel_ms(stream, lambda: capi.check(capi.lib().b2_factor_issue_linearize(fac.h, capi.dptr(delta), C.c_void_p(d_out.data_ptr()))))
-            lin_e = wall_ms(lambda: fac.linearize({1: delta}))
-            err_k = kernel_ms(stream, lambda: capi.check(capi.lib().b2_factor_issue_error(fac.h, capi.dptr(delta), C.c_void_p(d_out.data_ptr()))))
-            err_e = wall_ms(lambda: fac.error({1: delta}))
+            lin_k, lin_e, err_k, err_e = factor_times(stream, fac, delta, d_out)
+            if factor == "icp":
+                ifac = g.IntegratedICPFactor(np.eye(4), 1, ivox, g.PointCloud(p, ctx=ctx), ctx=ctx)
+                ifac.linearize({1: delta})
+                icp = factor_times(stream, ifac, delta, d_out)
             m = ivox.download()
             mp, mc = m["points"], m["covs"]
 
@@ -109,6 +124,9 @@ def run(n, count, threads):
                 rec["err_e2e_ms"].append(err_e)
                 rec["kd_rebuild_lin_e2e_ms"].append(kd_e)
                 rec["kd_lin_kernel_ms"].append(kd_k)
+                if factor == "icp":
+                    for k, v in zip(icp_keys, icp):
+                        rec[k].append(v)
                 if host_ms is not None:
                     rec["host_oracle_ms"].append(host_ms)
         ins = wall_ms(lambda: ivox.insert(world_p, world_c))
@@ -124,11 +142,12 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=12)
     ap.add_argument("--sizes", type=int, nargs="+", default=[20000, 120000])
+    ap.add_argument("--factor", choices=("gicp", "icp"), default="gicp", help="icp: also time point-to-point ICP on the map, next to GICP")
     a = ap.parse_args()
     threads = max(1, min(os.cpu_count() or 1, orc.max_threads()))
     print(json.dumps({"card": card()}))
     for n in a.sizes:
-        print(json.dumps(run(n, a.frames, threads)))
+        print(json.dumps(run(n, a.frames, threads, a.factor)))
 
 
 if __name__ == "__main__":

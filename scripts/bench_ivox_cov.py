@@ -6,10 +6,13 @@ KITTI-07 submaps of tests/golden.  Per frame it reports medians of:
   * insert, end to end, and its device phases by CUDA events (b2_ivox_insert_timings): base insert, estimation pass,
     statistics, removal of old invalid points with the valid view;
   * linearize and error of a GICP factor on the map: kernel time by CUDA events on the context's stream, and end to end;
-  * the host restatement (tests/ivox_cov_np.py) doing the same insert (numpy, one process; KITTI and the 20k loop only by default).
+  * the host restatement (tests/ivox_cov_np.py) doing the same insert (numpy, one process; KITTI and the 20k loop only by default);
+  * with --factor icp or plane, also linearize and error of a point-to-point or point-to-plane ICP factor on the same map and
+    frame (icp_* / plane_* keys), next to GICP in the same run.  A point-to-plane factor turns on the map's plane view, which
+    every later insert rewrites in its last phase (removal_ms): the insert columns then include it.
 Prints the card name, power limit and max SM clock of the same run.
 
-  python scripts/bench_ivox_cov.py [--frames 12] [--sizes 20000 120000] [--host-max 20000]
+  python scripts/bench_ivox_cov.py [--frames 12] [--sizes 20000 120000] [--host-max 20000] [--factor gicp|icp|plane]
 """
 import argparse
 import ctypes as C
@@ -71,14 +74,24 @@ def wall_ms(fn):
     return (time.perf_counter() - t) * 1e3
 
 
-def run(name, fr, host):
+def factor_times(stream, fac, delta, d_out):
+    """(linearize kernel, linearize end to end, error kernel, error end to end) in ms; the factor has been linearized once."""
+    lin_k = kernel_ms(stream, lambda: capi.check(capi.lib().b2_factor_issue_linearize(fac.h, capi.dptr(delta), C.c_void_p(d_out.data_ptr()))))
+    lin_e = wall_ms(lambda: fac.linearize({1: delta}))
+    err_k = kernel_ms(stream, lambda: capi.check(capi.lib().b2_factor_issue_error(fac.h, capi.dptr(delta), C.c_void_p(d_out.data_ptr()))))
+    err_e = wall_ms(lambda: fac.error({1: delta}))
+    return lin_k, lin_e, err_k, err_e
+
+
+def run(name, fr, host, factor="gicp"):
     stream = torch.cuda.current_stream()
     ctx = g.Context(0, stream.cuda_stream)
     m = g.iVoxCovarianceEstimation(1.0, ctx=ctx)
     ref = ivox_cov_np.IvoxCovNp(1.0) if host else None
     d_out = torch.zeros(capi.B2_LINEARIZED_DOUBLES, dtype=torch.float64, device="cuda")
     keys = ("insert_e2e_ms", "base_insert_ms", "estimation_ms", "statistics_ms", "removal_ms", "lin_kernel_ms", "lin_e2e_ms", "err_kernel_ms", "err_e2e_ms", "host_insert_ms")
-    rec = {k: [] for k in keys}
+    extra = tuple(f"{factor}_{k}" for k in ("lin_kernel_ms", "lin_e2e_ms", "err_kernel_ms", "err_e2e_ms")) if factor != "gicp" else ()
+    rec = {k: [] for k in keys + extra}
     warm = 1 if len(fr) <= 5 else 2
     for f, (p, c, T) in enumerate(fr):
         R, t = T[:3, :3], T[:3, 3]
@@ -88,15 +101,18 @@ def run(name, fr, host):
             delta = np.ascontiguousarray(T @ syn.random_pose(np.random.default_rng(f), 0.01, 0.1))
             fac = g.IntegratedGICPFactor(np.eye(4), 1, m, src, ctx=ctx)
             fac.linearize({1: delta})
-            lin_k = kernel_ms(stream, lambda: capi.check(capi.lib().b2_factor_issue_linearize(fac.h, capi.dptr(delta), C.c_void_p(d_out.data_ptr()))))
-            lin_e = wall_ms(lambda: fac.linearize({1: delta}))
-            err_k = kernel_ms(stream, lambda: capi.check(capi.lib().b2_factor_issue_error(fac.h, capi.dptr(delta), C.c_void_p(d_out.data_ptr()))))
-            err_e = wall_ms(lambda: fac.error({1: delta}))
+            lin_k, lin_e, err_k, err_e = factor_times(stream, fac, delta, d_out)
+            if extra:
+                ifac = g.IntegratedICPFactor(np.eye(4), 1, m, g.PointCloud(p, ctx=ctx), use_point_to_plane=factor == "plane", ctx=ctx)
+                ifac.linearize({1: delta})
+                times = factor_times(stream, ifac, delta, d_out)
             if f >= warm:
                 rec["lin_kernel_ms"].append(lin_k)
                 rec["lin_e2e_ms"].append(lin_e)
                 rec["err_kernel_ms"].append(err_k)
                 rec["err_e2e_ms"].append(err_e)
+                for k, v in zip(extra, times if extra else ()):
+                    rec[k].append(v)
         e2e = wall_ms(lambda: m.insert(world))
         ph = m.insert_timings()
         h = wall_ms(lambda: ref.insert(world)) if ref is not None else None
@@ -119,11 +135,12 @@ def main():
     ap.add_argument("--frames", type=int, default=12)
     ap.add_argument("--sizes", type=int, nargs="+", default=[20000, 120000])
     ap.add_argument("--host-max", type=int, default=20000, help="largest synthetic frame size the host restatement also runs")
+    ap.add_argument("--factor", choices=("gicp", "icp", "plane"), default="gicp", help="icp / plane: also time that ICP factor on the map, next to GICP")
     a = ap.parse_args()
     print(json.dumps({"card": card()}))
     for n in a.sizes:
-        print(json.dumps(run(f"synthetic {n} pts/frame", synthetic_frames(n, a.frames), n <= a.host_max)))
-    print(json.dumps(run("KITTI-07 submaps", kitti_frames(), True)))
+        print(json.dumps(run(f"synthetic {n} pts/frame", synthetic_frames(n, a.frames), n <= a.host_max, a.factor)))
+    print(json.dumps(run("KITTI-07 submaps", kitti_frames(), True, a.factor)))
 
 
 if __name__ == "__main__":

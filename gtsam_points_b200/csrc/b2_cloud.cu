@@ -330,7 +330,6 @@ b2_status merge_frames_check(b2_ctx* ctx, const double* poses, const b2_cloud* c
 // frame's coordinates for the keys, into the world for the sums.  Synchronises the context's stream.
 b2_status merge_frames_device(b2_ctx* ctx, const double* poses, const b2_cloud* const* frames, size_t num_frames, double downsample_resolution, size_t total,
                               bool have_covs, DeviceBuffer& d_xyz, DeviceBuffer& d_cov, size_t* out_n) {
-  B2_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
 
   // first_pose^-1 (rigid inverse) and the relative poses, with the CPU function's operation order
@@ -390,7 +389,6 @@ std::atomic<uint64_t> g_next_cloud_uid{1};
 namespace b2 {
 
 b2_status assemble_cloud(b2_ctx* ctx, const RawCloud& raw, unsigned flags, const b2_cloud* like, b2_cloud** out, const char* who) {
-  B2_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   const size_t n = like ? like->n : raw.n;
 
@@ -579,7 +577,7 @@ b2_status b2_cloud_create_with_normals(b2_ctx* ctx, const double* points, int po
   B2_REQUIRE(point_stride == 3 || point_stride == 4, "b2_cloud_create: point_stride must be 3 or 4 (got %d)", point_stride);
   B2_REQUIRE(covs == nullptr || cov_stride == 9 || cov_stride == 16, "b2_cloud_create: cov_stride must be 9 or 16 (got %d)", cov_stride);
   B2_REQUIRE(n < (1ull << 31), "b2_cloud_create: at most 2^31-1 points per cloud");
-  B2_CUDA(cudaSetDevice(ctx->device));
+  B2_ON_DEVICE(ctx);
   cudaStream_t st = ctx->stream;
 
   // H2D staging of the host arrays; assemble_cloud does the rest on the device
@@ -611,7 +609,7 @@ b2_status b2_cloud_create_voxelgrid(b2_ctx* ctx, double resolution, const double
   B2_REQUIRE(covs == nullptr || cov_stride == 9 || cov_stride == 16, "b2_cloud_create_voxelgrid: cov_stride must be 9 or 16 (got %d)", cov_stride);
   B2_REQUIRE(normals == nullptr || normal_stride == 3 || normal_stride == 4, "b2_cloud_create_voxelgrid: normal_stride must be 3 or 4 (got %d)", normal_stride);
   B2_REQUIRE(n < (1ull << 31), "b2_cloud_create_voxelgrid: at most 2^31-1 points per call");
-  B2_CUDA(cudaSetDevice(ctx->device));
+  B2_ON_DEVICE(ctx);
   cudaStream_t st = ctx->stream;
 
   // the averaged arrays (one entry per voxel, ascending key order).  For an empty result the caller's pointers stay in their place:
@@ -652,7 +650,7 @@ b2_status b2_cloud_create_transformed(const b2_cloud* cloud, const double* T, un
   *out = nullptr;
   B2_REQUIRE(cloud != nullptr, "b2_cloud_create_transformed: cloud is NULL");
   B2_TRY(check_pose(T, "b2_cloud_create_transformed"));
-  B2_CUDA(cudaSetDevice(cloud->ctx->device));
+  B2_ON_DEVICE(cloud->ctx);
   const size_t n = cloud->n, rows = std::max<size_t>(n, 1);  // n == 0: the buffers only mark which arrays the cloud has
   DeviceBuffer d_p, d_c, d_n;
   B2_TRY(d_p.alloc(rows * 3 * sizeof(double)));
@@ -676,6 +674,7 @@ b2_status b2_merge_frames(b2_ctx* ctx, const double* poses, const b2_cloud* cons
   *out_n = 0;
   if (total == 0) return B2_OK;
   B2_REQUIRE(out_points != nullptr && (out_covs != nullptr || !have_covs), "b2_merge_frames: output arrays are NULL");
+  B2_ON_DEVICE(ctx);
   DeviceBuffer d_xyz, d_cov;
   size_t m = 0;
   B2_TRY(merge_frames_device(ctx, poses, frames, num_frames, downsample_resolution, total, have_covs, d_xyz, d_cov, &m));
@@ -697,7 +696,7 @@ b2_status b2_merge_frames_to_cloud(b2_ctx* ctx, const double* poses, const b2_cl
   size_t total = 0;
   bool have_covs = true;
   B2_TRY(merge_frames_check(ctx, poses, frames, num_frames, downsample_resolution, "b2_merge_frames_to_cloud", &total, &have_covs));
-  B2_CUDA(cudaSetDevice(ctx->device));
+  B2_ON_DEVICE(ctx);
   DeviceBuffer d_xyz, d_cov;
   size_t m = 0;
   if (total > 0) B2_TRY(merge_frames_device(ctx, poses, frames, num_frames, downsample_resolution, total, have_covs, d_xyz, d_cov, &m));
@@ -711,7 +710,7 @@ b2_status b2_merge_frames_to_cloud(b2_ctx* ctx, const double* poses, const b2_cl
 
 b2_status b2_cloud_destroy(b2_cloud* c) {
   if (!c) return B2_OK;
-  cudaSetDevice(c->ctx->device);
+  const b2::DeviceScope on_device(c->ctx->device);
   delete c;
   return B2_OK;
 }
@@ -732,7 +731,7 @@ b2_status b2_cloud_download(const b2_cloud* c, double* out_points, double* out_c
   if (out_covs && !c->d_covs) return fail(B2_ERR_INVALID_STATE, "b2_cloud_download: the cloud has no covariances");
   if (out_normals && !c->d_normals) return fail(B2_ERR_INVALID_STATE, "b2_cloud_download: the cloud has no normals");
   if (c->n == 0) return B2_OK;
-  B2_CUDA(cudaSetDevice(c->ctx->device));
+  B2_ON_DEVICE(c->ctx);
   cudaStream_t st = c->ctx->stream;
   // one launch writes every array asked for into one device buffer: points | covs | normals
   const size_t np = out_points ? 3 * c->n : 0, nc = out_covs ? 9 * c->n : 0, nn = out_normals ? 3 * c->n : 0;

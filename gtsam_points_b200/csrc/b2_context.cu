@@ -7,19 +7,59 @@ namespace b2 {
 
 static thread_local char g_last_error[1024] = "";
 
-void set_error(const char* fmt, ...) {
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(g_last_error, sizeof(g_last_error), fmt, ap);
-  va_end(ap);
-}
-
 b2_status fail(b2_status st, const char* fmt, ...) {
   va_list ap;
   va_start(ap, fmt);
   vsnprintf(g_last_error, sizeof(g_last_error), fmt, ap);
   va_end(ap);
   return st;
+}
+
+namespace {
+// cuCtxGetCurrent and cuCtxSetCurrent, looked up once through the runtime: the library does not link libcuda, so it still loads on
+// a machine without a driver, where b2_ctx_create reports B2_ERR_NO_DEVICE before any scope is opened.  NULL if the lookup failed.
+struct CtxCalls {
+  CUresult (*get)(CUcontext*) = nullptr;
+  CUresult (*set)(CUcontext) = nullptr;
+};
+const CtxCalls* ctx_calls() {
+  static const CtxCalls calls = [] {
+    CtxCalls c;
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult found;
+    if (cudaGetDriverEntryPoint("cuCtxGetCurrent", &fn, cudaEnableDefault, &found) == cudaSuccess && found == cudaDriverEntryPointSuccess)
+      c.get = reinterpret_cast<CUresult (*)(CUcontext*)>(fn);
+    if (cudaGetDriverEntryPoint("cuCtxSetCurrent", &fn, cudaEnableDefault, &found) == cudaSuccess && found == cudaDriverEntryPointSuccess)
+      c.set = reinterpret_cast<CUresult (*)(CUcontext)>(fn);
+    return c;
+  }();
+  return calls.get && calls.set ? &calls : nullptr;
+}
+}  // namespace
+
+DeviceScope::DeviceScope(int device) {
+  const CtxCalls* calls = ctx_calls();
+  if (!calls) {
+    status_ = fail(B2_ERR_CUDA, "cudaGetDriverEntryPoint: cuCtxGetCurrent / cuCtxSetCurrent not found");
+    return;
+  }
+  const CUresult r = calls->get(&saved_);
+  if (r != CUDA_SUCCESS) {
+    status_ = fail(B2_ERR_CUDA, "cuCtxGetCurrent -> CUresult %d", static_cast<int>(r));
+    return;
+  }
+  restore_ = true;
+  const cudaError_t e = cudaSetDevice(device);
+  if (e != cudaSuccess) {
+    status_ = fail(e == cudaErrorMemoryAllocation ? B2_ERR_OUT_OF_MEMORY : B2_ERR_CUDA, "cudaSetDevice(%d) -> %s", device, cudaGetErrorString(e));
+    return;
+  }
+  CUcontext now = nullptr;
+  restore_ = calls->get(&now) != CUDA_SUCCESS || now != saved_;  // the common case: the device was current already
+}
+
+DeviceScope::~DeviceScope() {
+  if (restore_) ctx_calls()->set(saved_);
 }
 
 }  // namespace b2
@@ -55,7 +95,8 @@ b2_status b2_ctx_create(int device, void* stream, b2_ctx** out) {
     return b2::fail(B2_ERR_NO_DEVICE, "b2_ctx_create: no CUDA device available (%s)", e != cudaSuccess ? cudaGetErrorString(e) : "count = 0");
   }
   B2_REQUIRE(device >= 0 && device < count, "b2_ctx_create: device %d out of range [0, %d)", device, count);
-  B2_CUDA(cudaSetDevice(device));
+  const b2::DeviceScope on_device(device);
+  B2_TRY(on_device.status());
   b2_ctx* ctx = new b2_ctx;
   ctx->device = device;
   if (stream) {
@@ -101,7 +142,7 @@ b2_status b2_ctx_create(int device, void* stream, b2_ctx** out) {
 
 b2_status b2_ctx_destroy(b2_ctx* ctx) {
   if (!ctx) return B2_OK;
-  cudaSetDevice(ctx->device);
+  const b2::DeviceScope on_device(ctx->device);
   cudaStreamSynchronize(ctx->stream);
   if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
   if (ctx->h_done) cudaFreeHost(const_cast<unsigned int*>(ctx->h_done));
@@ -113,6 +154,7 @@ b2_status b2_ctx_destroy(b2_ctx* ctx) {
 
 b2_status b2_ctx_synchronize(b2_ctx* ctx) {
   B2_REQUIRE(ctx != nullptr, "b2_ctx_synchronize: ctx is NULL");
+  B2_ON_DEVICE(ctx);  // a runtime call on a thread without a current context would make device 0's primary context current
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
   return B2_OK;
 }
@@ -122,7 +164,7 @@ void* b2_ctx_stream(b2_ctx* ctx) { return ctx ? static_cast<void*>(ctx->stream) 
 b2_status b2_device_malloc(b2_ctx* ctx, size_t bytes, void** out) {
   B2_REQUIRE(ctx && out, "b2_device_malloc: NULL argument");
   *out = nullptr;
-  B2_CUDA(cudaSetDevice(ctx->device));
+  B2_ON_DEVICE(ctx);
   B2_CUDA(cudaMalloc(out, bytes ? bytes : 1));
   return B2_OK;
 }
@@ -130,7 +172,7 @@ b2_status b2_device_malloc(b2_ctx* ctx, size_t bytes, void** out) {
 b2_status b2_device_free(b2_ctx* ctx, void* ptr) {
   B2_REQUIRE(ctx != nullptr, "b2_device_free: ctx is NULL");
   if (!ptr) return B2_OK;
-  B2_CUDA(cudaSetDevice(ctx->device));
+  B2_ON_DEVICE(ctx);
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
   B2_CUDA(cudaFree(ptr));
   return B2_OK;
@@ -138,7 +180,7 @@ b2_status b2_device_free(b2_ctx* ctx, void* ptr) {
 
 b2_status b2_memcpy_d2h(b2_ctx* ctx, void* dst, const void* src, size_t bytes) {
   B2_REQUIRE(ctx && (bytes == 0 || (dst && src)), "b2_memcpy_d2h: NULL argument");
-  B2_CUDA(cudaSetDevice(ctx->device));
+  B2_ON_DEVICE(ctx);
   B2_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, ctx->stream));
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
   return B2_OK;
@@ -146,7 +188,7 @@ b2_status b2_memcpy_d2h(b2_ctx* ctx, void* dst, const void* src, size_t bytes) {
 
 b2_status b2_memcpy_h2d(b2_ctx* ctx, void* dst, const void* src, size_t bytes) {
   B2_REQUIRE(ctx && (bytes == 0 || (dst && src)), "b2_memcpy_h2d: NULL argument");
-  B2_CUDA(cudaSetDevice(ctx->device));
+  B2_ON_DEVICE(ctx);
   B2_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, ctx->stream));
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
   return B2_OK;

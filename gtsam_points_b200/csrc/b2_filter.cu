@@ -175,7 +175,7 @@ b2_status b2_cloud_create_sampled(const b2_cloud* cloud, const int64_t* indices,
     B2_REQUIRE(indices[r] >= 0 && static_cast<uint64_t>(indices[r]) < n, "%s: indices[%zu] = %lld is outside [0, %zu)", who, r, static_cast<long long>(indices[r]), n);
     K[r] = static_cast<uint32_t>(indices[r]);
   }
-  B2_CUDA(cudaSetDevice(cloud->ctx->device));
+  B2_ON_DEVICE(cloud->ctx);
   cudaStream_t st = cloud->ctx->stream;
   if (num_indices == 0) return assemble_selection(cloud, nullptr, nullptr, 0, flags, nullptr, out, who);
   Rows rows;
@@ -191,7 +191,7 @@ b2_status b2_cloud_create_random_sampled(const b2_cloud* cloud, double sampling_
   *out = nullptr;
   B2_REQUIRE(cloud != nullptr, "%s: cloud is NULL", who);
   B2_TRY(check_rate(sampling_rate, who));
-  B2_CUDA(cudaSetDevice(cloud->ctx->device));
+  B2_ON_DEVICE(cloud->ctx);
   cudaStream_t st = cloud->ctx->stream;
   const size_t n = cloud->n;
   if (n == 0) return assemble_selection(cloud, nullptr, nullptr, 0, flags, out_indices, out, who);
@@ -213,7 +213,7 @@ b2_status b2_cloud_create_randomgrid(const b2_cloud* cloud, double resolution, d
   B2_REQUIRE(cloud != nullptr, "%s: cloud is NULL", who);
   B2_REQUIRE(resolution > 0.0 && std::isfinite(resolution), "%s: resolution must be positive and finite (got %g)", who, resolution);
   B2_TRY(check_rate(sampling_rate, who));
-  B2_CUDA(cudaSetDevice(cloud->ctx->device));
+  B2_ON_DEVICE(cloud->ctx);
   cudaStream_t st = cloud->ctx->stream;
   const size_t n = cloud->n;
   if (n == 0) return assemble_selection(cloud, nullptr, nullptr, 0, flags, out_indices, out, who);
@@ -277,7 +277,7 @@ b2_status b2_cloud_create_inliers(const b2_cloud* cloud, const b2_kdtree* tree, 
   B2_REQUIRE(tree == nullptr || tree->cloud_uid == cloud->uid, "%s: the tree was not built by b2_kdtree_create_from_cloud from this cloud", who);
   const size_t n = cloud->n;
   B2_REQUIRE(n == 0 || n >= static_cast<size_t>(k), "%s: the cloud has %zu points, fewer than k = %d", who, n, k);
-  B2_CUDA(cudaSetDevice(cloud->ctx->device));
+  B2_ON_DEVICE(cloud->ctx);
   cudaStream_t st = cloud->ctx->stream;
   if (n == 0) {
     if (out_thresh) *out_thresh = std::numeric_limits<double>::quiet_NaN();  // mean = 0 / 0

@@ -2,6 +2,7 @@
 // Nothing here crosses the library boundary.
 #pragma once
 
+#include <cuda.h>  // CUcontext only: the driver is reached through cudaGetDriverEntryPoint, not linked
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -20,7 +21,6 @@
 namespace b2 {
 
 // ---- error plumbing -------------------------------------------------------------------------
-void set_error(const char* fmt, ...);
 b2_status fail(b2_status st, const char* fmt, ...);
 
 #define B2_CUDA(expr)                                                                                          \
@@ -43,10 +43,41 @@ b2_status fail(b2_status st, const char* fmt, ...);
     if (_s != B2_OK) return _s;    \
   } while (0)
 
+// ---- device selection -----------------------------------------------------------------------------
+// Every C ABI function that touches a device opens a DeviceScope on its handle's device (B2_ON_DEVICE), and nothing else selects
+// a device: every other function runs in its caller's scope.  The scope comes after the checks the call makes without CUDA, so a
+// NULL handle or a bad argument fails before any CUDA call, and before any local that owns device memory, so such a local is
+// freed while its device is current.  A body that several entry points share (ivox_knn, estimate_covs_normals, create_features,
+// exchange_step) makes their checks and then opens the scope for them.  The *_destroy functions open it too, and free whatever its
+// status.
+//
+// The scope records the CUDA context current on the calling thread (NULL if none), makes the device's primary context current,
+// and on exit makes the recorded one current again if it changed.  So the caller's current device (PyTorch's, for one) is the
+// same after a call as before it, and a thread that had no context has none again: restoring "device 0" would create a context on
+// GPU 0 in a process that only uses GPU 1.  Status: B2_OK, or B2_CUDA's status when the device cannot be made current.
+class DeviceScope {
+ public:
+  explicit DeviceScope(int device);
+  ~DeviceScope();
+  DeviceScope(const DeviceScope&) = delete;
+  DeviceScope& operator=(const DeviceScope&) = delete;
+  b2_status status() const { return status_; }
+
+ private:
+  CUcontext saved_ = nullptr;
+  bool restore_ = false;
+  b2_status status_ = B2_OK;
+};
+
+// Opens the scope on ctx's device for the rest of the enclosing block; returns from the function if that fails.
+#define B2_ON_DEVICE(ctx)                                  \
+  const ::b2::DeviceScope b2_device_scope((ctx)->device); \
+  B2_TRY(b2_device_scope.status())
+
 // ---- device memory --------------------------------------------------------------------------------
 // One cudaMalloc allocation and its size in bytes.  Move-only: a move hands the allocation over, a copy does not compile.
-// The destructor frees without selecting a device.  That is safe because a handle is destroyed, and a scratch buffer goes out
-// of scope, while its device is current: every *_destroy calls cudaSetDevice first, every other entry point before it allocates.
+// The destructor frees without selecting a device: under the rule of DeviceScope above, a buffer is freed while its device is
+// current.
 class DeviceBuffer {
  public:
   DeviceBuffer() = default;

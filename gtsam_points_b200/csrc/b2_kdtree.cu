@@ -492,7 +492,7 @@ b2_status b2_kdtree_create(b2_ctx* ctx, const double* points, int point_stride, 
   B2_REQUIRE(points != nullptr || n == 0, "b2_kdtree_create: points is NULL");
   B2_REQUIRE(point_stride == 3 || point_stride == 4, "b2_kdtree_create: point_stride must be 3 or 4");
   B2_REQUIRE(n < (1ull << 31), "b2_kdtree_create: at most 2^31-1 points");
-  B2_CUDA(cudaSetDevice(ctx->device));
+  B2_ON_DEVICE(ctx);
   DeviceBuffer d_pts;
   if (n > 0) B2_TRY(d_pts.upload(points, n * point_stride * sizeof(double), ctx->stream));
   return build_tree(ctx, d_pts.as<const double>(), point_stride, n, out);
@@ -503,7 +503,7 @@ b2_status b2_kdtree_create_from_cloud(const b2_cloud* cloud, b2_kdtree** out) {
   *out = nullptr;
   B2_REQUIRE(cloud != nullptr, "b2_kdtree_create_from_cloud: cloud is NULL");
   b2_ctx* ctx = cloud->ctx;
-  B2_CUDA(cudaSetDevice(ctx->device));
+  B2_ON_DEVICE(ctx);
   DeviceBuffer d_pts;
   if (cloud->n > 0) {
     // the stored points in caller order: what b2_kdtree_create over b2_cloud_download's points would upload
@@ -517,7 +517,7 @@ b2_status b2_kdtree_create_from_cloud(const b2_cloud* cloud, b2_kdtree** out) {
 
 b2_status b2_kdtree_destroy(b2_kdtree* t) {
   if (!t) return B2_OK;
-  cudaSetDevice(t->ctx->device);
+  const b2::DeviceScope on_device(t->ctx->device);
   delete t;
   return B2_OK;
 }
@@ -528,7 +528,7 @@ b2_status b2_kdtree_knn1(const b2_kdtree* t, const double* queries, int query_st
   B2_REQUIRE(query_stride == 3 || query_stride == 4, "b2_kdtree_knn1: query_stride must be 3 or 4");
   B2_REQUIRE(max_sq_dist >= 0.0, "b2_kdtree_knn1: max_sq_dist must be >= 0");
   if (nq == 0) return B2_OK;
-  B2_CUDA(cudaSetDevice(t->ctx->device));
+  B2_ON_DEVICE(t->ctx);
   cudaStream_t st = t->ctx->stream;
   DeviceBuffer dq, di, ds;
   B2_TRY(dq.upload(queries, nq * query_stride * sizeof(double), st));
@@ -551,7 +551,7 @@ b2_status b2_kdtree_knn(const b2_kdtree* t, const double* queries, int query_str
   B2_REQUIRE(max_sq_dist >= 0.0, "b2_kdtree_knn: max_sq_dist must be >= 0");
   if (nq == 0) return B2_OK;
   if (k == 1) return b2_kdtree_knn1(t, queries, query_stride, nq, max_sq_dist, out_index, out_sq_dist);
-  B2_CUDA(cudaSetDevice(t->ctx->device));
+  B2_ON_DEVICE(t->ctx);
   cudaStream_t st = t->ctx->stream;
   DeviceBuffer dq, di, ds;
   B2_TRY(dq.upload(queries, nq * query_stride * sizeof(double), st));
@@ -656,7 +656,7 @@ b2_status b2_kdtree_radius_search(const b2_kdtree* t, const double* queries, int
   B2_REQUIRE(nq < (1ull << 31), "b2_kdtree_radius_search: at most 2^31-1 queries per call");
   std::fill(out_offsets, out_offsets + nq + 1, uint64_t{0});
   if (nq == 0 || t->n == 0 || max_num_neighbors == 0) return B2_OK;
-  B2_CUDA(cudaSetDevice(t->ctx->device));
+  B2_ON_DEVICE(t->ctx);
   cudaStream_t st = t->ctx->stream;
   const double r2 = radius * radius;
   DeviceBuffer dq, d_raw, d_kept, dout_idx, dout_sq;
@@ -706,7 +706,7 @@ b2_status estimate_covs_normals(const b2_kdtree* t, int k_neighbors, const doubl
   B2_REQUIRE(k_neighbors >= 1 && k_neighbors <= B2_KNN_MAX_K, "%s: k_neighbors must be in [1, %d]", fn, B2_KNN_MAX_K);
   const size_t n = t->n;
   if (n == 0) return B2_OK;
-  B2_CUDA(cudaSetDevice(t->ctx->device));
+  B2_ON_DEVICE(t->ctx);
   cudaStream_t st = t->ctx->stream;
   DeviceBuffer dc, dn;
   B2_TRY(dc.alloc(n * 9 * sizeof(double)));
@@ -727,7 +727,7 @@ b2_status b2_cloud_create_estimated(const b2_cloud* cloud, const b2_kdtree* tree
   B2_REQUIRE(k_neighbors >= 1 && k_neighbors <= B2_KNN_MAX_K, "b2_cloud_create_estimated: k_neighbors must be in [1, %d]", B2_KNN_MAX_K);
   B2_REQUIRE(!(flags & B2_CLOUD_NO_REORDER), "b2_cloud_create_estimated: B2_CLOUD_NO_REORDER does not apply (the points keep the input cloud's order)");
   B2_REQUIRE(tree == nullptr || tree->cloud_uid == cloud->uid, "b2_cloud_create_estimated: the tree was not built by b2_kdtree_create_from_cloud from this cloud");
-  B2_CUDA(cudaSetDevice(cloud->ctx->device));
+  B2_ON_DEVICE(cloud->ctx);
   const size_t n = cloud->n;
   b2_kdtree* own = nullptr;  // covariance_estimation.cpp:19: a tree of its own when none is given
   if (!tree) {
@@ -770,7 +770,7 @@ b2_status b2_estimate_normals_from_covs(b2_ctx* ctx, const double* points, int p
   B2_REQUIRE(point_stride == 3 || point_stride == 4, "b2_estimate_normals_from_covs: point_stride must be 3 or 4 (got %d)", point_stride);
   B2_REQUIRE(cov_stride == 9 || cov_stride == 16, "b2_estimate_normals_from_covs: cov_stride must be 9 or 16 (got %d)", cov_stride);
   if (n == 0) return B2_OK;
-  B2_CUDA(cudaSetDevice(ctx->device));
+  B2_ON_DEVICE(ctx);
   cudaStream_t st = ctx->stream;
   DeviceBuffer dp, dc, dn;
   B2_TRY(dp.upload(points, n * point_stride * sizeof(double), st));

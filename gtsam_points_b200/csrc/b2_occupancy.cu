@@ -418,7 +418,7 @@ b2_status b2_occgrid_create(b2_ctx* ctx, double resolution, b2_occgrid** out) {
   *out = nullptr;
   B2_REQUIRE(ctx != nullptr, "%s: ctx is NULL", who);
   B2_REQUIRE(resolution > 0.0 && std::isfinite(resolution), "%s: resolution must be positive and finite (got %g)", who, resolution);
-  B2_CUDA(cudaSetDevice(ctx->device));
+  B2_ON_DEVICE(ctx);
   auto g = std::make_unique<b2_occgrid>();
   g->ctx = ctx;
   g->resolution = resolution;
@@ -435,14 +435,14 @@ b2_status b2_occgrid_create(b2_ctx* ctx, double resolution, b2_occgrid** out) {
 
 b2_status b2_occgrid_destroy(b2_occgrid* grid) {
   if (!grid) return B2_OK;
-  cudaSetDevice(grid->ctx->device);
+  const b2::DeviceScope on_device(grid->ctx->device);
   delete grid;
   return B2_OK;
 }
 
 b2_status b2_occgrid_get_info(const b2_occgrid* grid, b2_occgrid_info* info) {
   B2_REQUIRE(grid && info, "b2_occgrid_get_info: NULL argument");
-  B2_CUDA(cudaSetDevice(grid->ctx->device));
+  B2_ON_DEVICE(grid->ctx);
   unsigned long long cells = 0;
   B2_TRY(occupied_cells(grid, &cells));
   info->resolution = grid->resolution;
@@ -457,7 +457,7 @@ b2_status b2_occgrid_insert(b2_occgrid* grid, const b2_cloud* cloud, const doubl
   B2_TRY(check_cloud(grid, cloud, T, who));
   const size_t n = cloud->n;
   if (n == 0) return B2_OK;
-  B2_CUDA(cudaSetDevice(grid->ctx->device));
+  B2_ON_DEVICE(grid->ctx);
   cudaStream_t st = grid->ctx->stream;
   const Pose P = make_pose(T);
   // at most half full afterwards: room for one new block per point, else per distinct block key of the batch
@@ -511,7 +511,7 @@ b2_status b2_occgrid_overlap(const b2_occgrid* grid, const b2_cloud* cloud, cons
   }
   std::memset(out_counts, 0, num_poses * sizeof(uint64_t));
   if (n == 0) return B2_OK;
-  B2_CUDA(cudaSetDevice(grid->ctx->device));
+  B2_ON_DEVICE(grid->ctx);
   cudaStream_t st = grid->ctx->stream;
   DeviceBuffer d_poses, d_counts, d_flags;
   B2_TRY(d_poses.upload(poses.data(), num_poses * sizeof(Pose), st));
@@ -539,7 +539,7 @@ b2_status b2_occgrid_free_rays(b2_occgrid* grid, const b2_cloud* cloud, const do
     B2_REQUIRE(int32_coord(origin[a], grid->inv_resolution), "%s: the sensor origin's voxel coordinate %d is outside int32", who, a);
   const size_t n = cloud->n;
   if (n == 0) return B2_OK;
-  B2_CUDA(cudaSetDevice(grid->ctx->device));
+  B2_ON_DEVICE(grid->ctx);
   cudaStream_t st = grid->ctx->stream;
   const Pose P = make_pose(T);
   with_storage(cloud->point_bytes, [&](auto p) {
@@ -555,7 +555,7 @@ b2_status b2_occgrid_free_rays(b2_occgrid* grid, const b2_cloud* cloud, const do
 b2_status b2_occgrid_download(const b2_occgrid* grid, int32_t* out_coords) {
   const char* who = "b2_occgrid_download";
   B2_REQUIRE(grid != nullptr, "%s: grid is NULL", who);
-  B2_CUDA(cudaSetDevice(grid->ctx->device));
+  B2_ON_DEVICE(grid->ctx);
   cudaStream_t st = grid->ctx->stream;
   const size_t cap = grid->capacity;
   DeviceBuffer counts, offsets, cells, sorted, coords, tmp;
@@ -600,7 +600,7 @@ b2_status b2_raycast(b2_ctx* ctx, const double* starts, const double* ends, size
   const double inv = 1.0 / voxel_size;
   for (size_t i = 0; i < n * 3; i++)
     B2_REQUIRE(int32_coord(starts[i], inv) && int32_coord(ends[i], inv), "%s: ray %zu: an endpoint is not finite or its voxel coordinate is outside int32", who, i / 3);
-  B2_CUDA(cudaSetDevice(ctx->device));
+  B2_ON_DEVICE(ctx);
   cudaStream_t st = ctx->stream;
   DeviceBuffer d_s, d_e, counts, offsets, coords, tmp;
   B2_TRY(d_s.upload(starts, n * 3 * sizeof(double), st));

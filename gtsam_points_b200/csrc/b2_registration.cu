@@ -905,7 +905,7 @@ b2_status create_features(bool pfh, const char* who, const b2_cloud* cloud, cons
     B2_REQUIRE(indices[k] >= 0 && static_cast<uint64_t>(indices[k]) < n, "%s: index %zu (%lld) is outside [0, %zu)", who, k, static_cast<long long>(indices[k]), n);
   B2_REQUIRE(nk < (1ull << 31), "%s: at most 2^31-1 rows", who);
   b2_ctx* ctx = cloud->ctx;
-  B2_CUDA(cudaSetDevice(ctx->device));
+  B2_ON_DEVICE(ctx);
   cudaStream_t st = ctx->stream;
   const int dim = pfh ? kPfhDim : kFpfhDim;
   auto f = std::make_unique<b2_features>();
@@ -976,7 +976,7 @@ b2_status b2_features_create(b2_ctx* ctx, const double* host, size_t n, int dim,
   B2_REQUIRE(host != nullptr || n == 0, "b2_features_create: host is NULL");
   B2_REQUIRE(n < (1ull << 31), "b2_features_create: at most 2^31-1 rows");
   for (size_t e = 0; e < n * dim; e++) B2_REQUIRE(std::isfinite(host[e]), "b2_features_create: value %zu is not finite", e);
-  B2_CUDA(cudaSetDevice(ctx->device));
+  B2_ON_DEVICE(ctx);
   auto f = std::make_unique<b2_features>();
   f->ctx = ctx, f->n = n, f->dim = dim;
   B2_TRY(f->d_rows.alloc(std::max<size_t>(n, 1) * dim * sizeof(double)));
@@ -990,7 +990,7 @@ b2_status b2_features_download(const b2_features* f, double* out) {
   B2_TRY(check_features(f, "b2_features_download"));
   B2_REQUIRE(out != nullptr || f->n == 0, "b2_features_download: out is NULL");
   if (f->n == 0) return B2_OK;
-  B2_CUDA(cudaSetDevice(f->ctx->device));
+  B2_ON_DEVICE(f->ctx);
   B2_CUDA(cudaMemcpyAsync(out, f->d_rows.get(), f->n * f->dim * sizeof(double), cudaMemcpyDeviceToHost, f->ctx->stream));
   B2_CUDA(cudaStreamSynchronize(f->ctx->stream));
   return B2_OK;
@@ -1007,7 +1007,7 @@ b2_status b2_features_get_info(const b2_features* f, b2_features_info* info) {
 
 b2_status b2_features_destroy(b2_features* f) {
   if (!f) return B2_OK;
-  cudaSetDevice(f->ctx->device);
+  const b2::DeviceScope on_device(f->ctx->device);
   delete f;
   return B2_OK;
 }
@@ -1034,7 +1034,7 @@ b2_status b2_features_nearest(const b2_features* queries, const b2_features* tar
   B2_REQUIRE(queries->ctx->device == targets->ctx->device, "b2_features_nearest: queries and targets live on different devices");
   const size_t nq = queries->n;
   if (nq == 0) return B2_OK;
-  B2_CUDA(cudaSetDevice(queries->ctx->device));
+  B2_ON_DEVICE(queries->ctx);
   cudaStream_t st = queries->ctx->stream;
   DeviceBuffer di, ds, part;
   B2_TRY(di.alloc(nq * sizeof(long long)));
@@ -1073,7 +1073,7 @@ b2_status b2_estimate_pose_ransac(const b2_cloud* target, const b2_cloud* source
   B2_REQUIRE(target->n > 0, "%s: the target is empty", who);
   const int dev = target->ctx->device;
   B2_REQUIRE(source->ctx->device == dev && target_features->ctx->device == dev && source_features->ctx->device == dev, "%s: inputs live on different devices", who);
-  B2_CUDA(cudaSetDevice(dev));
+  B2_ON_DEVICE(target->ctx);
   cudaStream_t st = target->ctx->stream;
 
   std::memset(out, 0, sizeof(*out));
@@ -1193,7 +1193,7 @@ b2_status b2_estimate_pose_gnc(const b2_cloud* target, const b2_cloud* source, c
   B2_REQUIRE(target->n > 0 && source->n > 0, "%s: the target and the source must not be empty", who);
   const int dev = target->ctx->device;
   B2_REQUIRE(source->ctx->device == dev && target_features->ctx->device == dev && source_features->ctx->device == dev, "%s: inputs live on different devices", who);
-  B2_CUDA(cudaSetDevice(dev));
+  B2_ON_DEVICE(target->ctx);
   cudaStream_t st = target->ctx->stream;
   const int sm = target->ctx->sm_count, D = source_features->dim;
 

@@ -624,7 +624,7 @@ b2_status b2_region_growing_create(const b2_cloud* cloud, const b2_kdtree* tree,
   B2_REQUIRE(tree == nullptr || tree->cloud_uid == cloud->uid, "%s: the tree was not built by b2_kdtree_create_from_cloud from this cloud", who);
   const size_t n = cloud->n;
   B2_REQUIRE(n < (1ull << 31), "%s: at most 2^31 - 1 points", who);
-  B2_CUDA(cudaSetDevice(cloud->ctx->device));
+  B2_ON_DEVICE(cloud->ctx);
   auto rg = std::make_unique<b2_region_growing>();
   rg->ctx = cloud->ctx;
   if (n > 0) {
@@ -656,7 +656,7 @@ b2_status b2_region_growing_get(const b2_region_growing* rg, uint64_t* size, int
   const uint64_t m = rg->dilated ? rg->num_dilated : std::min(rg->steps, rg->visits);
   *size = m;
   if (indices && m > 0) {
-    B2_CUDA(cudaSetDevice(rg->ctx->device));
+    B2_ON_DEVICE(rg->ctx);
     const DeviceBuffer& src = rg->dilated ? rg->d_dilated : rg->d_order;
     B2_CUDA(cudaMemcpyAsync(indices, src.get(), m * sizeof(int64_t), cudaMemcpyDeviceToHost, rg->ctx->stream));
     B2_CUDA(cudaStreamSynchronize(rg->ctx->stream));
@@ -666,7 +666,7 @@ b2_status b2_region_growing_get(const b2_region_growing* rg, uint64_t* size, int
 
 b2_status b2_region_growing_destroy(b2_region_growing* rg) {
   if (!rg) return B2_OK;
-  B2_CUDA(cudaSetDevice(rg->ctx->device));
+  B2_ON_DEVICE(rg->ctx);
   delete rg;
   return B2_OK;
 }
@@ -698,7 +698,7 @@ b2_status b2_min_cut(const b2_cloud* cloud, const b2_kdtree* tree, int64_t sourc
     info->flags = source_index < 0 ? B2_MIN_CUT_NO_SEED : 0;
     return B2_OK;
   }
-  B2_CUDA(cudaSetDevice(cloud->ctx->device));
+  B2_ON_DEVICE(cloud->ctx);
   b2_kdtree* own = nullptr;
   if (!tree) {
     B2_TRY(b2_kdtree_create_from_cloud(cloud, &own));

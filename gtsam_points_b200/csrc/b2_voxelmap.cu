@@ -551,7 +551,6 @@ b2_status insert_batch(b2_voxelmap* vm, int slots, const Cell& cell, OnChange&& 
 template <typename Cell, typename OnChange>
 b2_status insert_host(b2_voxelmap* vm, int slots, const Cell& cell, OnChange&& on_change, const double* points, int point_stride, const double* covs, int cov_stride,
                       size_t n, const char* who) {
-  B2_CUDA(cudaSetDevice(vm->ctx->device));
   DeviceBuffer d_p, d_c;
   if (n > 0) {
     B2_TRY(d_p.upload(points, n * point_stride * sizeof(double), vm->ctx->stream));
@@ -566,7 +565,6 @@ b2_status insert_host(b2_voxelmap* vm, int slots, const Cell& cell, OnChange&& o
 // reads its output there (the frame's planes are immutable once assemble_cloud has returned).
 template <typename Cell, typename OnChange>
 b2_status insert_cloud(b2_voxelmap* vm, int slots, const Cell& cell, OnChange&& on_change, const b2_cloud* frame, const double* T, bool with_covs, const char* who) {
-  B2_CUDA(cudaSetDevice(vm->ctx->device));
   const size_t n = frame->n;
   DeviceBuffer d_p, d_c;
   if (n > 0) {
@@ -858,7 +856,7 @@ b2_status ivox_knn(const b2_ivox* iv, const double* records, const double* queri
   B2_REQUIRE(nq == 0 || (queries && out_index && out_sq_dist), "%s: NULL argument", who);
   if (nq == 0) return B2_OK;
   const b2_voxelmap* vm = &iv->map;
-  B2_CUDA(cudaSetDevice(vm->ctx->device));
+  B2_ON_DEVICE(vm->ctx);
   cudaStream_t st = vm->ctx->stream;
   DeviceBuffer dq, di, ds;
   B2_TRY(dq.upload(queries, nq * query_stride * sizeof(double), st));
@@ -896,7 +894,6 @@ using namespace b2;
 
 b2_status ivox_enable_plane_view(const b2_ivox* iv) {
   if (iv->plane_view) return B2_OK;
-  B2_CUDA(cudaSetDevice(iv->map.ctx->device));
   iv->plane_view = true;
   const b2_status s = write_views(iv);
   if (s != B2_OK) {
@@ -917,7 +914,7 @@ b2_status b2_voxelmap_create_from_voxels(b2_ctx* ctx, double resolution, const i
   B2_REQUIRE(resolution > 0.0, "b2_voxelmap_create_from_voxels: resolution must be positive");
   B2_REQUIRE(V == 0 || (coords && means && covs), "b2_voxelmap_create_from_voxels: NULL voxel arrays");
   B2_REQUIRE(V < (1ull << 30), "b2_voxelmap_create_from_voxels: too many voxels");
-  B2_CUDA(cudaSetDevice(ctx->device));
+  B2_ON_DEVICE(ctx);
   auto vm = std::make_unique<b2_voxelmap>();
   B2_TRY(init_map(*vm, ctx, resolution, V));
 
@@ -964,7 +961,7 @@ b2_status b2_voxelmap_create(b2_ctx* ctx, double resolution, b2_voxelmap** out) 
   *out = nullptr;
   B2_REQUIRE(ctx != nullptr, "b2_voxelmap_create: ctx is NULL");
   B2_REQUIRE(resolution > 0.0, "b2_voxelmap_create: resolution must be positive");
-  B2_CUDA(cudaSetDevice(ctx->device));
+  B2_ON_DEVICE(ctx);
   auto vm = std::make_unique<b2_voxelmap>();
   B2_TRY(init_map(*vm, ctx, resolution, 0));
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -988,6 +985,7 @@ b2_status b2_voxelmap_insert(b2_voxelmap* vm, const double* points, int point_st
   B2_REQUIRE(cov_stride == 9 || cov_stride == 16, "b2_voxelmap_insert: cov_stride must be 9 or 16");
   B2_REQUIRE(n == 0 || (points && covs), "error: points/covs have not been allocated!!");  // GaussianVoxel::add reads covs
   B2_REQUIRE(n < (1ull << 31), "b2_voxelmap_insert: at most 2^31-1 points per insert");
+  B2_ON_DEVICE(vm->ctx);
   return insert_host(vm, 0, GaussianCell{}, [] {}, points, point_stride, covs, cov_stride, n, "b2_voxelmap_insert");
 }
 
@@ -997,6 +995,7 @@ b2_status b2_voxelmap_insert_cloud(b2_voxelmap* vm, const b2_cloud* frame, const
   B2_REQUIRE(vm != nullptr, "b2_voxelmap_insert_cloud: vm is NULL");
   B2_TRY(check_insert_cloud(*vm, frame, T_map_frame, "b2_voxelmap_insert_cloud"));
   B2_REQUIRE(frame->n == 0 || frame->d_covs, "b2_voxelmap_insert_cloud: the frame has no covariances");  // GaussianVoxel::add reads covs
+  B2_ON_DEVICE(vm->ctx);
   return insert_cloud(vm, 0, GaussianCell{}, [] {}, frame, T_map_frame, true, "b2_voxelmap_insert_cloud");
 }
 
@@ -1010,6 +1009,7 @@ b2_status b2_voxelmap_create_from_points(b2_ctx* ctx, double resolution, const d
   B2_REQUIRE(cov_stride == 9 || cov_stride == 16, "b2_voxelmap_create_from_points: cov_stride must be 9 or 16");
   B2_REQUIRE(n == 0 || (points && covs), "b2_voxelmap_create_from_points: points and covs are required");  // reference: GaussianVoxel::add reads covs
   B2_REQUIRE(n < (1ull << 31), "b2_voxelmap_create_from_points: at most 2^31-1 points");
+  B2_ON_DEVICE(ctx);
   b2_voxelmap* created = nullptr;
   B2_TRY(b2_voxelmap_create(ctx, resolution, &created));
   std::unique_ptr<b2_voxelmap> vm(created);
@@ -1020,7 +1020,7 @@ b2_status b2_voxelmap_create_from_points(b2_ctx* ctx, double resolution, const d
 
 b2_status b2_voxelmap_destroy(b2_voxelmap* vm) {
   if (!vm) return B2_OK;
-  cudaSetDevice(vm->ctx->device);
+  const b2::DeviceScope on_device(vm->ctx->device);
   delete vm;
   return B2_OK;
 }
@@ -1038,7 +1038,7 @@ b2_status b2_voxelmap_download(const b2_voxelmap* vm, int32_t* coords, double* m
   B2_REQUIRE(vm != nullptr, "b2_voxelmap_download: vm is NULL");
   const size_t V = vm->num_voxels;
   if (V == 0) return B2_OK;
-  B2_CUDA(cudaSetDevice(vm->ctx->device));
+  B2_ON_DEVICE(vm->ctx);
   cudaStream_t st = vm->ctx->stream;
   std::vector<double> rec(V * kRecordDoubles);
   B2_CUDA(cudaMemcpyAsync(rec.data(), vm->d_records.get(), rec.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
@@ -1130,7 +1130,7 @@ b2_status b2_overlap(const b2_voxelmap* const* targets, size_t num_targets, cons
   B2_REQUIRE(targets && source && Ts_target_source && out_overlap && num_targets > 0, "b2_overlap: NULL / empty argument");
   B2_REQUIRE(source->d_points, "error: source points have not been allocated!!");
   b2_ctx* ctx = source->ctx;
-  B2_CUDA(cudaSetDevice(ctx->device));
+  B2_ON_DEVICE(ctx);
   cudaStream_t st = ctx->stream;
   std::vector<OverlapMap> maps(num_targets);
   for (size_t j = 0; j < num_targets; j++) {
@@ -1164,7 +1164,7 @@ b2_status b2_voxelmap_lookup(const b2_voxelmap* vm, const double* points, int po
   B2_REQUIRE(vm && (n == 0 || (points && out_index)), "b2_voxelmap_lookup: NULL argument");
   B2_REQUIRE(point_stride == 3 || point_stride == 4, "b2_voxelmap_lookup: point_stride must be 3 or 4");
   if (n == 0) return B2_OK;
-  B2_CUDA(cudaSetDevice(vm->ctx->device));
+  B2_ON_DEVICE(vm->ctx);
   cudaStream_t st = vm->ctx->stream;
   DeviceBuffer dp, di;
   B2_TRY(dp.upload(points, n * point_stride * sizeof(double), st));
@@ -1184,7 +1184,7 @@ b2_status b2_ivox_create(b2_ctx* ctx, double resolution, b2_ivox** out) {
   *out = nullptr;
   B2_REQUIRE(ctx != nullptr, "b2_ivox_create: ctx is NULL");
   B2_REQUIRE(resolution > 0.0, "b2_ivox_create: resolution must be positive");
-  B2_CUDA(cudaSetDevice(ctx->device));
+  B2_ON_DEVICE(ctx);
   auto iv = std::make_unique<b2_ivox>();
   B2_TRY(init_map(iv->map, ctx, resolution, 0));  // the per-voxel arrays get their slot layout at the first insert
   B2_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -1194,7 +1194,7 @@ b2_status b2_ivox_create(b2_ctx* ctx, double resolution, b2_ivox** out) {
 
 b2_status b2_ivox_destroy(b2_ivox* iv) {
   if (!iv) return B2_OK;
-  cudaSetDevice(iv->map.ctx->device);
+  const b2::DeviceScope on_device(iv->map.ctx->device);
   for (cudaEvent_t e : iv->phase_ev)
     if (e) cudaEventDestroy(e);
   delete iv;
@@ -1203,7 +1203,7 @@ b2_status b2_ivox_destroy(b2_ivox* iv) {
 
 b2_status b2_ivox_clear(b2_ivox* iv) {
   B2_REQUIRE(iv != nullptr, "b2_ivox_clear: ivox is NULL");
-  B2_CUDA(cudaSetDevice(iv->map.ctx->device));
+  B2_ON_DEVICE(iv->map.ctx);
   iv->map.num_voxels = 0;  // incremental_voxelmap_impl.hpp:24-28
   iv->map.lru_counter = 0;
   iv->has_covs = -1;  // the next insert decides again whether the map holds covariances (the slot layout is kept)
@@ -1253,16 +1253,14 @@ b2_status b2_ivox_insert(b2_ivox* iv, const double* points, int point_stride, co
   B2_REQUIRE(covs == nullptr || cov_stride == 9 || cov_stride == 16, "b2_ivox_insert: cov_stride must be 9 or 16");
   B2_REQUIRE(n == 0 || points != nullptr, "b2_ivox_insert: points is NULL");
   B2_REQUIRE(n < (1ull << 31), "b2_ivox_insert: at most 2^31-1 points per insert");
-  if (iv->cov_est) {  // input covariances are ignored: the map estimates its own
-    const int slots = iv->map.slots > 0 ? iv->map.slots : iv->max_num_points_in_cell;
-    const FlatCell cell{slots, iv->max_num_points_in_cell, iv->min_sq_dist_in_cell};
-    return cov_est_insert(iv, [&] { return insert_host(&iv->map, slots, cell, [] {}, points, point_stride, nullptr, 9, n, "b2_ivox_insert"); });
-  }
   const int with_covs = covs != nullptr ? 1 : 0;
-  B2_REQUIRE(n == 0 || iv->has_covs < 0 || iv->has_covs == with_covs, "b2_ivox_insert: the map holds points %s covariances; inserts cannot mix both",
+  B2_REQUIRE(iv->cov_est || n == 0 || iv->has_covs < 0 || iv->has_covs == with_covs, "b2_ivox_insert: the map holds points %s covariances; inserts cannot mix both",
              iv->has_covs ? "with" : "without");
+  B2_ON_DEVICE(iv->map.ctx);
   const int slots = iv->map.slots > 0 ? iv->map.slots : iv->max_num_points_in_cell;  // the first insert fixes the slot layout
   const FlatCell cell{slots, iv->max_num_points_in_cell, iv->min_sq_dist_in_cell};
+  if (iv->cov_est)  // input covariances are ignored: the map estimates its own
+    return cov_est_insert(iv, [&] { return insert_host(&iv->map, slots, cell, [] {}, points, point_stride, nullptr, 9, n, "b2_ivox_insert"); });
   return insert_host(&iv->map, slots, cell, [&] { iv->has_covs = with_covs; }, points, point_stride, covs, cov_stride, n, "b2_ivox_insert");
 }
 
@@ -1272,16 +1270,14 @@ b2_status b2_ivox_insert(b2_ivox* iv, const double* points, int point_stride, co
 b2_status b2_ivox_insert_cloud(b2_ivox* iv, const b2_cloud* frame, const double* T_map_frame) {
   B2_REQUIRE(iv != nullptr, "b2_ivox_insert_cloud: ivox is NULL");
   B2_TRY(check_insert_cloud(iv->map, frame, T_map_frame, "b2_ivox_insert_cloud"));
-  if (iv->cov_est) {
-    const int slots = iv->map.slots > 0 ? iv->map.slots : iv->max_num_points_in_cell;
-    const FlatCell cell{slots, iv->max_num_points_in_cell, iv->min_sq_dist_in_cell};
-    return cov_est_insert(iv, [&] { return insert_cloud(&iv->map, slots, cell, [] {}, frame, T_map_frame, false, "b2_ivox_insert_cloud"); });
-  }
   const int with_covs = frame->d_covs ? 1 : 0;
-  B2_REQUIRE(frame->n == 0 || iv->has_covs < 0 || iv->has_covs == with_covs, "b2_ivox_insert_cloud: the map holds points %s covariances; inserts cannot mix both",
-             iv->has_covs ? "with" : "without");
+  B2_REQUIRE(iv->cov_est || frame->n == 0 || iv->has_covs < 0 || iv->has_covs == with_covs,
+             "b2_ivox_insert_cloud: the map holds points %s covariances; inserts cannot mix both", iv->has_covs ? "with" : "without");
+  B2_ON_DEVICE(iv->map.ctx);
   const int slots = iv->map.slots > 0 ? iv->map.slots : iv->max_num_points_in_cell;
   const FlatCell cell{slots, iv->max_num_points_in_cell, iv->min_sq_dist_in_cell};
+  if (iv->cov_est)
+    return cov_est_insert(iv, [&] { return insert_cloud(&iv->map, slots, cell, [] {}, frame, T_map_frame, false, "b2_ivox_insert_cloud"); });
   return insert_cloud(&iv->map, slots, cell, [&] { iv->has_covs = with_covs; }, frame, T_map_frame, with_covs != 0, "b2_ivox_insert_cloud");
 }
 
@@ -1294,7 +1290,7 @@ b2_status b2_ivox_get_info(const b2_ivox* iv, b2_ivox_info* info) {
   info->device_bytes = vm->device_bytes() + iv->d_plane_records.bytes();
   if (vm->num_voxels > 0) {
     std::vector<uint32_t> cnt(vm->num_voxels);
-    B2_CUDA(cudaSetDevice(vm->ctx->device));
+    B2_ON_DEVICE(vm->ctx);
     B2_CUDA(cudaMemcpyAsync(cnt.data(), vm->d_counts.get(), cnt.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, vm->ctx->stream));
     B2_CUDA(cudaStreamSynchronize(vm->ctx->stream));
     for (uint32_t c : cnt) info->num_points += c;
@@ -1307,7 +1303,7 @@ b2_status b2_ivox_download(const b2_ivox* iv, int32_t* coords, int32_t* counts, 
   const b2_voxelmap* vm = &iv->map;
   const size_t V = vm->num_voxels;
   if (V == 0) return B2_OK;
-  B2_CUDA(cudaSetDevice(vm->ctx->device));
+  B2_ON_DEVICE(vm->ctx);
   cudaStream_t st = vm->ctx->stream;
   std::vector<uint32_t> cnt(V);
   std::vector<double> rec(V * voxel_payload_doubles(vm->slots));
@@ -1396,6 +1392,7 @@ b2_status b2_ivox_download_state(const b2_ivox* iv, int32_t* coords, int32_t* co
   const size_t V = vm->num_voxels;
   B2_TRY(b2_ivox_download(iv, coords, counts, points, covs));
   if (V == 0 || (!flags && !normals)) return B2_OK;
+  B2_ON_DEVICE(vm->ctx);
   cudaStream_t st = vm->ctx->stream;
   const size_t P = V * vm->slots;
   std::vector<uint32_t> cnt(V);
@@ -1420,7 +1417,7 @@ b2_status b2_ivox_insert_timings(const b2_ivox* iv, double* ms) {
   B2_TRY(check_cov_est(iv, "b2_ivox_insert_timings"));
   B2_REQUIRE(ms != nullptr, "b2_ivox_insert_timings: ms is NULL");
   if (!iv->phase_ev[0]) return fail(B2_ERR_INVALID_STATE, "b2_ivox_insert_timings: nothing has been inserted");
-  B2_CUDA(cudaSetDevice(iv->map.ctx->device));
+  B2_ON_DEVICE(iv->map.ctx);
   for (int k = 0; k < 4; k++) {
     float t = 0.0f;
     B2_CUDA(cudaEventElapsedTime(&t, iv->phase_ev[k], iv->phase_ev[k + 1]));

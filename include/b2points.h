@@ -105,7 +105,9 @@ B2_API const char* b2_version(void);
 
 /* Create a context on CUDA device `device`.  `stream` is a cudaStream_t the caller owns (e.g. torch's current
  * stream) or NULL to let the context create its own non-blocking stream.  Replaces the reference's per-object
- * CUstream_st* arguments and StreamTempBufferRoundRobin (include/gtsam_points/cuda/stream_temp_buffer_roundrobin.hpp:49-65). */
+ * CUstream_st* arguments and StreamTempBufferRoundRobin (include/gtsam_points/cuda/stream_temp_buffer_roundrobin.hpp:49-65).
+ * Every call runs on its handles' device and returns with the calling thread's current CUDA context as it found it (none
+ * included), so a caller's own device selection survives calls on other devices. */
 B2_API b2_status b2_ctx_create(int device, void* stream, b2_ctx** out);
 B2_API b2_status b2_ctx_destroy(b2_ctx* ctx);
 B2_API b2_status b2_ctx_synchronize(b2_ctx* ctx);

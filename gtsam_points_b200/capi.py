@@ -102,6 +102,11 @@ SIGNATURES = {
     "b2_cloud_create": (C.c_int, [_vp, _dp, C.c_int, _dp, C.c_int, C.c_size_t, C.c_uint, _pp]),
     "b2_cloud_create_with_normals": (C.c_int, [_vp, _dp, C.c_int, _dp, C.c_int, _dp, C.c_int, C.c_size_t, C.c_uint, _pp]),
     "b2_cloud_download_normals": (C.c_int, [_vp, _dp]),
+    "b2_cloud_create_with_intensities": (C.c_int, [_vp, _dp, C.c_int, _dp, C.c_int, _dp, C.c_int, _dp, C.c_size_t, C.c_uint, _pp]),
+    "b2_cloud_intensity_bytes": (C.c_int, [_vp, C.POINTER(C.c_int)]),
+    "b2_cloud_create_with_added_intensities": (C.c_int, [_vp, _dp, C.c_uint, _pp]),
+    "b2_cloud_download_intensities": (C.c_int, [_vp, _dp]),
+    "b2_cloud_create_voxelgrid_with_intensities": (C.c_int, [_vp, C.c_double, _dp, C.c_int, _dp, C.c_int, _dp, C.c_int, _dp, C.c_size_t, C.c_uint, _pp]),
     "b2_cloud_download": (C.c_int, [_vp, _dp, _dp, _dp]),
     "b2_cloud_create_voxelgrid": (C.c_int, [_vp, C.c_double, _dp, C.c_int, _dp, C.c_int, _dp, C.c_int, C.c_size_t, C.c_uint, _pp]),
     "b2_cloud_create_estimated": (C.c_int, [_vp, _vp, C.c_int, _dp, C.c_int, C.c_uint, _pp]),
@@ -117,6 +122,9 @@ SIGNATURES = {
     "b2_voxelmap_set_lru": (C.c_int, [_vp, C.c_size_t, C.c_size_t]),
     "b2_voxelmap_insert": (C.c_int, [_vp, _dp, C.c_int, _dp, C.c_int, C.c_size_t]),
     "b2_voxelmap_insert_cloud": (C.c_int, [_vp, _vp, _dp]),
+    "b2_voxelmap_insert_with_intensities": (C.c_int, [_vp, _dp, C.c_int, _dp, C.c_int, _dp, C.c_size_t]),
+    "b2_voxelmap_create_from_voxels_with_intensities": (C.c_int, [_vp, C.c_double, _ip, _dp, _dp, _ip, _dp, C.c_size_t, _pp]),
+    "b2_voxelmap_download_intensities": (C.c_int, [_vp, _dp]),
     "b2_voxelmap_create_from_voxels": (C.c_int, [_vp, C.c_double, _ip, _dp, _dp, _ip, C.c_size_t, _pp]),
     "b2_voxelmap_destroy": (C.c_int, [_vp]),
     "b2_voxelmap_get_info": (C.c_int, [_vp, C.POINTER(VoxelMapInfo)]),
@@ -135,6 +143,8 @@ SIGNATURES = {
     "b2_ivox_set_insertion_setting": (C.c_int, [_vp, C.c_double, C.c_int]),
     "b2_ivox_insert": (C.c_int, [_vp, _dp, C.c_int, _dp, C.c_int, C.c_size_t]),
     "b2_ivox_insert_cloud": (C.c_int, [_vp, _vp, _dp]),
+    "b2_ivox_insert_with_intensities": (C.c_int, [_vp, _dp, C.c_int, _dp, C.c_int, _dp, C.c_size_t]),
+    "b2_ivox_download_intensities": (C.c_int, [_vp, _dp]),
     "b2_ivox_get_info": (C.c_int, [_vp, C.POINTER(IvoxInfo)]),
     "b2_ivox_download": (C.c_int, [_vp, _ip, _ip, _dp, _dp]),
     "b2_ivox_knn": (C.c_int, [_vp, _dp, C.c_int, C.c_size_t, C.c_int, C.c_double, _lp, _dp]),

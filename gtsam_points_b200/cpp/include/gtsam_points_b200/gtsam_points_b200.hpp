@@ -140,6 +140,14 @@ private:
 // ---------------------------------------------------------------------------------------------------------------------
 // Types
 // ---------------------------------------------------------------------------------------------------------------------
+namespace detail {
+// frame->intensities where the frame type has such a member (frame::has_intensities / frame::intensity, point_cloud.hpp:109), else null
+template <typename Frame>
+auto frame_intensities(const Frame& f, int) -> decltype(static_cast<const double*>(f.intensities)) { return f.intensities; }
+template <typename Frame>
+const double* frame_intensities(const Frame&, long) { return nullptr; }
+}  // namespace detail
+
 class PointCloudGPU {
 public:
   using Ptr = std::shared_ptr<PointCloudGPU>;
@@ -147,14 +155,20 @@ public:
 
   // points: the reference's Vector4d array (x,y,z,1), covs: its Matrix4d array (may be null) -- types/point_cloud.hpp:106-108
   PointCloudGPU(const double* points_xyz1, const double* covs_4x4, std::size_t n, Context::Ptr ctx = Context::default_context(), unsigned flags = B2_CLOUD_DEFAULT)
-  : ctx_(ctx), num_points_(n), has_covs_(covs_4x4 != nullptr) {
+  : ctx_(ctx), num_points_(n), has_covs_(covs_4x4 != nullptr), flags_(flags) {
     check(b2_cloud_create(ctx_->get(), points_xyz1, 4, covs_4x4, 16, n, flags, &cloud_), "b2_cloud_create");
   }
   // ... with the reference's normals array (Vector4d (nx,ny,nz,0), point_cloud.hpp:107; may be null)
   PointCloudGPU(const double* points_xyz1, const double* covs_4x4, const double* normals_xyz0, std::size_t n, Context::Ptr ctx = Context::default_context(),
                 unsigned flags = B2_CLOUD_DEFAULT)
-  : ctx_(ctx), num_points_(n), has_covs_(covs_4x4 != nullptr), has_normals_(normals_xyz0 != nullptr) {
+  : ctx_(ctx), num_points_(n), has_covs_(covs_4x4 != nullptr), has_normals_(normals_xyz0 != nullptr), flags_(flags) {
     check(b2_cloud_create_with_normals(ctx_->get(), points_xyz1, 4, covs_4x4, 16, normals_xyz0, 4, n, flags, &cloud_), "b2_cloud_create_with_normals");
+  }
+  // ... and the reference's intensities array (one double per point, point_cloud.hpp:109; may be null)
+  PointCloudGPU(const double* points_xyz1, const double* covs_4x4, const double* normals_xyz0, const double* intensities, std::size_t n,
+                Context::Ptr ctx = Context::default_context(), unsigned flags = B2_CLOUD_DEFAULT)
+  : ctx_(ctx), num_points_(n), has_covs_(covs_4x4 != nullptr), has_normals_(normals_xyz0 != nullptr), has_intensities_(intensities != nullptr), flags_(flags) {
+    check(b2_cloud_create_with_intensities(ctx_->get(), points_xyz1, 4, covs_4x4, 16, normals_xyz0, 4, intensities, n, flags, &cloud_), "b2_cloud_create_with_intensities");
   }
   // packed variants (xyz / 3x3)
   static Ptr from_packed(const double* xyz, const double* cov3x3, std::size_t n, Context::Ptr ctx = Context::default_context(), unsigned flags = B2_CLOUD_DEFAULT) {
@@ -162,12 +176,14 @@ public:
     p->ctx_ = ctx;
     p->num_points_ = n;
     p->has_covs_ = cov3x3 != nullptr;
+    p->flags_ = flags;
     check(b2_cloud_create(ctx->get(), xyz, 3, cov3x3, 9, n, flags, &p->cloud_), "b2_cloud_create");
     return p;
   }
   // Any frame with the reference's PointCloud shape: `points` -> array of 4 doubles per point, `covs` -> array of 16 doubles
-  // per point or null, size(), and -- if the frame type has one -- `normals` -> array of 4 doubles per point or null
-  // (frame::has_normals / frame::normal).  (Eigen::Vector4d / Matrix4d are exactly that.)  Uploaded once per frame and context.
+  // per point or null, size(), and -- if the frame type has them -- `normals` -> array of 4 doubles per point or null
+  // (frame::has_normals / frame::normal) and `intensities` -> array of doubles or null (frame::has_intensities / frame::intensity).
+  // (Eigen::Vector4d / Matrix4d are exactly that.)  Uploaded once per frame and context.
   template <typename Frame>
   static ConstPtr from_frame(const std::shared_ptr<const Frame>& frame, Context::Ptr ctx = Context::default_context()) {
     if (!frame || !frame->points) return nullptr;
@@ -178,7 +194,7 @@ public:
       if (auto alive = it->second.lock()) return alive;
     }
     auto cloud = std::make_shared<PointCloudGPU>(reinterpret_cast<const double*>(frame->points), reinterpret_cast<const double*>(frame->covs), frame_normals(*frame, 0),
-                                                 frame->size(), ctx);
+                                                 detail::frame_intensities(*frame, 0), frame->size(), ctx);
     ctx->frame_cache_[key] = cloud;
     return cloud;
   }
@@ -192,15 +208,39 @@ public:
     p->num_points_ = info.num_points;
     p->has_covs_ = info.cov_bytes != 0;
     p->has_normals_ = info.normal_bytes != 0;
+    int intensity_bytes = 0;
+    check(b2_cloud_intensity_bytes(cloud, &intensity_bytes), "b2_cloud_intensity_bytes");
+    p->has_intensities_ = intensity_bytes != 0;
     return p;
   }
-  ~PointCloudGPU() { b2_cloud_destroy(cloud_); }
+  // PointCloudGPU::add_intensities (point_cloud_gpu.hpp:113-119): n doubles in caller order.  A device cloud is immutable, so
+  // handle() becomes a new cloud with the same stored points, covariances, normals, Morton order and centre, copied on the device,
+  // and these intensities (b2_cloud_create_with_added_intensities).  Factors and trees made from the previous handle keep it: it
+  // lives until this object does, and every factor computes the same on either.
+  void add_intensities(const double* intensities) {
+    b2_cloud* fresh = nullptr;
+    check(b2_cloud_create_with_added_intensities(cloud_, intensities, flags_, &fresh), "b2_cloud_create_with_added_intensities");
+    retired_.push_back(cloud_);
+    cloud_ = fresh;
+    has_intensities_ = true;
+  }
+  // The intensities as stored on the device, in caller order (intensities_gpu)
+  std::vector<double> download_intensities() const {
+    std::vector<double> out(num_points_);
+    check(b2_cloud_download_intensities(cloud_, out.data()), "b2_cloud_download_intensities");
+    return out;
+  }
+  ~PointCloudGPU() {
+    b2_cloud_destroy(cloud_);
+    for (b2_cloud* c : retired_) b2_cloud_destroy(c);
+  }
   PointCloudGPU(const PointCloudGPU&) = delete;
 
   std::size_t size() const { return num_points_; }
   bool has_points() const { return true; }
   bool has_covs() const { return has_covs_; }
   bool has_normals() const { return has_normals_; }
+  bool has_intensities() const { return has_intensities_; }
   b2_cloud* handle() const { return cloud_; }
   Context::Ptr context() const { return ctx_; }
 
@@ -216,6 +256,9 @@ private:
   std::size_t num_points_ = 0;
   bool has_covs_ = false;
   bool has_normals_ = false;
+  bool has_intensities_ = false;
+  unsigned flags_ = B2_CLOUD_DEFAULT;  // those it was made with (adopt: B2_CLOUD_DEFAULT)
+  std::vector<b2_cloud*> retired_;     // handles add_intensities replaced: factors and trees made from them may still read them
 };
 
 // types/gaussian_voxelmap.hpp:16-50: the abstract map the factor constructors take
@@ -242,9 +285,10 @@ public:
   // GaussianVoxelMap::insert(const PointCloud&).  Unlike the reference's GPU map (one-shot, types/gaussian_voxelmap_gpu.hpp:63)
   // this is the CPU map's INCREMENTAL insert (ann/impl/incremental_voxelmap_impl.hpp:31-68): repeated calls extend the map,
   // ids stay first-touch, voxels untouched for lru_horizon inserts are dropped every lru_clear_cycle inserts.
-  void insert(const double* points, int point_stride, const double* covs, int cov_stride, std::size_t n) {
+  // intensities (n, may be null) raise each voxel's intensity to their maximum (GaussianVoxel::add; see b2points.h).
+  void insert(const double* points, int point_stride, const double* covs, int cov_stride, std::size_t n, const double* intensities = nullptr) {
     if (!vm_) check(b2_voxelmap_create(ctx_->get(), resolution_, &vm_), "b2_voxelmap_create");
-    check(b2_voxelmap_insert(vm_, points, point_stride, covs, cov_stride, n), "b2_voxelmap_insert");
+    check(b2_voxelmap_insert_with_intensities(vm_, points, point_stride, covs, cov_stride, intensities, n), "b2_voxelmap_insert_with_intensities");
   }
   // IncrementalVoxelMap::set_lru_horizon / set_lru_clear_cycle (ann/incremental_voxelmap.hpp:41-46); defaults 10 / 10
   void set_lru(std::size_t lru_horizon, std::size_t lru_clear_cycle) {
@@ -253,7 +297,7 @@ public:
   }
   // insert() of a device cloud posed by T_map_frame (null: as stored), without a host copy: GaussianVoxelMapGPU::insert(const
   // PointCloud&) from the frame's device arrays (gaussian_voxelmap_gpu.cu:211-227); the map afterwards equals insert() of the cloud's
-  // stored values posed as transform_gpu poses them.  The frame must have covariances.
+  // stored values posed as transform_gpu poses them.  The frame must have covariances; its intensities go in when it has them.
   void insert_cloud(const PointCloudGPU& frame, const Mat4* T_map_frame = nullptr) {
     if (!vm_) check(b2_voxelmap_create(ctx_->get(), resolution_, &vm_), "b2_voxelmap_create");
     check(b2_voxelmap_insert_cloud(vm_, frame.handle(), T_map_frame ? T_map_frame->data() : nullptr), "b2_voxelmap_insert_cloud");
@@ -264,7 +308,7 @@ public:
       std::cerr << "error: points/covs have not been allocated!!" << std::endl;  // gaussian_voxelmap_gpu.cu:218-222
       abort();
     }
-    insert(reinterpret_cast<const double*>(frame.points), 4, reinterpret_cast<const double*>(frame.covs), 16, frame.size());
+    insert(reinterpret_cast<const double*>(frame.points), 4, reinterpret_cast<const double*>(frame.covs), 16, frame.size(), detail::frame_intensities(frame, 0));
   }
   void save_compact(const std::string& path) const override {
     if (!vm_) throw std::runtime_error("GaussianVoxelMapGPU::save_compact: empty map");
@@ -292,6 +336,13 @@ private:
   double resolution_;
   b2_voxelmap* vm_ = nullptr;
 };
+
+// Each voxel's intensity in id order (GaussianVoxel::intensity: the maximum, from 0, of its points' intensities)
+inline std::vector<double> download_voxel_intensities(const GaussianVoxelMapGPU& voxelmap) {
+  std::vector<double> out(voxelmap.num_voxels());
+  if (voxelmap.handle()) check(b2_voxelmap_download_intensities(voxelmap.handle(), out.data()), "b2_voxelmap_download_intensities");
+  return out;
+}
 
 // overlap_gpu (types/gaussian_voxelmap_gpu.hpp:116-125): fraction of source points that fall into a voxel of the target
 inline double overlap_gpu(const GaussianVoxelMap::ConstPtr& target, const PointCloudGPU::ConstPtr& source, const Mat4& T_target_source) {
@@ -844,17 +895,19 @@ public:
   iVoxGPU(const iVoxGPU&) = delete;
 
   // IncrementalVoxelMap::insert (incremental_voxelmap_impl.hpp:31-68): points (point_stride 3 or 4) with optional covariances
-  // (cov_stride 9 or 16); every insert into one map either has covariances or has none
-  void insert(const double* points, int point_stride, const double* covs, int cov_stride, std::size_t n) {
-    check(b2_ivox_insert(ivox_, points, point_stride, covs, cov_stride, n), "b2_ivox_insert");
+  // (cov_stride 9 or 16) and intensities (n, may be null); every insert into one map either has covariances or has none, and the
+  // same for intensities
+  void insert(const double* points, int point_stride, const double* covs, int cov_stride, std::size_t n, const double* intensities = nullptr) {
+    check(b2_ivox_insert_with_intensities(ivox_, points, point_stride, covs, cov_stride, intensities, n), "b2_ivox_insert_with_intensities");
   }
-  // the reference's frame shape (gtsam_points::PointCloud: Vector4d points, Matrix4d covs, size())
+  // the reference's frame shape (gtsam_points::PointCloud: Vector4d points, Matrix4d covs, intensities, size())
   template <typename Frame, typename = decltype(std::declval<const Frame&>().points)>
   void insert(const Frame& frame) {
-    insert(reinterpret_cast<const double*>(frame.points), 4, frame.covs ? reinterpret_cast<const double*>(frame.covs) : nullptr, 16, frame.size());
+    insert(reinterpret_cast<const double*>(frame.points), 4, frame.covs ? reinterpret_cast<const double*>(frame.covs) : nullptr, 16, frame.size(),
+           detail::frame_intensities(frame, 0));
   }
   // insert() of a device cloud posed by T_map_frame (null: as stored), without a host copy: the map update of frame-to-map odometry
-  // (advanced_scan_matching.cpp:84-95) in one call.  The frame's covariances go in iff it has them.
+  // (advanced_scan_matching.cpp:84-95) in one call.  The frame's covariances and intensities go in iff it has them.
   void insert_cloud(const PointCloudGPU& frame, const Mat4* T_map_frame = nullptr) {
     check(b2_ivox_insert_cloud(ivox_, frame.handle(), T_map_frame ? T_map_frame->data() : nullptr), "b2_ivox_insert_cloud");
   }
@@ -906,6 +959,13 @@ public:
     points.resize(n * 3);
     covs.resize(n * 9);
     check(b2_ivox_download(ivox_, nullptr, nullptr, points.data(), covs.data()), "b2_ivox_download");
+  }
+  // voxel_intensities() (incremental_voxelmap_impl.hpp:183-189): in download()'s order; throws on a map whose points came without
+  // intensities, and on an iVoxCovarianceEstimationGPU
+  std::vector<double> voxel_intensities() const {
+    std::vector<double> out(size());
+    check(b2_ivox_download_intensities(ivox_, out.data()), "b2_ivox_download_intensities");
+    return out;
   }
   b2_ivox* handle() const { return ivox_; }
   Context::Ptr context() const { return ctx_; }

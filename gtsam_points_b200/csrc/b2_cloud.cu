@@ -159,6 +159,31 @@ __global__ void gather_normals_kernel(const double* __restrict__ nrm, int nstrid
   for (int k = 0; k < 3; k++) out_n[k * n_pad + i] = i < n ? static_cast<NT>(nrm[s * nstride + k]) : static_cast<NT>(0);
 }
 
+// Intensities of the raw upload: bit0 = some value not f32-exact (NaN included: it is kept bit for bit only in float64).  Any
+// value is accepted; nothing computes on them.
+__global__ void scan_intensities_kernel(const double* __restrict__ v, size_t n, unsigned int* __restrict__ res) {
+  unsigned int flags = 0;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    if (!f32_exact(v[i])) flags = 1u;
+  flags = __reduce_or_sync(0xffffffffu, flags);
+  if ((threadIdx.x & 31) == 0 && flags) atomicOr(res, flags);
+}
+
+// The intensity plane in the stored order of the points; padding is 0 (never read).
+template <typename IT>
+__global__ void gather_intensities_kernel(const double* __restrict__ v, const uint32_t* __restrict__ perm, size_t n, size_t n_pad, IT* __restrict__ out) {
+  const size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
+  if (i >= n_pad) return;
+  out[i] = i < n ? static_cast<IT>(v[perm ? perm[i] : i]) : static_cast<IT>(0);
+}
+
+// Its inverse: stored position i -> caller row perm[i], as doubles
+template <typename IT>
+__global__ void scatter_intensities_kernel(const IT* __restrict__ v, const uint32_t* __restrict__ perm, size_t n, double* __restrict__ out) {
+  const size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
+  if (i < n) out[perm ? perm[i] : i] = static_cast<double>(v[i]);
+}
+
 // The inverse of the gathers, in one launch: the stored planes -> doubles in the caller's order, point i of the storage to row
 // perm[i].  Points n x 3, covariances n x 9 (unposed: the symmetric 3x3 of the stored upper triangle; posed: T C T^T as computed),
 // normals n x 3; a NULL output is not written.  posed == 0 copies the stored values as they are (no arithmetic, so -0.0 keeps its
@@ -235,14 +260,17 @@ __global__ void key_starts_kernel(const uint32_t* __restrict__ flags, const uint
 
 // One thread per voxel: sums of the points, all nine covariance entries (row-major 3x3, stride 9, or 4x4, stride 16) and normals of
 // its segment of the sorted caller indices (caller order: the sort is stable), in float64 one addition after another, each divided
-// by the count (Averager::average, point_cloud_cpu_funcs.cpp:96-116).  Outputs m x 3 / m x 9 / m x 3.
+// by the count (Averager::average, point_cloud_cpu_funcs.cpp:96-116).  Outputs m x 3 / m x 9 / m x 3.  Intensities (ints, may be
+// NULL) go to out_i (m): averaged the same way, or with int_max their maximum from 0.0 in the same order, v = (v < x) ? x : v
+// (std::max(v, x) of merge_frames, gaussian_voxelmap_cpu_funcs.cpp:88-101).
 __global__ void voxel_sum_kernel(const double* __restrict__ pts, int pstride, const double* __restrict__ covs, int cstride, const double* __restrict__ nrm,
-                                 int nstride, const uint32_t* __restrict__ sorted_vals, const uint32_t* __restrict__ starts, uint32_t num_voxels,
-                                 double* __restrict__ out_p, double* __restrict__ out_c, double* __restrict__ out_n) {
+                                 int nstride, const double* __restrict__ ints, int int_max, const uint32_t* __restrict__ sorted_vals,
+                                 const uint32_t* __restrict__ starts, uint32_t num_voxels, double* __restrict__ out_p, double* __restrict__ out_c,
+                                 double* __restrict__ out_n, double* __restrict__ out_i) {
   const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= num_voxels) return;
   const int ld = cstride == 16 ? 4 : 3;
-  double sp[3] = {0.0, 0.0, 0.0}, sc[9] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0}, sn[3] = {0.0, 0.0, 0.0};
+  double sp[3] = {0.0, 0.0, 0.0}, sc[9] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0}, sn[3] = {0.0, 0.0, 0.0}, si = 0.0;
   const uint32_t first = starts[v], last = starts[v + 1];
   for (uint32_t k = first; k < last; k++) {
     const size_t i = sorted_vals[k];
@@ -256,6 +284,7 @@ __global__ void voxel_sum_kernel(const double* __restrict__ pts, int pstride, co
     if (nrm)
 #pragma unroll
       for (int a = 0; a < 3; a++) sn[a] = __dadd_rn(sn[a], nrm[i * nstride + a]);
+    if (ints) si = int_max ? (si < ints[i] ? ints[i] : si) : __dadd_rn(si, ints[i]);
   }
   const double cnt = static_cast<double>(last - first);
 #pragma unroll
@@ -266,14 +295,15 @@ __global__ void voxel_sum_kernel(const double* __restrict__ pts, int pstride, co
   if (nrm)
 #pragma unroll
     for (int a = 0; a < 3; a++) out_n[static_cast<size_t>(v) * 3 + a] = __ddiv_rn(sn[a], cnt);
+  if (ints) out_i[v] = int_max ? si : __ddiv_rn(si, cnt);
 }
 
 // The averages of `in`'s in.n points per voxel: a stable sort of the n (key, caller index) pairs over all 64 bits, the
-// segments of equal keys among the first `count` sorted entries, then voxel_sum_kernel.  out_p / out_c / out_n get m x 3 / m x 9 /
-// m x 3 doubles (out_c, out_n: iff in has covariances / normals) in ascending key order, *m = the number of voxels (0 for count 0).
-// Synchronises the stream, so the inputs may be freed afterwards.
+// segments of equal keys among the first `count` sorted entries, then voxel_sum_kernel.  out_p / out_c / out_n / out_i get m x 3 /
+// m x 9 / m x 3 / m doubles (out_c, out_n, out_i: iff in has covariances / normals / intensities; out_i the maxima with int_max) in
+// ascending key order, *m = the number of voxels (0 for count 0).  Synchronises the stream, so the inputs may be freed afterwards.
 b2_status average_voxels(const DeviceBuffer& keys, const DeviceBuffer& vals, const RawCloud& in, size_t count, cudaStream_t st, DeviceBuffer& out_p, DeviceBuffer& out_c,
-                         DeviceBuffer& out_n, uint32_t* m) {
+                         DeviceBuffer& out_n, DeviceBuffer& out_i, bool int_max, uint32_t* m) {
   *m = 0;
   if (count == 0) return B2_OK;
   const size_t n = in.n;
@@ -289,9 +319,10 @@ b2_status average_voxels(const DeviceBuffer& keys, const DeviceBuffer& vals, con
   B2_TRY(out_p.alloc(v * 3 * sizeof(double)));
   if (in.covs) B2_TRY(out_c.alloc(v * 9 * sizeof(double)));
   if (in.normals) B2_TRY(out_n.alloc(v * 3 * sizeof(double)));
+  if (in.intensities) B2_TRY(out_i.alloc(v * sizeof(double)));
   voxel_sum_kernel<<<static_cast<unsigned>((v + 127) / 128), 128, 0, st>>>(in.points, in.point_stride, in.covs, in.cov_stride, in.normals, in.normal_stride,
-                                                                           vals2.as<const uint32_t>(), starts.as<const uint32_t>(), *m, out_p.as<double>(),
-                                                                           out_c.as<double>(), out_n.as<double>());
+                                                                           in.intensities, int_max ? 1 : 0, vals2.as<const uint32_t>(), starts.as<const uint32_t>(),
+                                                                           *m, out_p.as<double>(), out_c.as<double>(), out_n.as<double>(), out_i.as<double>());
   B2_CUDA(cudaGetLastError());
   B2_CUDA(cudaStreamSynchronize(st));
   return B2_OK;
@@ -307,29 +338,33 @@ struct MinU64 {
   __host__ __device__ unsigned long long operator()(unsigned long long a, unsigned long long b) const { return a < b ? a : b; }
 };
 
-// The checks of both merge entry points; *total = the number of input points, *have_covs = every non-empty frame has covariances.
+// The checks of both merge entry points; *total = the number of input points, *have_covs = every non-empty frame has covariances,
+// *have_ints = every frame has intensities (empty ones too: merge_frames asks frame::has_intensities of each, :88).
 b2_status merge_frames_check(b2_ctx* ctx, const double* poses, const b2_cloud* const* frames, size_t num_frames, double downsample_resolution, const char* who,
-                             size_t* total, bool* have_covs) {
+                             size_t* total, bool* have_covs, bool* have_ints) {
   B2_REQUIRE(ctx && poses && frames && num_frames > 0, "%s: NULL / empty argument", who);
   B2_REQUIRE(downsample_resolution > 0.0, "%s: downsample_resolution must be positive", who);
   *total = 0;
   *have_covs = true;
+  *have_ints = true;
   for (size_t f = 0; f < num_frames; f++) {
     B2_REQUIRE(frames[f] != nullptr && (frames[f]->n == 0 || frames[f]->d_points), "error: frame %zu has no points", f);
     B2_REQUIRE(frames[f]->ctx->device == ctx->device, "%s: frame %zu lives on another device", who, f);
     B2_TRY(check_pose(poses + 16 * f, who));
     *total += frames[f]->n;
     *have_covs = *have_covs && (frames[f]->n == 0 || frames[f]->d_covs);
+    *have_ints = *have_ints && frames[f]->d_intensities;
   }
   B2_REQUIRE(*total < (1ull << 31), "%s: too many points", who);
   return B2_OK;
 }
 
 // merge_frames of total > 0 checked points on the device: d_xyz (m x 3) and d_cov (m x 9, zeros where no frame has covariances)
-// get the m = *out_n merged points.  Every frame is posed by the cloud scatter twice, into frame-major caller order: into the first
-// frame's coordinates for the keys, into the world for the sums.  Synchronises the context's stream.
+// get the m = *out_n merged points, and with have_ints (every frame has intensities) d_int (m) their per-voxel maxima from 0.0.
+// Every frame is posed by the cloud scatter twice, into frame-major caller order: into the first frame's coordinates for the keys,
+// into the world for the sums.  Synchronises the context's stream.
 b2_status merge_frames_device(b2_ctx* ctx, const double* poses, const b2_cloud* const* frames, size_t num_frames, double downsample_resolution, size_t total,
-                              bool have_covs, DeviceBuffer& d_xyz, DeviceBuffer& d_cov, size_t* out_n) {
+                              bool have_covs, bool have_ints, DeviceBuffer& d_xyz, DeviceBuffer& d_cov, DeviceBuffer& d_int, size_t* out_n) {
   cudaStream_t st = ctx->stream;
 
   // first_pose^-1 (rigid inverse) and the relative poses, with the CPU function's operation order
@@ -339,10 +374,11 @@ b2_status merge_frames_device(b2_ctx* ctx, const double* poses, const b2_cloud* 
     for (int c = 0; c < 3; c++) inv0[r * 4 + c] = at(poses, c, r);
   for (int r = 0; r < 3; r++) inv0[r * 4 + 3] = -(inv0[r * 4 + 0] * at(poses, 0, 3) + inv0[r * 4 + 1] * at(poses, 1, 3) + inv0[r * 4 + 2] * at(poses, 2, 3));
   inv0[15] = 1.0;
-  DeviceBuffer key_pts, world_pts, world_covs, keys, vals, d_min, tmp, no_normals;
+  DeviceBuffer key_pts, world_pts, world_covs, world_ints, keys, vals, d_min, tmp, no_normals;
   B2_TRY(key_pts.alloc(total * 3 * sizeof(double)));
   B2_TRY(world_pts.alloc(total * 3 * sizeof(double)));
   if (have_covs) B2_TRY(world_covs.alloc(total * 9 * sizeof(double)));
+  if (have_ints) B2_TRY(world_ints.alloc(total * sizeof(double)));
   size_t off = 0;
   for (size_t f = 0; f < num_frames; f++) {
     const b2_cloud* c = frames[f];
@@ -357,6 +393,7 @@ b2_status merge_frames_device(b2_ctx* ctx, const double* poses, const b2_cloud* 
       }
     B2_TRY(cloud_arrays_to_device(c, st, rel, key_pts.as<double>() + 3 * off, nullptr, nullptr));
     B2_TRY(cloud_arrays_to_device(c, st, P, world_pts.as<double>() + 3 * off, have_covs ? world_covs.as<double>() + 9 * off : nullptr, nullptr));
+    if (have_ints) B2_TRY(cloud_intensities_to_device(c, st, world_ints.as<double>() + off));
     off += c->n;
   }
   unsigned int kept = 0;
@@ -368,9 +405,9 @@ b2_status merge_frames_device(b2_ctx* ctx, const double* poses, const b2_cloud* 
   fold_unkeyed_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(keys.as<unsigned long long>(), total, d_min.as<const unsigned long long>());
   B2_CUDA(cudaGetLastError());
   RawCloud world;
-  world.points = world_pts.as<const double>(), world.covs = world_covs.as<const double>(), world.n = total;
+  world.points = world_pts.as<const double>(), world.covs = world_covs.as<const double>(), world.intensities = world_ints.as<const double>(), world.n = total;
   uint32_t m = 0;
-  B2_TRY(average_voxels(keys, vals, world, total, st, d_xyz, d_cov, no_normals, &m));
+  B2_TRY(average_voxels(keys, vals, world, total, st, d_xyz, d_cov, no_normals, d_int, true, &m));
   if (!have_covs) {
     B2_TRY(d_cov.alloc(static_cast<size_t>(m) * 9 * sizeof(double)));
     B2_CUDA(cudaMemsetAsync(d_cov.get(), 0, d_cov.bytes(), st));
@@ -484,6 +521,26 @@ b2_status assemble_cloud(b2_ctx* ctx, const RawCloud& raw, unsigned flags, const
     B2_CUDA(cudaGetLastError());
   }
 
+  if (raw.intensities) {
+    unsigned int iflags = 0;
+    if (n > 0) {
+      unsigned int* d_iflags = &d_res.as<ScanResult>()->flags;
+      B2_CUDA(cudaMemsetAsync(d_iflags, 0, sizeof(unsigned int), st));
+      const int grid = static_cast<int>(std::min<size_t>((n + 255) / 256, static_cast<size_t>(ctx->sm_count) * 8));
+      scan_intensities_kernel<<<grid, 256, 0, st>>>(raw.intensities, n, d_iflags);
+      B2_CUDA(cudaGetLastError());
+      B2_CUDA(cudaMemcpyAsync(&iflags, d_iflags, sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
+      B2_CUDA(cudaStreamSynchronize(st));
+    }
+    c->intensity_bytes = force64 ? 8 : (compact || !(iflags & 1u)) ? 4 : 8;
+    B2_TRY(c->d_intensities.alloc(c->n_pad * c->intensity_bytes));
+    with_storage(c->intensity_bytes, [&](auto t) {
+      using IT = decltype(t);
+      gather_intensities_kernel<IT><<<static_cast<unsigned>((c->n_pad + 255) / 256), 256, 0, st>>>(raw.intensities, perm, n, c->n_pad, c->d_intensities.as<IT>());
+    });
+    B2_CUDA(cudaGetLastError());
+  }
+
   // planes
   if (!like) B2_TRY(c->d_points.alloc(3 * c->n_pad * c->point_bytes));
   if (raw.covs) B2_TRY(c->d_covs.alloc(6 * c->n_pad * c->cov_bytes));
@@ -556,6 +613,15 @@ b2_status cloud_arrays_to_device(const b2_cloud* c, cudaStream_t st, const doubl
   return B2_OK;
 }
 
+b2_status cloud_intensities_to_device(const b2_cloud* c, cudaStream_t st, double* d_out) {
+  with_storage(c->intensity_bytes, [&](auto t) {
+    using IT = decltype(t);
+    scatter_intensities_kernel<IT><<<static_cast<unsigned>((c->n + 255) / 256), 256, 0, st>>>(c->d_intensities.as<const IT>(), c->d_perm.as<const uint32_t>(), c->n, d_out);
+  });
+  B2_CUDA(cudaGetLastError());
+  return B2_OK;
+}
+
 }  // namespace b2
 
 using namespace b2;
@@ -569,6 +635,11 @@ b2_status b2_cloud_create(b2_ctx* ctx, const double* points, int point_stride, c
 
 b2_status b2_cloud_create_with_normals(b2_ctx* ctx, const double* points, int point_stride, const double* covs, int cov_stride, const double* normals,
                                        int normal_stride, size_t n, unsigned flags, b2_cloud** out) {
+  return b2_cloud_create_with_intensities(ctx, points, point_stride, covs, cov_stride, normals, normal_stride, nullptr, n, flags, out);
+}
+
+b2_status b2_cloud_create_with_intensities(b2_ctx* ctx, const double* points, int point_stride, const double* covs, int cov_stride, const double* normals,
+                                           int normal_stride, const double* intensities, size_t n, unsigned flags, b2_cloud** out) {
   B2_REQUIRE(out != nullptr, "b2_cloud_create: out is NULL");
   *out = nullptr;
   B2_REQUIRE(ctx != nullptr, "b2_cloud_create: ctx is NULL");
@@ -581,7 +652,7 @@ b2_status b2_cloud_create_with_normals(b2_ctx* ctx, const double* points, int po
   cudaStream_t st = ctx->stream;
 
   // H2D staging of the host arrays; assemble_cloud does the rest on the device
-  DeviceBuffer raw_p, raw_c, raw_n;
+  DeviceBuffer raw_p, raw_c, raw_n, raw_i;
   RawCloud raw;
   raw.point_stride = point_stride, raw.cov_stride = cov_stride, raw.normal_stride = normal_stride, raw.n = n;
   auto stage = [&](DeviceBuffer& buf, const double* src, int stride, const double** dst) -> b2_status {
@@ -595,11 +666,72 @@ b2_status b2_cloud_create_with_normals(b2_ctx* ctx, const double* points, int po
   B2_TRY(stage(raw_p, points, point_stride, &raw.points));
   B2_TRY(stage(raw_c, covs, cov_stride, &raw.covs));
   B2_TRY(stage(raw_n, normals, normal_stride, &raw.normals));
-  return assemble_cloud(ctx, raw, flags, nullptr, out, normals ? "b2_cloud_create_with_normals" : "b2_cloud_create");
+  B2_TRY(stage(raw_i, intensities, 1, &raw.intensities));
+  return assemble_cloud(ctx, raw, flags, nullptr, out, intensities ? "b2_cloud_create_with_intensities" : normals ? "b2_cloud_create_with_normals" : "b2_cloud_create");
+}
+
+b2_status b2_cloud_intensity_bytes(const b2_cloud* cloud, int* out) {
+  B2_REQUIRE(cloud && out, "b2_cloud_intensity_bytes: NULL argument");
+  *out = cloud->intensity_bytes;
+  return B2_OK;
+}
+
+b2_status b2_cloud_download_intensities(const b2_cloud* c, double* out) {
+  B2_REQUIRE(c != nullptr && (out != nullptr || c->n == 0), "b2_cloud_download_intensities: NULL argument");
+  if (!c->d_intensities) return fail(B2_ERR_INVALID_STATE, "b2_cloud_download_intensities: the cloud has no intensities");
+  if (c->n == 0) return B2_OK;
+  B2_ON_DEVICE(c->ctx);
+  cudaStream_t st = c->ctx->stream;
+  DeviceBuffer d_out;
+  B2_TRY(d_out.alloc(c->n * sizeof(double)));
+  B2_TRY(cloud_intensities_to_device(c, st, d_out.as<double>()));
+  B2_CUDA(cudaMemcpyAsync(out, d_out.get(), c->n * sizeof(double), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  return B2_OK;
+}
+
+// PointCloudGPU::add_intensities without touching the input: a new cloud with the input's stored planes, permutation and centre
+// (assemble_cloud's `like` copies), its covariance and normal buffers copied as they are, and the given intensities.
+b2_status b2_cloud_create_with_added_intensities(const b2_cloud* cloud, const double* intensities, unsigned flags, b2_cloud** out) {
+  const char* who = "b2_cloud_create_with_added_intensities";
+  B2_REQUIRE(out != nullptr, "%s: out is NULL", who);
+  *out = nullptr;
+  B2_REQUIRE(cloud != nullptr, "%s: cloud is NULL", who);
+  B2_REQUIRE(intensities != nullptr, "%s: intensities is NULL", who);
+  B2_ON_DEVICE(cloud->ctx);
+  cudaStream_t st = cloud->ctx->stream;
+  DeviceBuffer d_i;
+  RawCloud raw;
+  raw.intensities = intensities;  // n == 0: marks that the cloud has them; never read
+  if (cloud->n > 0) {
+    B2_TRY(d_i.upload(intensities, cloud->n * sizeof(double), st));
+    raw.intensities = d_i.as<const double>();
+  }
+  b2_cloud* made = nullptr;
+  B2_TRY(assemble_cloud(cloud->ctx, raw, flags, cloud, &made, who));
+  std::unique_ptr<b2_cloud> c(made);
+  auto copy = [&](DeviceBuffer& dst, const DeviceBuffer& src) -> b2_status {
+    if (!src) return B2_OK;
+    B2_TRY(dst.alloc(src.bytes()));
+    B2_CUDA(cudaMemcpyAsync(dst.get(), src.get(), src.bytes(), cudaMemcpyDeviceToDevice, st));
+    return B2_OK;
+  };
+  B2_TRY(copy(c->d_covs, cloud->d_covs));
+  B2_TRY(copy(c->d_normals, cloud->d_normals));
+  c->cov_bytes = cloud->cov_bytes;
+  c->normal_bytes = cloud->normal_bytes;
+  B2_CUDA(cudaStreamSynchronize(st));
+  *out = c.release();
+  return B2_OK;
 }
 
 b2_status b2_cloud_create_voxelgrid(b2_ctx* ctx, double resolution, const double* points, int point_stride, const double* covs, int cov_stride, const double* normals,
                                     int normal_stride, size_t n, unsigned flags, b2_cloud** out) {
+  return b2_cloud_create_voxelgrid_with_intensities(ctx, resolution, points, point_stride, covs, cov_stride, normals, normal_stride, nullptr, n, flags, out);
+}
+
+b2_status b2_cloud_create_voxelgrid_with_intensities(b2_ctx* ctx, double resolution, const double* points, int point_stride, const double* covs, int cov_stride,
+                                                     const double* normals, int normal_stride, const double* intensities, size_t n, unsigned flags, b2_cloud** out) {
   B2_REQUIRE(out != nullptr, "b2_cloud_create_voxelgrid: out is NULL");
   *out = nullptr;
   B2_REQUIRE(ctx != nullptr, "b2_cloud_create_voxelgrid: ctx is NULL");
@@ -614,29 +746,32 @@ b2_status b2_cloud_create_voxelgrid(b2_ctx* ctx, double resolution, const double
 
   // the averaged arrays (one entry per voxel, ascending key order).  For an empty result the caller's pointers stay in their place:
   // they tell assemble_cloud which arrays the cloud has and are never read.
-  DeviceBuffer avg_p, avg_c, avg_n;
+  DeviceBuffer avg_p, avg_c, avg_n, avg_i;
   RawCloud avg;
-  avg.points = points, avg.covs = covs, avg.normals = normals;
+  avg.points = points, avg.covs = covs, avg.normals = normals, avg.intensities = intensities;
   avg.point_stride = 3, avg.cov_stride = 9, avg.normal_stride = 3;
   if (n > 0) {
-    DeviceBuffer raw_p, raw_c, raw_n, keys, vals;
+    DeviceBuffer raw_p, raw_c, raw_n, raw_i, keys, vals;
     B2_TRY(raw_p.upload(points, n * point_stride * sizeof(double), st));
     if (covs) B2_TRY(raw_c.upload(covs, n * cov_stride * sizeof(double), st));
     if (normals) B2_TRY(raw_n.upload(normals, n * normal_stride * sizeof(double), st));
+    if (intensities) B2_TRY(raw_i.upload(intensities, n * sizeof(double), st));
     RawCloud in;
     in.points = raw_p.as<const double>(), in.point_stride = point_stride;
     in.covs = raw_c.as<const double>(), in.cov_stride = cov_stride;
     in.normals = raw_n.as<const double>(), in.normal_stride = normal_stride;
+    in.intensities = raw_i.as<const double>();
     in.n = n;
     unsigned int kept = 0;
     B2_TRY(voxel_keys(in.points, point_stride, n, 1.0 / resolution, st, keys, vals, &kept));
     // points that cannot be keyed sort behind every kept one and are dropped
     uint32_t num_voxels = 0;
-    B2_TRY(average_voxels(keys, vals, in, kept, st, avg_p, avg_c, avg_n, &num_voxels));
+    B2_TRY(average_voxels(keys, vals, in, kept, st, avg_p, avg_c, avg_n, avg_i, false, &num_voxels));
     if (num_voxels > 0) {
       avg.points = avg_p.as<const double>();
       if (covs) avg.covs = avg_c.as<const double>();
       if (normals) avg.normals = avg_n.as<const double>();
+      if (intensities) avg.intensities = avg_i.as<const double>();
     }
     avg.n = num_voxels;
   }
@@ -652,15 +787,18 @@ b2_status b2_cloud_create_transformed(const b2_cloud* cloud, const double* T, un
   B2_TRY(check_pose(T, "b2_cloud_create_transformed"));
   B2_ON_DEVICE(cloud->ctx);
   const size_t n = cloud->n, rows = std::max<size_t>(n, 1);  // n == 0: the buffers only mark which arrays the cloud has
-  DeviceBuffer d_p, d_c, d_n;
+  DeviceBuffer d_p, d_c, d_n, d_i;
   B2_TRY(d_p.alloc(rows * 3 * sizeof(double)));
   if (cloud->d_covs) B2_TRY(d_c.alloc(rows * 9 * sizeof(double)));
   if (cloud->d_normals) B2_TRY(d_n.alloc(rows * 3 * sizeof(double)));
+  if (cloud->d_intensities) B2_TRY(d_i.alloc(rows * sizeof(double)));
   if (n > 0) B2_TRY(cloud_arrays_to_device(cloud, cloud->ctx->stream, T, d_p.as<double>(), d_c.as<double>(), d_n.as<double>()));
+  if (n > 0 && cloud->d_intensities) B2_TRY(cloud_intensities_to_device(cloud, cloud->ctx->stream, d_i.as<double>()));  // unposed, as transform() copies them
   RawCloud raw;
   raw.points = d_p.as<const double>(), raw.point_stride = 3;
   raw.covs = d_c.as<const double>(), raw.cov_stride = 9;
   raw.normals = d_n.as<const double>(), raw.normal_stride = 3;
+  raw.intensities = d_i.as<const double>();
   raw.n = n;
   return assemble_cloud(cloud->ctx, raw, flags, nullptr, out, "b2_cloud_create_transformed");
 }
@@ -669,15 +807,15 @@ b2_status b2_merge_frames(b2_ctx* ctx, const double* poses, const b2_cloud* cons
                           double* out_covs, size_t* out_n) {
   B2_REQUIRE(out_n != nullptr, "b2_merge_frames: NULL / empty argument");
   size_t total = 0;
-  bool have_covs = true;
-  B2_TRY(merge_frames_check(ctx, poses, frames, num_frames, downsample_resolution, "b2_merge_frames", &total, &have_covs));
+  bool have_covs = true, have_ints = true;
+  B2_TRY(merge_frames_check(ctx, poses, frames, num_frames, downsample_resolution, "b2_merge_frames", &total, &have_covs, &have_ints));
   *out_n = 0;
   if (total == 0) return B2_OK;
   B2_REQUIRE(out_points != nullptr && (out_covs != nullptr || !have_covs), "b2_merge_frames: output arrays are NULL");
   B2_ON_DEVICE(ctx);
-  DeviceBuffer d_xyz, d_cov;
+  DeviceBuffer d_xyz, d_cov, no_ints;
   size_t m = 0;
-  B2_TRY(merge_frames_device(ctx, poses, frames, num_frames, downsample_resolution, total, have_covs, d_xyz, d_cov, &m));
+  B2_TRY(merge_frames_device(ctx, poses, frames, num_frames, downsample_resolution, total, have_covs, false, d_xyz, d_cov, no_ints, &m));
   cudaStream_t st = ctx->stream;
   B2_CUDA(cudaMemcpyAsync(out_points, d_xyz.get(), m * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
   if (out_covs) B2_CUDA(cudaMemcpyAsync(out_covs, d_cov.get(), m * 9 * sizeof(double), cudaMemcpyDeviceToHost, st));
@@ -688,22 +826,24 @@ b2_status b2_merge_frames(b2_ctx* ctx, const double* poses, const b2_cloud* cons
 
 // b2_merge_frames with the merged points and covariances assembled into a device cloud (assemble_cloud, b2_cloud_create's storage
 // rules for `flags`): the cloud b2_cloud_create makes of b2_merge_frames's output.  It always has covariances (zeros where the
-// frames have none), as that output does; no input points give an empty cloud.
+// frames have none), as that output does; no input points give an empty cloud.  When every frame has intensities, it has the
+// per-voxel maxima of them from 0.0 (merge_frames, gaussian_voxelmap_cpu_funcs.cpp:83-101).
 b2_status b2_merge_frames_to_cloud(b2_ctx* ctx, const double* poses, const b2_cloud* const* frames, size_t num_frames, double downsample_resolution, unsigned flags,
                                    b2_cloud** out) {
   B2_REQUIRE(out != nullptr, "b2_merge_frames_to_cloud: out is NULL");
   *out = nullptr;
   size_t total = 0;
-  bool have_covs = true;
-  B2_TRY(merge_frames_check(ctx, poses, frames, num_frames, downsample_resolution, "b2_merge_frames_to_cloud", &total, &have_covs));
+  bool have_covs = true, have_ints = true;
+  B2_TRY(merge_frames_check(ctx, poses, frames, num_frames, downsample_resolution, "b2_merge_frames_to_cloud", &total, &have_covs, &have_ints));
   B2_ON_DEVICE(ctx);
-  DeviceBuffer d_xyz, d_cov;
+  DeviceBuffer d_xyz, d_cov, d_int;
   size_t m = 0;
-  if (total > 0) B2_TRY(merge_frames_device(ctx, poses, frames, num_frames, downsample_resolution, total, have_covs, d_xyz, d_cov, &m));
+  if (total > 0) B2_TRY(merge_frames_device(ctx, poses, frames, num_frames, downsample_resolution, total, have_covs, have_ints, d_xyz, d_cov, d_int, &m));
   RawCloud raw;
   const double marker = 0.0;  // m == 0: the arrays' presence is marked by a pointer that is never read
   raw.points = m ? d_xyz.as<const double>() : &marker, raw.point_stride = 3;
   raw.covs = m ? d_cov.as<const double>() : &marker, raw.cov_stride = 9;
+  if (have_ints) raw.intensities = m ? d_int.as<const double>() : &marker;
   raw.n = m;
   return assemble_cloud(ctx, raw, flags, nullptr, out, "b2_merge_frames_to_cloud");
 }

@@ -74,7 +74,8 @@ __global__ void inlier_flags_kernel(const double* __restrict__ stats, const doub
 
 // Row r of the new cloud = row K[r] of the input's caller-order arrays (K == NULL: row r); ok (may be NULL) gets K[r] as int64.
 __global__ void gather_rows_kernel(const uint32_t* __restrict__ K, size_t m, const double* __restrict__ p, const double* __restrict__ c, const double* __restrict__ nr,
-                                   double* __restrict__ op, double* __restrict__ oc, double* __restrict__ on, long long* __restrict__ ok) {
+                                   const double* __restrict__ in, double* __restrict__ op, double* __restrict__ oc, double* __restrict__ on, double* __restrict__ oi,
+                                   long long* __restrict__ ok) {
   const size_t r = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
   if (r >= m) return;
   const size_t i = K ? K[r] : r;
@@ -86,21 +87,26 @@ __global__ void gather_rows_kernel(const uint32_t* __restrict__ K, size_t m, con
   if (nr)
 #pragma unroll
     for (int a = 0; a < 3; a++) on[r * 3 + a] = nr[i * 3 + a];
+  if (in) oi[r] = in[i];
   if (ok) ok[r] = static_cast<long long>(i);
 }
 
 unsigned grid_of(size_t n) { return static_cast<unsigned>((n + 255) / 256); }
 
-// The input's stored arrays in caller order (b2_cloud_download's values, on the device): points n x 3, covs n x 9, normals n x 3
-// where the cloud has them.
+// The input's stored arrays in caller order (b2_cloud_download's values, on the device): points n x 3, covs n x 9, normals n x 3,
+// intensities n where the cloud has them.
 struct Rows {
-  DeviceBuffer p, c, n;
+  DeviceBuffer p, c, n, i;
 };
 b2_status cloud_rows(const b2_cloud* cloud, cudaStream_t st, Rows& r) {
   const size_t n = cloud->n;
   B2_TRY(r.p.alloc(n * 3 * sizeof(double)));
   if (cloud->d_covs) B2_TRY(r.c.alloc(n * 9 * sizeof(double)));
   if (cloud->d_normals) B2_TRY(r.n.alloc(n * 3 * sizeof(double)));
+  if (cloud->d_intensities) {
+    B2_TRY(r.i.alloc(n * sizeof(double)));
+    B2_TRY(cloud_intensities_to_device(cloud, st, r.i.as<double>()));
+  }
   return cloud_arrays_to_device(cloud, st, nullptr, r.p.as<double>(), r.c.as<double>(), r.n.as<double>());
 }
 
@@ -110,14 +116,15 @@ b2_status cloud_rows(const b2_cloud* cloud, cudaStream_t st, Rows& r) {
 b2_status assemble_selection(const b2_cloud* cloud, const Rows* rows, const uint32_t* d_K, size_t m, unsigned flags, int64_t* out_indices, b2_cloud** out, const char* who) {
   cudaStream_t st = cloud->ctx->stream;
   const size_t cap = std::max<size_t>(m, 1);
-  DeviceBuffer op, oc, on, ok;
+  DeviceBuffer op, oc, on, oi, ok;
   B2_TRY(op.alloc(cap * 3 * sizeof(double)));
   if (cloud->d_covs) B2_TRY(oc.alloc(cap * 9 * sizeof(double)));
   if (cloud->d_normals) B2_TRY(on.alloc(cap * 3 * sizeof(double)));
+  if (cloud->d_intensities) B2_TRY(oi.alloc(cap * sizeof(double)));
   if (out_indices) B2_TRY(ok.alloc(cap * sizeof(long long)));
   if (m > 0) {
-    gather_rows_kernel<<<grid_of(m), 256, 0, st>>>(d_K, m, rows->p.as<const double>(), rows->c.as<const double>(), rows->n.as<const double>(), op.as<double>(),
-                                                   oc.as<double>(), on.as<double>(), ok.as<long long>());
+    gather_rows_kernel<<<grid_of(m), 256, 0, st>>>(d_K, m, rows->p.as<const double>(), rows->c.as<const double>(), rows->n.as<const double>(), rows->i.as<const double>(),
+                                                   op.as<double>(), oc.as<double>(), on.as<double>(), oi.as<double>(), ok.as<long long>());
     B2_CUDA(cudaGetLastError());
     if (out_indices) B2_CUDA(cudaMemcpyAsync(out_indices, ok.get(), m * sizeof(long long), cudaMemcpyDeviceToHost, st));
   }
@@ -125,6 +132,7 @@ b2_status assemble_selection(const b2_cloud* cloud, const Rows* rows, const uint
   raw.points = op.as<const double>(), raw.point_stride = 3;
   raw.covs = oc.as<const double>(), raw.cov_stride = 9;
   raw.normals = on.as<const double>(), raw.normal_stride = 3;
+  raw.intensities = oi.as<const double>();
   raw.n = m;
   return assemble_cloud(cloud->ctx, raw, flags, nullptr, out, who);  // synchronises the stream: out_indices is written
 }

@@ -297,7 +297,7 @@ struct KdTreeView {
 
 // ---- cloud assembly (b2_cloud.cu) ------------------------------------------------------------------
 // Per-point device arrays in the caller's order, AoS: points n x point_stride, covs n x cov_stride (9 or 16; NULL = none),
-// normals n x normal_stride (3 or 4; NULL = none).
+// normals n x normal_stride (3 or 4; NULL = none), intensities n (NULL = none).
 struct RawCloud {
   const double* points = nullptr;
   int point_stride = 3;
@@ -305,12 +305,13 @@ struct RawCloud {
   int cov_stride = 9;
   const double* normals = nullptr;
   int normal_stride = 3;
+  const double* intensities = nullptr;
   size_t n = 0;
 };
 // Every cloud handle is made here from device arrays: the finite and float32-exactness scans, the Morton permutation, the plane
 // gathers (b2_cloud_create's storage rules for `flags`).  With `like` != NULL the new cloud takes like's point planes, storage
-// type and permutation (device-to-device copies) and raw.points / raw.n are ignored: raw.covs / raw.normals are then per caller
-// index of `like`.  Synchronises the context's stream before it returns, so `raw` may be freed afterwards.  `who` names the entry
+// type and permutation (device-to-device copies) and raw.points / raw.n are ignored: raw.covs / raw.normals / raw.intensities are
+// then per caller index of `like`.  Intensities may be any doubles (NaN and infinities included): they are stored, never computed on.  Synchronises the context's stream before it returns, so `raw` may be freed afterwards.  `who` names the entry
 // point in error messages.
 b2_status assemble_cloud(b2_ctx* ctx, const RawCloud& raw, unsigned flags, const b2_cloud* like, b2_cloud** out, const char* who);
 // The stored arrays of a cloud with n > 0 points as doubles in the caller's order (point i of the storage goes to row perm[i]),
@@ -321,6 +322,9 @@ b2_status assemble_cloud(b2_ctx* ctx, const RawCloud& raw, unsigned flags, const
 // Asynchronous on `st`, which may belong to another context on the cloud's device (a map's): the planes are not written after
 // assemble_cloud returns, so any stream may read them.  The caller's device is the cloud's.
 b2_status cloud_arrays_to_device(const b2_cloud* c, cudaStream_t st, const double* T, double* d_points, double* d_covs, double* d_normals);
+// The stored intensities of a cloud with n > 0 points and intensities, as doubles in the caller's order, into device memory (n
+// entries).  A pose leaves an intensity as it is, so every producer copies them with this.  Asynchronous on `st`, as above.
+b2_status cloud_intensities_to_device(const b2_cloud* c, cudaStream_t st, double* d_out);
 // ---- voxel keys (b2_cloud.cu): voxelgrid_sampling, merge_frames and the RANSAC occupancy test key points alike ----------------
 // Key of a point on the grid of 1 / inv_res: 3 x 21-bit voxel coordinates c = fast_floor(x * inv_res) + 2^20 (x | y << 21 | z << 42),
 // false for a point that cannot be keyed (a non-finite coordinate, or a coordinate outside [0, 2^21 - 1]).  floor() in float64 is
@@ -423,6 +427,7 @@ struct b2_cloud {
   int point_bytes = 0;   // 4 or 8
   int cov_bytes = 0;     // 0, 4 or 8
   int normal_bytes = 0;  // 0, 4 or 8
+  int intensity_bytes = 0;  // 0, 4 or 8
   bool reordered = false;
   // centre of the points' bounding box, 0.5 * (min + max) per axis (0 for an empty cloud): the factor kernels expand the
   // per-correspondence Jacobian about this point so that coordinates far from the cloud's own origin do not cancel
@@ -431,7 +436,10 @@ struct b2_cloud {
   b2::DeviceBuffer d_covs;    // 6 planes (c00, c01, c02, c11, c12, c22) of n_pad elements
   b2::DeviceBuffer d_normals; // 3 planes (nx, ny, nz) of n_pad elements (empty if the cloud has no normals)
   b2::DeviceBuffer d_perm;    // uint32: stored position -> caller index (empty if not reordered)
-  size_t device_bytes() const { return d_points.bytes() + d_covs.bytes() + d_normals.bytes() + d_perm.bytes(); }
+  // 1 plane of n_pad elements in the stored order of the points (empty if the cloud has no intensities).  Kept apart from the
+  // planes above: no factor reads it.
+  b2::DeviceBuffer d_intensities;
+  size_t device_bytes() const { return d_points.bytes() + d_covs.bytes() + d_normals.bytes() + d_perm.bytes() + d_intensities.bytes(); }
 };
 
 // A voxel-keyed map: a bucket table (integer voxel coordinate -> voxel id) over per-voxel arrays in id order.  `slots` is the
@@ -457,10 +465,15 @@ struct b2_voxelmap {
   // a normal (3 doubles); growth, the first insert's layout and the LRU compaction move them with the records
   bool point_state = false;
   b2::DeviceBuffer d_flags, d_normals;
+  // Intensities, double, one per voxel (slots = 0: GaussianVoxel::intensity, the running max) or one per point slot (slots > 0:
+  // FlatContainer::intensities); empty until an insert brings intensities.  Not part of the records: no factor reads them.
+  // Growth, the first insert's layout and the LRU compaction move them with the records.
+  b2::DeviceBuffer d_intensities;
   uint32_t group_mask() const { return static_cast<uint32_t>(num_buckets / b2::kGroup - 1); }  // bucket groups - 1
   b2::VoxelTableView table() const { return {d_buckets.as<const b2::VoxelBucket>(), group_mask(), 0u, inv_resolution}; }
   size_t device_bytes() const {
-    return d_buckets.bytes() + d_records.bytes() + d_coords.bytes() + d_lru.bytes() + d_counts.bytes() + d_flags.bytes() + d_normals.bytes();
+    return d_buckets.bytes() + d_records.bytes() + d_coords.bytes() + d_lru.bytes() + d_counts.bytes() + d_flags.bytes() + d_normals.bytes() +
+           d_intensities.bytes();
   }
 };
 
@@ -480,6 +493,7 @@ struct b2_ivox {
   double min_sq_dist_in_cell = 0.1 * 0.1;  // FlatContainer::Setting (flat_container.hpp:19-23)
   int max_num_points_in_cell = 20;
   int has_covs = -1;                // -1 unknown (nothing inserted yet), 0 / 1: whether inserted points carry covariances
+  int has_intensities = -1;         // the same for intensities (a plain iVox only: a covariance-estimating one keeps none)
   // iVoxCovarianceEstimation (IncrementalCovarianceVoxelMap, ann/incremental_covariance_voxelmap.hpp): fixed at creation.  The
   // records' covariance entries hold the estimated covariances (zero until first estimated); map.point_state is set.
   bool cov_est = false;

@@ -735,13 +735,16 @@ b2_status b2_cloud_create_estimated(const b2_cloud* cloud, const b2_kdtree* tree
     tree = own;
   }
   std::unique_ptr<b2_kdtree, b2_status (*)(b2_kdtree*)> own_guard(own, b2_kdtree_destroy);
-  DeviceBuffer dc, dn;  // at least one entry, so that an empty cloud still has the arrays
+  DeviceBuffer dc, dn, di;  // at least one entry, so that an empty cloud still has the arrays
   B2_TRY(dc.alloc(std::max<size_t>(n, 1) * 9 * sizeof(double)));
   if (with_normals) B2_TRY(dn.alloc(std::max<size_t>(n, 1) * 3 * sizeof(double)));
+  if (cloud->d_intensities) B2_TRY(di.alloc(std::max<size_t>(n, 1) * sizeof(double)));
   if (n > 0) B2_TRY(launch_covariances(tree, k_neighbors, eigen_values, dc.as<double>(), dn.as<double>()));
+  if (n > 0 && cloud->d_intensities) B2_TRY(cloud_intensities_to_device(cloud, cloud->ctx->stream, di.as<double>()));  // kept, as estimate_covariances keeps them
   RawCloud raw;
   raw.covs = dc.as<const double>(), raw.cov_stride = 9;
   raw.normals = dn.as<const double>(), raw.normal_stride = 3;
+  raw.intensities = di.as<const double>();
   return assemble_cloud(cloud->ctx, raw, flags, cloud, out, "b2_cloud_create_estimated");
 }
 

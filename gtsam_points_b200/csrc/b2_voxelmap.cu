@@ -96,9 +96,10 @@ __global__ void batch_voxels_kernel(const double* __restrict__ pts, int pstride,
   is_new[r] = e < 0 ? 1u : 0u;
 }
 
-// The points of one voxel of an inserted batch: pts / covs rows idx[begin..end), in insertion order (covs may be NULL for the iVox).
+// The points of one voxel of an inserted batch: pts / covs / ints rows idx[begin..end), in insertion order (covs may be NULL for the
+// iVox; ints is NULL for a batch without intensities).
 struct CellPoints {
-  const double *pts, *covs;
+  const double *pts, *covs, *ints;
   int pstride, cstride;
   const uint32_t* idx;
   size_t begin, end;
@@ -107,9 +108,11 @@ struct CellPoints {
 // Per-voxel step of the Gaussian voxel map (slots = 0): GaussianVoxel::add for each point in insertion order, then finalize
 // (src/gtsam_points/types/gaussian_voxelmap_cpu.cpp:23-47).  A voxel that already exists is finalized, so add() first re-opens it
 // (mean *= n, cov *= n); the sums then continue from there one point at a time -- exactly the CPU's float64 operation sequence, so
-// means / covariances stay bit-identical over any number of insert() calls.
+// means / covariances stay bit-identical over any number of insert() calls.  With intensities, the voxel's intensity v (0.0 for a new
+// voxel) becomes (v < x) ? x : v for each point's x in the same order: std::max(v, x) of GaussianVoxel::add (:34-36), so NaN and
+// -0.0 never change v and v never drops below 0.  A batch without intensities leaves v as it is.
 struct GaussianCell {
-  __device__ __forceinline__ void add(const CellPoints& b, bool existing, double* __restrict__ records, uint32_t* __restrict__, size_t dest) const {
+  __device__ __forceinline__ void add(const CellPoints& b, bool existing, double* __restrict__ records, uint32_t* __restrict__, double* __restrict__ ints, size_t dest) const {
     double* rec = records + dest * kRecordDoubles;
     double m[3] = {0, 0, 0}, c[6] = {0, 0, 0, 0, 0, 0}, cnt0 = 0.0;
     if (existing) {
@@ -135,16 +138,25 @@ struct GaussianCell {
 #pragma unroll
     for (int k = 0; k < 6; k++) rec[3 + k] = __ddiv_rn(c[k], cnt);
     rec[9] = cnt;
+    if (b.ints) {
+      double v = existing ? ints[dest] : 0.0;
+      for (size_t j = b.begin; j < b.end; j++) {
+        const double x = b.ints[b.idx[j]];
+        v = v < x ? x : v;
+      }
+      ints[dest] = v;
+    }
   }
 };
 
 // Per-voxel step of the iVox (slots > 0): FlatContainer::add (flat_container.hpp:33-50) for each point in insertion order -- rejected
 // if the voxel already holds max_points points or a stored point lies closer than min_sq -- appending the rest to the voxel's slots
-// as records (point | covariance upper | 1).
+// as records (point | covariance upper | 1) and, with intensities, the point's intensity to the slot's entry of `ints`.
 struct FlatCell {
   int slots, max_points;
   double min_sq;
-  __device__ __forceinline__ void add(const CellPoints& b, bool existing, double* __restrict__ records, uint32_t* __restrict__ counts, size_t dest) const {
+  __device__ __forceinline__ void add(const CellPoints& b, bool existing, double* __restrict__ records, uint32_t* __restrict__ counts, double* __restrict__ ints,
+                                      size_t dest) const {
     double* rec = records + dest * static_cast<size_t>(slots) * kRecordDoubles;
     int cnt = existing ? static_cast<int>(counts[dest]) : 0;
     for (size_t j = b.begin; j < b.end && cnt < max_points; j++) {
@@ -161,6 +173,7 @@ struct FlatCell {
         o[3] = o[4] = o[5] = o[6] = o[7] = o[8] = 0.0;
       }
       o[9] = 1.0;
+      if (b.ints) ints[dest * static_cast<size_t>(slots) + cnt] = b.ints[i];
       cnt++;
     }
     counts[dest] = static_cast<uint32_t>(cnt);
@@ -170,11 +183,12 @@ struct FlatCell {
 // Insert (IncrementalVoxelMap::insert, incremental_voxelmap_impl.hpp:31-50): one thread per voxel of the batch runs the cell's
 // per-voxel step over its points, gives a new voxel its coordinate and stamps the voxel's lru -- also when the step took no point.
 template <typename Cell>
-__global__ void insert_voxels_kernel(Cell cell, const double* __restrict__ pts, int pstride, const double* __restrict__ covs, int cstride, size_t n, size_t num_batch,
+__global__ void insert_voxels_kernel(Cell cell, const double* __restrict__ pts, int pstride, const double* __restrict__ covs, int cstride, const double* __restrict__ ints,
+                                     size_t n, size_t num_batch,
                                      const uint32_t* __restrict__ idx, const uint32_t* __restrict__ seg_start, const uint32_t* __restrict__ seg_of_rank,
                                      const int32_t* __restrict__ batch_coords, const int32_t* __restrict__ existing_id, const uint32_t* __restrict__ new_rank,
-                                     size_t num_existing, uint32_t lru_counter, double* __restrict__ records, uint32_t* __restrict__ counts, int32_t* __restrict__ coords,
-                                     uint32_t* __restrict__ lru) {
+                                     size_t num_existing, uint32_t lru_counter, double* __restrict__ records, uint32_t* __restrict__ counts, double* __restrict__ intensities,
+                                     int32_t* __restrict__ coords, uint32_t* __restrict__ lru) {
   const size_t r = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
   if (r >= num_batch) return;
   const uint32_t s = seg_of_rank[r];
@@ -182,7 +196,7 @@ __global__ void insert_voxels_kernel(Cell cell, const double* __restrict__ pts, 
   const size_t end = (s + 1 < num_batch) ? seg_start[s + 1] : n;
   const int e = existing_id[r];
   const size_t dest = e >= 0 ? static_cast<size_t>(e) : num_existing + new_rank[r];  // new voxels: first-touch order after the existing ones
-  cell.add(CellPoints{pts, covs, pstride, cstride, idx, begin, end}, e >= 0, records, counts, dest);
+  cell.add(CellPoints{pts, covs, ints, pstride, cstride, idx, begin, end}, e >= 0, records, counts, intensities, dest);
   if (e < 0) {
 #pragma unroll
     for (int k = 0; k < 3; k++) coords[dest * 3 + k] = batch_coords[r * 3 + k];
@@ -197,12 +211,13 @@ __global__ void lru_keep_flags_kernel(const uint32_t* __restrict__ lru, size_t V
   if (r < V) keep[r] = (static_cast<unsigned long long>(lru[r]) + horizon < counter) ? 0u : 1u;
 }
 // payload: voxel_payload_doubles(slots); counts: the point counts of a map with slots, or nullptr; flags / normals: the point state
-// of a map that keeps it (slots entries per voxel), or nullptr
+// of a map that keeps it (slots entries per voxel), or nullptr; ints: the intensities of a map that has them (max(slots, 1) per
+// voxel), or nullptr
 __global__ void lru_compact_kernel(const uint32_t* __restrict__ keep, const uint32_t* __restrict__ pos, size_t V, size_t payload, int slots, const double* __restrict__ rec_in,
                                    const int32_t* __restrict__ coords_in, const uint32_t* __restrict__ lru_in, const uint32_t* __restrict__ counts_in,
-                                   const unsigned long long* __restrict__ flags_in, const double* __restrict__ normals_in, double* __restrict__ rec_out,
-                                   int32_t* __restrict__ coords_out, uint32_t* __restrict__ lru_out, uint32_t* __restrict__ counts_out, unsigned long long* __restrict__ flags_out,
-                                   double* __restrict__ normals_out) {
+                                   const unsigned long long* __restrict__ flags_in, const double* __restrict__ normals_in, const double* __restrict__ ints_in,
+                                   double* __restrict__ rec_out, int32_t* __restrict__ coords_out, uint32_t* __restrict__ lru_out, uint32_t* __restrict__ counts_out,
+                                   unsigned long long* __restrict__ flags_out, double* __restrict__ normals_out, double* __restrict__ ints_out) {
   const size_t r = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
   if (r >= V || !keep[r]) return;
   const size_t d = pos[r];
@@ -214,6 +229,10 @@ __global__ void lru_compact_kernel(const uint32_t* __restrict__ keep, const uint
   if (flags_in) {
     for (int k = 0; k < slots; k++) flags_out[d * slots + k] = flags_in[r * slots + k];
     for (int k = 0; k < 3 * slots; k++) normals_out[d * 3 * slots + k] = normals_in[r * 3 * slots + k];
+  }
+  if (ints_in) {
+    const int per = slots > 0 ? slots : 1;
+    for (int k = 0; k < per; k++) ints_out[d * per + k] = ints_in[r * per + k];
   }
 }
 
@@ -289,10 +308,13 @@ __global__ void overlap_kernel(const PT* __restrict__ pts, size_t n, size_t n_pa
 size_t bucket_count_for(size_t num_voxels) { return static_cast<size_t>(next_pow2(std::max<uint64_t>(64, 4 * static_cast<uint64_t>(num_voxels)))); }
 
 // The per-voxel arrays of a voxel map: payload records, coordinates, LRU stamps and, iff slots > 0, point counts and, iff the map
-// keeps point state, the flags and normals of its point slots.
+// keeps point state, the flags and normals of its point slots and, iff the map has intensities, max(slots, 1) of them per voxel.
 struct VoxelArrays {
-  DeviceBuffer records, coords, lru, counts, flags, normals;
+  DeviceBuffer records, coords, lru, counts, flags, normals, intensities;
 };
+
+// Intensities per voxel of a map with `slots` point slots per voxel
+inline size_t intensities_per_voxel(int slots) { return static_cast<size_t>(slots > 0 ? slots : 1); }
 
 // Gives the map new per-voxel arrays for `cap` voxels in the layout `slots`.  `fill` runs on them once all are allocated, while the
 // map still holds its current arrays (growth copies from them, the LRU sweep compacts them); the map takes the new arrays only after
@@ -312,9 +334,13 @@ b2_status set_voxel_arrays(b2_voxelmap* vm, size_t cap, int slots, Fill&& fill) 
     B2_CUDA(cudaMemsetAsync(a.flags.get(), 0, a.flags.bytes(), vm->ctx->stream));
     B2_CUDA(cudaMemsetAsync(a.normals.get(), 0, a.normals.bytes(), vm->ctx->stream));
   }
+  if (vm->d_intensities) {  // zeroed as the flags are; `fill` copies or compacts the occupied entries
+    B2_TRY(a.intensities.alloc(cap * intensities_per_voxel(slots) * sizeof(double)));
+    B2_CUDA(cudaMemsetAsync(a.intensities.get(), 0, a.intensities.bytes(), vm->ctx->stream));
+  }
   B2_TRY(fill(a));
   vm->d_records = std::move(a.records), vm->d_coords = std::move(a.coords), vm->d_lru = std::move(a.lru), vm->d_counts = std::move(a.counts);
-  vm->d_flags = std::move(a.flags), vm->d_normals = std::move(a.normals);
+  vm->d_flags = std::move(a.flags), vm->d_normals = std::move(a.normals), vm->d_intensities = std::move(a.intensities);
   vm->capacity = cap;
   vm->slots = slots;
   return B2_OK;
@@ -351,6 +377,8 @@ b2_status reserve_voxels(b2_voxelmap* vm, size_t want) {
         B2_CUDA(cudaMemcpyAsync(a.flags.get(), vm->d_flags.get(), V * vm->slots * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
         B2_CUDA(cudaMemcpyAsync(a.normals.get(), vm->d_normals.get(), V * vm->slots * 3 * sizeof(double), cudaMemcpyDeviceToDevice, st));
       }
+      if (a.intensities)
+        B2_CUDA(cudaMemcpyAsync(a.intensities.get(), vm->d_intensities.get(), V * intensities_per_voxel(vm->slots) * sizeof(double), cudaMemcpyDeviceToDevice, st));
     }
     B2_CUDA(cudaStreamSynchronize(st));
     return B2_OK;
@@ -481,8 +509,8 @@ b2_status compact_voxels(b2_voxelmap* vm, DeviceBuffer& keep, bool* dropped) {
     B2_TRY(set_voxel_arrays(vm, vm->capacity, vm->slots, [&](VoxelArrays& a) -> b2_status {
       lru_compact_kernel<<<g, 256, 0, st>>>(keep.as<uint32_t>(), pos.as<uint32_t>(), V, voxel_payload_doubles(vm->slots), vm->slots, vm->d_records.as<double>(),
                                             vm->d_coords.as<int32_t>(), vm->d_lru.as<uint32_t>(), vm->d_counts.as<uint32_t>(), vm->d_flags.as<unsigned long long>(),
-                                            vm->d_normals.as<double>(), a.records.as<double>(), a.coords.as<int32_t>(), a.lru.as<uint32_t>(), a.counts.as<uint32_t>(),
-                                            a.flags.as<unsigned long long>(), a.normals.as<double>());
+                                            vm->d_normals.as<double>(), vm->d_intensities.as<double>(), a.records.as<double>(), a.coords.as<int32_t>(), a.lru.as<uint32_t>(),
+                                            a.counts.as<uint32_t>(), a.flags.as<unsigned long long>(), a.normals.as<double>(), a.intensities.as<double>());
       B2_CUDA(cudaGetLastError());
       B2_CUDA(cudaStreamSynchronize(st));
       return B2_OK;
@@ -516,10 +544,11 @@ b2_status lru_sweep_and_rebuild(b2_voxelmap* vm) {
 // by first touch), voxels that already exist are found through the table and continued, new ones get the next ids in first-touch
 // order; `cell` is the per-voxel step; then the LRU sweep and the table rebuild.  `slots` is the map's layout, or the one an iVox's
 // first insert gives it.  Every check that can fail runs before the map changes; `on_change` runs when it does.  The map's device
-// is current, and the batch is ready on the map's stream.  `who` names the entry point in error messages.
+// is current, and the batch is ready on the map's stream.  d_ints (n, may be NULL): the batch's intensities; the first batch that
+// has them gives the map its zeroed intensity array.  `who` names the entry point in error messages.
 template <typename Cell, typename OnChange>
 b2_status insert_batch(b2_voxelmap* vm, int slots, const Cell& cell, OnChange&& on_change, const double* d_points, int point_stride, const double* d_covs, int cov_stride,
-                       size_t n, const char* who) {
+                       const double* d_ints, size_t n, const char* who) {
   cudaStream_t st = vm->ctx->stream;
   if (n > 0) {
     const size_t V_old = vm->num_voxels;
@@ -534,12 +563,16 @@ b2_status insert_batch(b2_voxelmap* vm, int slots, const Cell& cell, OnChange&& 
       B2_TRY(set_voxel_arrays(vm, std::max<size_t>(V_new, 1), slots, [](VoxelArrays&) { return B2_OK; }));
     else
       B2_TRY(reserve_voxels(vm, V_new));
+    if (d_ints && !vm->d_intensities) {  // every voxel the map holds so far has intensity 0
+      B2_TRY(vm->d_intensities.alloc(vm->capacity * intensities_per_voxel(vm->slots) * sizeof(double)));
+      B2_CUDA(cudaMemsetAsync(vm->d_intensities.get(), 0, vm->d_intensities.bytes(), st));
+    }
     on_change();
-    insert_voxels_kernel<<<static_cast<unsigned>((sg.B + 127) / 128), 128, 0, st>>>(cell, d_points, point_stride, d_covs, cov_stride, n, sg.B, sg.idx(),
+    insert_voxels_kernel<<<static_cast<unsigned>((sg.B + 127) / 128), 128, 0, st>>>(cell, d_points, point_stride, d_covs, cov_stride, d_ints, n, sg.B, sg.idx(),
                                                                                      sg.seg_start.as<uint32_t>(), sg.seg_of_rank.as<uint32_t>(), sg.batch_coords.as<int32_t>(),
                                                                                      sg.existing_id.as<int32_t>(), sg.new_rank.as<uint32_t>(), V_old, static_cast<uint32_t>(vm->lru_counter),
-                                                                                     vm->d_records.as<double>(), vm->d_counts.as<uint32_t>(), vm->d_coords.as<int32_t>(),
-                                                                                     vm->d_lru.as<uint32_t>());
+                                                                                     vm->d_records.as<double>(), vm->d_counts.as<uint32_t>(), vm->d_intensities.as<double>(),
+                                                                                     vm->d_coords.as<int32_t>(), vm->d_lru.as<uint32_t>());
     B2_CUDA(cudaGetLastError());
     vm->num_voxels = V_new;
     B2_CUDA(cudaStreamSynchronize(st));  // the scratch buffers above are released at scope exit
@@ -547,32 +580,39 @@ b2_status insert_batch(b2_voxelmap* vm, int slots, const Cell& cell, OnChange&& 
   return lru_sweep_and_rebuild(vm);
 }
 
-// insert_batch of host arrays: uploaded, then inserted.
+// insert_batch of host arrays (intensities may be NULL): uploaded, then inserted.
 template <typename Cell, typename OnChange>
 b2_status insert_host(b2_voxelmap* vm, int slots, const Cell& cell, OnChange&& on_change, const double* points, int point_stride, const double* covs, int cov_stride,
-                      size_t n, const char* who) {
-  DeviceBuffer d_p, d_c;
+                      const double* intensities, size_t n, const char* who) {
+  DeviceBuffer d_p, d_c, d_i;
   if (n > 0) {
     B2_TRY(d_p.upload(points, n * point_stride * sizeof(double), vm->ctx->stream));
     if (covs) B2_TRY(d_c.upload(covs, n * cov_stride * sizeof(double), vm->ctx->stream));
+    if (intensities) B2_TRY(d_i.upload(intensities, n * sizeof(double), vm->ctx->stream));
   }
-  return insert_batch(vm, slots, cell, on_change, d_p.as<const double>(), point_stride, d_c.as<const double>(), cov_stride, n, who);
+  return insert_batch(vm, slots, cell, on_change, d_p.as<const double>(), point_stride, d_c.as<const double>(), cov_stride, d_i.as<const double>(), n, who);
 }
 
 // insert_batch of a device cloud posed by T (16 doubles, or NULL: as stored): the cloud's arrays in caller order, posed, as the
-// AoS batch (points n x 3, covariances n x 9 iff with_covs).  The caller has checked the cloud, the pose and the map's rules.  The
-// frame may belong to another context on the map's device: the scatter runs on the MAP's stream, ahead of the segmentation that
-// reads its output there (the frame's planes are immutable once assemble_cloud has returned).
+// AoS batch (points n x 3, covariances n x 9 iff with_covs, intensities n iff with_ints; a pose leaves them as they are).  The
+// caller has checked the cloud, the pose and the map's rules.  The frame may belong to another context on the map's device: the
+// scatter runs on the MAP's stream, ahead of the segmentation that reads its output there (the frame's planes are immutable once
+// assemble_cloud has returned).
 template <typename Cell, typename OnChange>
-b2_status insert_cloud(b2_voxelmap* vm, int slots, const Cell& cell, OnChange&& on_change, const b2_cloud* frame, const double* T, bool with_covs, const char* who) {
+b2_status insert_cloud(b2_voxelmap* vm, int slots, const Cell& cell, OnChange&& on_change, const b2_cloud* frame, const double* T, bool with_covs, bool with_ints,
+                       const char* who) {
   const size_t n = frame->n;
-  DeviceBuffer d_p, d_c;
+  DeviceBuffer d_p, d_c, d_i;
   if (n > 0) {
     B2_TRY(d_p.alloc(n * 3 * sizeof(double)));
     if (with_covs) B2_TRY(d_c.alloc(n * 9 * sizeof(double)));
     B2_TRY(cloud_arrays_to_device(frame, vm->ctx->stream, T, d_p.as<double>(), d_c.as<double>(), nullptr));
+    if (with_ints) {
+      B2_TRY(d_i.alloc(n * sizeof(double)));
+      B2_TRY(cloud_intensities_to_device(frame, vm->ctx->stream, d_i.as<double>()));
+    }
   }
-  return insert_batch(vm, slots, cell, on_change, d_p.as<const double>(), 3, d_c.as<const double>(), 9, n, who);
+  return insert_batch(vm, slots, cell, on_change, d_p.as<const double>(), 3, d_c.as<const double>(), 9, d_i.as<const double>(), n, who);
 }
 
 // The checks every *_insert_cloud makes before the map changes: the frame handle, its device, the pose (NULL allowed).
@@ -908,6 +948,11 @@ extern "C" {
 
 b2_status b2_voxelmap_create_from_voxels(b2_ctx* ctx, double resolution, const int32_t* coords, const double* means, const double* covs,
                                          const int32_t* num_points, size_t V, b2_voxelmap** out) {
+  return b2_voxelmap_create_from_voxels_with_intensities(ctx, resolution, coords, means, covs, num_points, nullptr, V, out);
+}
+
+b2_status b2_voxelmap_create_from_voxels_with_intensities(b2_ctx* ctx, double resolution, const int32_t* coords, const double* means, const double* covs,
+                                                          const int32_t* num_points, const double* intensities, size_t V, b2_voxelmap** out) {
   B2_REQUIRE(out != nullptr, "b2_voxelmap_create_from_voxels: out is NULL");
   *out = nullptr;
   B2_REQUIRE(ctx != nullptr, "b2_voxelmap_create_from_voxels: ctx is NULL");
@@ -950,6 +995,11 @@ b2_status b2_voxelmap_create_from_voxels(b2_ctx* ctx, double resolution, const i
     B2_CUDA(cudaMemcpyAsync(vm->d_records.get(), records.data(), records.size() * sizeof(double), cudaMemcpyHostToDevice, st));
     B2_CUDA(cudaMemcpyAsync(vm->d_coords.get(), coords, V * 3 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   }
+  if (intensities) {  // stored as given, as GaussianVoxelData::uncompact does (gaussian_voxel_data.hpp:44)
+    B2_TRY(vm->d_intensities.alloc(vm->capacity * sizeof(double)));
+    B2_CUDA(cudaMemsetAsync(vm->d_intensities.get(), 0, vm->d_intensities.bytes(), st));
+    if (V > 0) B2_CUDA(cudaMemcpyAsync(vm->d_intensities.get(), intensities, V * sizeof(double), cudaMemcpyHostToDevice, st));
+  }
   vm->num_voxels = V;
   B2_CUDA(cudaStreamSynchronize(st));
   *out = vm.release();
@@ -980,23 +1030,30 @@ b2_status b2_voxelmap_set_lru(b2_voxelmap* vm, size_t lru_horizon, size_t lru_cl
 // IncrementalVoxelMap<GaussianVoxel>::insert on the device (insert_batch).  Deterministic; ids, counts, means and covariances equal
 // the CPU map's.
 b2_status b2_voxelmap_insert(b2_voxelmap* vm, const double* points, int point_stride, const double* covs, int cov_stride, size_t n) {
+  return b2_voxelmap_insert_with_intensities(vm, points, point_stride, covs, cov_stride, nullptr, n);
+}
+
+b2_status b2_voxelmap_insert_with_intensities(b2_voxelmap* vm, const double* points, int point_stride, const double* covs, int cov_stride, const double* intensities,
+                                              size_t n) {
   B2_REQUIRE(vm != nullptr, "b2_voxelmap_insert: vm is NULL");
   B2_REQUIRE(point_stride == 3 || point_stride == 4, "b2_voxelmap_insert: point_stride must be 3 or 4");
   B2_REQUIRE(cov_stride == 9 || cov_stride == 16, "b2_voxelmap_insert: cov_stride must be 9 or 16");
   B2_REQUIRE(n == 0 || (points && covs), "error: points/covs have not been allocated!!");  // GaussianVoxel::add reads covs
   B2_REQUIRE(n < (1ull << 31), "b2_voxelmap_insert: at most 2^31-1 points per insert");
   B2_ON_DEVICE(vm->ctx);
-  return insert_host(vm, 0, GaussianCell{}, [] {}, points, point_stride, covs, cov_stride, n, "b2_voxelmap_insert");
+  return insert_host(vm, 0, GaussianCell{}, [] {}, points, point_stride, covs, cov_stride, intensities, n,
+                     intensities ? "b2_voxelmap_insert_with_intensities" : "b2_voxelmap_insert");
 }
 
 // GaussianVoxelMapGPU::insert(const PointCloud& frame) from the frame's device arrays (gaussian_voxelmap_gpu.cu:211-227), posed by
-// T_map_frame: the same insert_batch as b2_voxelmap_insert over b2_cloud_download's arrays posed by transform().
+// T_map_frame: the same insert_batch as b2_voxelmap_insert over b2_cloud_download's arrays posed by transform(), with the frame's
+// intensities when it has them.
 b2_status b2_voxelmap_insert_cloud(b2_voxelmap* vm, const b2_cloud* frame, const double* T_map_frame) {
   B2_REQUIRE(vm != nullptr, "b2_voxelmap_insert_cloud: vm is NULL");
   B2_TRY(check_insert_cloud(*vm, frame, T_map_frame, "b2_voxelmap_insert_cloud"));
   B2_REQUIRE(frame->n == 0 || frame->d_covs, "b2_voxelmap_insert_cloud: the frame has no covariances");  // GaussianVoxel::add reads covs
   B2_ON_DEVICE(vm->ctx);
-  return insert_cloud(vm, 0, GaussianCell{}, [] {}, frame, T_map_frame, true, "b2_voxelmap_insert_cloud");
+  return insert_cloud(vm, 0, GaussianCell{}, [] {}, frame, T_map_frame, true, static_cast<bool>(frame->d_intensities), "b2_voxelmap_insert_cloud");
 }
 
 b2_status b2_voxelmap_create_from_points(b2_ctx* ctx, double resolution, const double* points, int point_stride, const double* covs, int cov_stride,
@@ -1054,6 +1111,20 @@ b2_status b2_voxelmap_download(const b2_voxelmap* vm, int32_t* coords, double* m
   return B2_OK;
 }
 
+b2_status b2_voxelmap_download_intensities(const b2_voxelmap* vm, double* intensities) {
+  B2_REQUIRE(vm != nullptr && (intensities != nullptr || vm->num_voxels == 0), "b2_voxelmap_download_intensities: NULL argument");
+  const size_t V = vm->num_voxels;
+  if (V == 0) return B2_OK;
+  if (!vm->d_intensities) {  // no insert brought intensities: every voxel holds the initial 0
+    std::fill(intensities, intensities + V, 0.0);
+    return B2_OK;
+  }
+  B2_ON_DEVICE(vm->ctx);
+  B2_CUDA(cudaMemcpyAsync(intensities, vm->d_intensities.get(), V * sizeof(double), cudaMemcpyDeviceToHost, vm->ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(vm->ctx->stream));
+  return B2_OK;
+}
+
 // ---- save_compact / load: the reference's wire format (types/gaussian_voxel_data.hpp:11-54, gaussian_voxelmap_cpu.cpp:79-135) ----
 namespace {
 struct GaussianVoxelData {  // 56 bytes, as in the reference
@@ -1070,15 +1141,16 @@ b2_status b2_voxelmap_save_compact(const b2_voxelmap* vm, const char* path) {
   B2_REQUIRE(vm && path, "b2_voxelmap_save_compact: NULL argument");
   const size_t V = vm->num_voxels;
   std::vector<int32_t> coords(V * 3), cnt(V);
-  std::vector<double> means(V * 3), covs(V * 9);
+  std::vector<double> means(V * 3), covs(V * 9), ints(V);
   B2_TRY(b2_voxelmap_download(vm, coords.data(), means.data(), covs.data(), cnt.data()));
+  B2_TRY(b2_voxelmap_download_intensities(vm, ints.data()));
   std::vector<GaussianVoxelData> serial(V);
   for (size_t r = 0; r < V; r++) {
     GaussianVoxelData& d = serial[r];
     for (int k = 0; k < 3; k++) d.coord[k] = coords[r * 3 + k], d.mean[k] = static_cast<float>(means[r * 3 + k]);
     d.num_points = cnt[r];
     cov_upper(&covs[r * 9], 9, d.cov);
-    d.intensity = 0.0f;  // intensities are not part of the scan-matching path
+    d.intensity = static_cast<float>(ints[r]);
   }
   std::FILE* fp = std::fopen(path, "wb");
   if (!fp) return fail(B2_ERR_INVALID_ARGUMENT, "b2_voxelmap_save_compact: cannot open %s", path);
@@ -1114,14 +1186,19 @@ b2_status b2_voxelmap_load(b2_ctx* ctx, const char* path, b2_voxelmap** out) {
   std::fclose(fp);
   if (rd != V) return fail(B2_ERR_INVALID_ARGUMENT, "b2_voxelmap_load: %s is truncated (%zu of %zu voxels)", path, rd, V);
   std::vector<int32_t> coords(V * 3), cnt(V);
-  std::vector<double> means(V * 3), covs(V * 9);
+  std::vector<double> means(V * 3), covs(V * 9), ints(V);
+  bool any_intensity = false;  // a file of zero intensities loads as a map that has none, as it did before maps kept them
   for (size_t r = 0; r < V; r++) {  // GaussianVoxelData::uncompact (gaussian_voxel_data.hpp:27-46)
     const GaussianVoxelData& d = serial[r];
     for (int k = 0; k < 3; k++) coords[r * 3 + k] = d.coord[k], means[r * 3 + k] = d.mean[k];
     cnt[r] = d.num_points;
     cov_full(d.cov, &covs[r * 9]);
+    ints[r] = d.intensity;
+    uint32_t bits;
+    std::memcpy(&bits, &d.intensity, sizeof(bits));
+    any_intensity = any_intensity || bits != 0u;  // -0.0f too, so that it is written back as it was read
   }
-  B2_TRY(b2_voxelmap_create_from_voxels(ctx, resolution, coords.data(), means.data(), covs.data(), cnt.data(), V, out));
+  B2_TRY(b2_voxelmap_create_from_voxels_with_intensities(ctx, resolution, coords.data(), means.data(), covs.data(), cnt.data(), any_intensity ? ints.data() : nullptr, V, out));
   (*out)->lru_counter = lru_count, (*out)->lru_clear_cycle = lru_cycle ? lru_cycle : 10, (*out)->lru_horizon = lru_thresh;
   return B2_OK;
 }
@@ -1206,7 +1283,9 @@ b2_status b2_ivox_clear(b2_ivox* iv) {
   B2_ON_DEVICE(iv->map.ctx);
   iv->map.num_voxels = 0;  // incremental_voxelmap_impl.hpp:24-28
   iv->map.lru_counter = 0;
-  iv->has_covs = -1;  // the next insert decides again whether the map holds covariances (the slot layout is kept)
+  iv->has_covs = -1;  // the next insert decides again whether the map holds covariances and intensities (the slot layout is kept)
+  iv->has_intensities = -1;
+  iv->map.d_intensities.reset();
   if (iv->cov_est) {  // IncrementalCovarianceVoxelMap::clear: the ring too; slots reused later must read as unborn
     for (b2_eig_stats& r : iv->ring) r = b2_eig_stats{};
     if (iv->map.d_flags) {
@@ -1248,6 +1327,17 @@ b2_status b2_ivox_set_insertion_setting(b2_ivox* iv, double min_dist_in_cell, in
 }
 
 b2_status b2_ivox_insert(b2_ivox* iv, const double* points, int point_stride, const double* covs, int cov_stride, size_t n) {
+  return b2_ivox_insert_with_intensities(iv, points, point_stride, covs, cov_stride, nullptr, n);
+}
+
+// The check of b2_ivox_insert_with_intensities and b2_ivox_insert_cloud: a plain iVox holds intensities for all its points or none.
+static b2_status check_ivox_intensities(const b2_ivox* iv, bool with_ints, size_t n, const char* who) {
+  B2_REQUIRE(iv->cov_est || n == 0 || iv->has_intensities < 0 || iv->has_intensities == (with_ints ? 1 : 0),
+             "%s: the map holds points %s intensities; inserts cannot mix both", who, iv->has_intensities ? "with" : "without");
+  return B2_OK;
+}
+
+b2_status b2_ivox_insert_with_intensities(b2_ivox* iv, const double* points, int point_stride, const double* covs, int cov_stride, const double* intensities, size_t n) {
   B2_REQUIRE(iv != nullptr, "b2_ivox_insert: ivox is NULL");
   B2_REQUIRE(point_stride == 3 || point_stride == 4, "b2_ivox_insert: point_stride must be 3 or 4");
   B2_REQUIRE(covs == nullptr || cov_stride == 9 || cov_stride == 16, "b2_ivox_insert: cov_stride must be 9 or 16");
@@ -1256,29 +1346,35 @@ b2_status b2_ivox_insert(b2_ivox* iv, const double* points, int point_stride, co
   const int with_covs = covs != nullptr ? 1 : 0;
   B2_REQUIRE(iv->cov_est || n == 0 || iv->has_covs < 0 || iv->has_covs == with_covs, "b2_ivox_insert: the map holds points %s covariances; inserts cannot mix both",
              iv->has_covs ? "with" : "without");
+  const char* who = intensities ? "b2_ivox_insert_with_intensities" : "b2_ivox_insert";
+  B2_TRY(check_ivox_intensities(iv, intensities != nullptr, n, who));
   B2_ON_DEVICE(iv->map.ctx);
   const int slots = iv->map.slots > 0 ? iv->map.slots : iv->max_num_points_in_cell;  // the first insert fixes the slot layout
   const FlatCell cell{slots, iv->max_num_points_in_cell, iv->min_sq_dist_in_cell};
-  if (iv->cov_est)  // input covariances are ignored: the map estimates its own
-    return cov_est_insert(iv, [&] { return insert_host(&iv->map, slots, cell, [] {}, points, point_stride, nullptr, 9, n, "b2_ivox_insert"); });
-  return insert_host(&iv->map, slots, cell, [&] { iv->has_covs = with_covs; }, points, point_stride, covs, cov_stride, n, "b2_ivox_insert");
+  if (iv->cov_est)  // input covariances and intensities are ignored: the map estimates its own covariances and keeps no intensities
+    return cov_est_insert(iv, [&] { return insert_host(&iv->map, slots, cell, [] {}, points, point_stride, nullptr, 9, nullptr, n, who); });
+  const int with_ints = intensities != nullptr ? 1 : 0;
+  return insert_host(&iv->map, slots, cell, [&] { iv->has_covs = with_covs, iv->has_intensities = with_ints; }, points, point_stride, covs, cov_stride, intensities, n, who);
 }
 
 // IncrementalVoxelMap<FlatContainer>::insert of a device frame posed by T_map_frame (advanced_scan_matching.cpp:84-95: transform the
 // aligned frame into the map, insert it): b2_ivox_insert over b2_cloud_download's arrays posed by transform().  The frame's
-// covariances go in iff it has them, under b2_ivox_insert's rule that all inserts into one map agree.
+// covariances and intensities go in iff it has them, under b2_ivox_insert's rule that all inserts into one map agree.
 b2_status b2_ivox_insert_cloud(b2_ivox* iv, const b2_cloud* frame, const double* T_map_frame) {
   B2_REQUIRE(iv != nullptr, "b2_ivox_insert_cloud: ivox is NULL");
   B2_TRY(check_insert_cloud(iv->map, frame, T_map_frame, "b2_ivox_insert_cloud"));
   const int with_covs = frame->d_covs ? 1 : 0;
   B2_REQUIRE(iv->cov_est || frame->n == 0 || iv->has_covs < 0 || iv->has_covs == with_covs,
              "b2_ivox_insert_cloud: the map holds points %s covariances; inserts cannot mix both", iv->has_covs ? "with" : "without");
+  const int with_ints = frame->d_intensities ? 1 : 0;
+  B2_TRY(check_ivox_intensities(iv, with_ints != 0, frame->n, "b2_ivox_insert_cloud"));
   B2_ON_DEVICE(iv->map.ctx);
   const int slots = iv->map.slots > 0 ? iv->map.slots : iv->max_num_points_in_cell;
   const FlatCell cell{slots, iv->max_num_points_in_cell, iv->min_sq_dist_in_cell};
   if (iv->cov_est)
-    return cov_est_insert(iv, [&] { return insert_cloud(&iv->map, slots, cell, [] {}, frame, T_map_frame, false, "b2_ivox_insert_cloud"); });
-  return insert_cloud(&iv->map, slots, cell, [&] { iv->has_covs = with_covs; }, frame, T_map_frame, with_covs != 0, "b2_ivox_insert_cloud");
+    return cov_est_insert(iv, [&] { return insert_cloud(&iv->map, slots, cell, [] {}, frame, T_map_frame, false, false, "b2_ivox_insert_cloud"); });
+  return insert_cloud(&iv->map, slots, cell, [&] { iv->has_covs = with_covs, iv->has_intensities = with_ints; }, frame, T_map_frame, with_covs != 0, with_ints != 0,
+                      "b2_ivox_insert_cloud");
 }
 
 b2_status b2_ivox_get_info(const b2_ivox* iv, b2_ivox_info* info) {
@@ -1321,6 +1417,27 @@ b2_status b2_ivox_download(const b2_ivox* iv, int32_t* coords, int32_t* counts, 
       if (covs) cov_full(q + 3, covs + o * 9);
     }
   }
+  return B2_OK;
+}
+
+b2_status b2_ivox_download_intensities(const b2_ivox* iv, double* intensities) {
+  B2_REQUIRE(iv != nullptr, "b2_ivox_download_intensities: ivox is NULL");
+  if (iv->cov_est) return fail(B2_ERR_INVALID_STATE, "b2_ivox_download_intensities: an iVoxCovarianceEstimation keeps no intensities");
+  if (iv->has_intensities == 0) return fail(B2_ERR_INVALID_STATE, "b2_ivox_download_intensities: the map holds points without intensities");
+  const b2_voxelmap* vm = &iv->map;
+  const size_t V = vm->num_voxels;
+  if (V == 0) return B2_OK;  // nothing stored (has_intensities < 0 only while the map is empty)
+  B2_REQUIRE(intensities != nullptr, "b2_ivox_download_intensities: NULL argument");
+  B2_ON_DEVICE(vm->ctx);
+  cudaStream_t st = vm->ctx->stream;
+  std::vector<uint32_t> cnt(V);
+  std::vector<double> all(V * vm->slots);
+  B2_CUDA(cudaMemcpyAsync(cnt.data(), vm->d_counts.get(), V * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(all.data(), vm->d_intensities.get(), all.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  size_t o = 0;
+  for (size_t v = 0; v < V; v++)
+    for (uint32_t s = 0; s < cnt[v]; s++) intensities[o++] = all[v * vm->slots + s];
   return B2_OK;
 }
 

@@ -57,14 +57,18 @@ def default_context(device: int = 0) -> Context:
 
 
 class PointCloud:
-    """Points (N x 3 or N x 4 float64) with optional covariances (N x 3 x 3 or N x 4 x 4 float64) and normals (N x 3 or N x 4).
+    """Points (N x 3 or N x 4 float64) with optional covariances (N x 3 x 3 or N x 4 x 4 float64), normals (N x 3 or N x 4) and
+    intensities (N).
 
-    The device copy (`points_gpu` / `covs_gpu` / `normals_gpu` in the reference) is created on construction.
+    The device copy (`points_gpu` / `covs_gpu` / `normals_gpu` / `intensities_gpu` in the reference) is created on construction.
     flags: capi.B2_CLOUD_* (default lossless storage, Morton-ordered on the device).
     """
 
-    def __init__(self, points, covs=None, ctx: Context | None = None, flags: int = capi.B2_CLOUD_DEFAULT, normals=None):
+    def __init__(self, points, covs=None, ctx: Context | None = None, flags: int = capi.B2_CLOUD_DEFAULT, normals=None, intensities=None):
         self.ctx = ctx or default_context()
+        self.intensities = None if intensities is None else np.ascontiguousarray(intensities, dtype=np.float64)
+        if self.intensities is not None and (self.intensities.ndim != 1 or len(self.intensities) != len(points)):
+            raise ValueError("intensities must be N values, one per point")
         self.normals = None if normals is None else np.ascontiguousarray(normals, dtype=np.float64)
         if self.normals is not None and (self.normals.ndim != 2 or self.normals.shape[1] not in (3, 4) or len(self.normals) != len(points)):
             raise ValueError("normals must be N x 3 or N x 4, one per point")
@@ -87,17 +91,18 @@ class PointCloud:
             self.covs = covs
         h = C.c_void_p()
         capi.check(
-            capi.lib().b2_cloud_create_with_normals(
+            capi.lib().b2_cloud_create_with_intensities(
                 self.ctx.h, capi.dptr(self.points), self.points.shape[1], capi.dptr(self.covs) if self.covs is not None else None, cov_stride,
-                capi.dptr(self.normals) if self.normals is not None else None, 0 if self.normals is None else self.normals.shape[1], len(self.points), flags, C.byref(h)
+                capi.dptr(self.normals) if self.normals is not None else None, 0 if self.normals is None else self.normals.shape[1],
+                None if self.intensities is None else capi.dptr(self.intensities), len(self.points), flags, C.byref(h)
             )
         )
         self.h = h
 
     @classmethod
     def _from_handle(cls, h, ctx: Context) -> "PointCloud":
-        """Wraps a device cloud the library created (voxel grid, estimation): .points / .covs / .normals are its stored values in
-        caller order (b2_cloud_download), so every consumer of a PointCloud takes it as it is."""
+        """Wraps a device cloud the library created (voxel grid, estimation): .points / .covs / .normals / .intensities are its stored
+        values in caller order (b2_cloud_download), so every consumer of a PointCloud takes it as it is."""
         self = cls.__new__(cls)
         self.ctx, self.h = ctx, h
         info = self.info()
@@ -107,13 +112,15 @@ class PointCloud:
         self.normals = np.zeros((n, 3)) if info.normal_bytes else None
         capi.check(capi.lib().b2_cloud_download(h, capi.dptr(self.points), None if self.covs is None else capi.dptr(self.covs), None if self.normals is None else capi.dptr(self.normals)))
         self._device_normals = self.normals
+        self.intensities = self.intensities_gpu() if self.intensity_bytes() else None
         return self
 
     def estimated(self, k_neighbors: int = 10, eigen_values=(1e-3, 1.0, 1.0), normals: bool = False, tree: "KdTree | None" = None,
                   flags: int = capi.B2_CLOUD_DEFAULT) -> "PointCloud":
         """A new device cloud with these points and the covariances of estimate_covariances over them (features/covariance_estimation.cpp:
         18-77), with normals=True also the normals of estimate_normals from the same neighbour search; the points never leave the
-        device.  tree: None builds one; else a KdTree.from_cloud(self).  flags pick the storage of the estimated arrays."""
+        device; intensities, if the cloud has them, are kept.  tree: None builds one; else a KdTree.from_cloud(self).  flags pick the
+        storage of the estimated arrays and of the intensities."""
         ev = np.ascontiguousarray(eigen_values, dtype=np.float64)
         h = C.c_void_p()
         capi.check(capi.lib().b2_cloud_create_estimated(self.h, None if tree is None else tree.h, int(k_neighbors), capi.dptr(ev), 1 if normals else 0, flags, C.byref(h)))
@@ -138,6 +145,21 @@ class PointCloud:
         """The normals as stored on the device (after any float32 rounding), N x 3 in the caller's order."""
         out = np.zeros((len(self.points), 3))
         capi.check(capi.lib().b2_cloud_download_normals(self.h, capi.dptr(out)))
+        return out
+
+    def has_intensities(self):
+        return self.intensities is not None
+
+    def intensity_bytes(self) -> int:
+        """Storage of the device copy's intensities: 4 or 8 bytes, 0 = none."""
+        out = C.c_int()
+        capi.check(capi.lib().b2_cloud_intensity_bytes(self.h, C.byref(out)))
+        return out.value
+
+    def intensities_gpu(self) -> np.ndarray:
+        """The intensities as stored on the device (after any float32 rounding), N values in the caller's order."""
+        out = np.zeros(len(self.points))
+        capi.check(capi.lib().b2_cloud_download_intensities(self.h, capi.dptr(out)))
         return out
 
     def info(self) -> capi.CloudInfo:
@@ -169,12 +191,15 @@ class GaussianVoxelMapGPU:
     def insert(self, frame: PointCloud):
         """GaussianVoxelMap::insert(const PointCloud&).  The first call builds the map; further calls are incremental with the
         CPU map's semantics (IncrementalVoxelMap::insert + LRU eviction, ann/impl/incremental_voxelmap_impl.hpp:31-68) -- the
-        reference's own GPU map is one-shot only (types/gaussian_voxelmap_gpu.hpp:63)."""
+        reference's own GPU map is one-shot only (types/gaussian_voxelmap_gpu.hpp:63).  The frame's intensities, if it has them,
+        raise each voxel's intensity to their maximum (voxel_intensities())."""
         if frame.covs is None:
             raise ValueError("GaussianVoxelMapGPU.insert: the frame has no covariances")
         cov_stride = 9 if frame.covs.shape[1:] == (3, 3) else 16
         self._ensure()
-        capi.check(capi.lib().b2_voxelmap_insert(self.h, capi.dptr(frame.points), frame.points.shape[1], capi.dptr(frame.covs), cov_stride, len(frame.points)))
+        ints = getattr(frame, "intensities", None)
+        capi.check(capi.lib().b2_voxelmap_insert_with_intensities(self.h, capi.dptr(frame.points), frame.points.shape[1], capi.dptr(frame.covs), cov_stride,
+                                                                  None if ints is None else capi.dptr(ints), len(frame.points)))
 
     def insert_cloud(self, cloud: PointCloud, T=None):
         """insert() of a device cloud posed by T (map <- frame 4x4; None: as stored) without a host copy: the map afterwards equals
@@ -214,17 +239,22 @@ class GaussianVoxelMapGPU:
         return self
 
     @classmethod
-    def from_voxels(cls, resolution, coords, means, covs, num_points=None, ctx: Context | None = None):
-        """Upload an existing map (e.g. the contents of a GaussianVoxelMapCPU); ids = the given order."""
+    def from_voxels(cls, resolution, coords, means, covs, num_points=None, ctx: Context | None = None, intensities=None):
+        """Upload an existing map (e.g. the contents of a GaussianVoxelMapCPU); ids = the given order.  intensities: each voxel's
+        intensity (None: 0)."""
         self = cls(resolution, ctx)
         coords = np.ascontiguousarray(coords, dtype=np.int32)
         means = np.ascontiguousarray(means, dtype=np.float64)
         covs = np.ascontiguousarray(covs, dtype=np.float64).reshape(len(coords), 9)
         npts = None if num_points is None else np.ascontiguousarray(num_points, dtype=np.int32)
+        ints = None if intensities is None else np.ascontiguousarray(intensities, dtype=np.float64)
+        if ints is not None and ints.shape != (len(coords),):
+            raise ValueError("intensities must hold one value per voxel")
         h = C.c_void_p()
         capi.check(
-            capi.lib().b2_voxelmap_create_from_voxels(
-                self.ctx.h, float(resolution), coords.ctypes.data_as(C.POINTER(C.c_int32)), capi.dptr(means), capi.dptr(covs), None if npts is None else npts.ctypes.data_as(C.POINTER(C.c_int32)), len(coords), C.byref(h)
+            capi.lib().b2_voxelmap_create_from_voxels_with_intensities(
+                self.ctx.h, float(resolution), coords.ctypes.data_as(C.POINTER(C.c_int32)), capi.dptr(means), capi.dptr(covs), None if npts is None else npts.ctypes.data_as(C.POINTER(C.c_int32)),
+                None if ints is None else capi.dptr(ints), len(coords), C.byref(h)
             )
         )
         self.h = h
@@ -248,6 +278,13 @@ class GaussianVoxelMapGPU:
         n = np.zeros(V, dtype=np.int32)
         capi.check(capi.lib().b2_voxelmap_download(self.h, coords.ctypes.data_as(C.POINTER(C.c_int32)), capi.dptr(means), capi.dptr(covs), n.ctypes.data_as(C.POINTER(C.c_int32))))
         return dict(coords=coords, means=means, covs=covs, n=n, resolution=self._resolution)
+
+    def voxel_intensities(self) -> np.ndarray:
+        """Each voxel's intensity in id order: the maximum, from 0.0, of the intensities of the points inserted into it
+        (GaussianVoxel::intensity); all 0 for a map that never received intensities."""
+        out = np.zeros(self.num_voxels)
+        capi.check(capi.lib().b2_voxelmap_download_intensities(self.h, capi.dptr(out)))
+        return out
 
     def lookup_voxel_index(self, points) -> np.ndarray:
         """voxel_coord + lookup_voxel_index for a batch of points; -1 where no voxel exists."""
@@ -285,22 +322,28 @@ class iVox:
     def voxel_resolution(self) -> float:
         return self._resolution
 
-    def insert(self, frame, covs=None):
+    def insert(self, frame, covs=None, intensities=None):
         """IncrementalVoxelMap::insert(const PointCloud&) (ann/impl/incremental_voxelmap_impl.hpp:31-68).  `frame`: a PointCloud, or
-        an N x 3 / N x 4 array with optional N x 3 x 3 / N x 4 x 4 `covs`; covariances are stored with the points when given
-        (all inserts into one map must agree)."""
+        an N x 3 / N x 4 array with optional N x 3 x 3 / N x 4 x 4 `covs` and N `intensities`; covariances and intensities are
+        stored with the points when given (all inserts into one map must agree on each)."""
         pts = frame.points if isinstance(frame, PointCloud) else np.ascontiguousarray(frame, dtype=np.float64)
         if isinstance(frame, PointCloud):
-            covs = frame.covs
-        elif covs is not None:
-            covs = np.ascontiguousarray(covs, dtype=np.float64)
+            covs, intensities = frame.covs, frame.intensities
+        else:
+            if covs is not None:
+                covs = np.ascontiguousarray(covs, dtype=np.float64)
+            if intensities is not None:
+                intensities = np.ascontiguousarray(intensities, dtype=np.float64)
+                if intensities.shape != (len(pts),):
+                    raise ValueError("intensities must be N values, one per point")
         cov_stride = 0 if covs is None else (9 if covs.shape[1:] == (3, 3) else 16)
-        capi.check(capi.lib().b2_ivox_insert(self.h, capi.dptr(pts), pts.shape[1], capi.dptr(covs) if covs is not None else None, cov_stride, len(pts)))
+        capi.check(capi.lib().b2_ivox_insert_with_intensities(self.h, capi.dptr(pts), pts.shape[1], capi.dptr(covs) if covs is not None else None, cov_stride,
+                                                              None if intensities is None else capi.dptr(intensities), len(pts)))
 
     def insert_cloud(self, cloud: PointCloud, T=None):
         """insert() of a device cloud posed by T (map <- frame 4x4; None: as stored) without a host copy -- the map update of
         frame-to-map odometry (advanced_scan_matching.cpp:84-95) in one call.  The map afterwards equals insert() of the cloud's
-        stored values posed as transform_gpu() poses them (b2_ivox_insert_cloud); its covariances go in iff it has them."""
+        stored values posed as transform_gpu() poses them (b2_ivox_insert_cloud); its covariances and intensities go in iff it has them."""
         T16 = _pose16(T)
         capi.check(capi.lib().b2_ivox_insert_cloud(self.h, cloud.h, None if T16 is None else capi.dptr(T16)))
 
@@ -359,6 +402,13 @@ class iVox:
         """iVox::voxel_points(): every stored point, voxels in id order, points in slot order (N x 4, w = 1)."""
         p = self.download()["points"]
         return np.concatenate([p, np.ones((len(p), 1))], 1)
+
+    def voxel_intensities(self) -> np.ndarray:
+        """iVox::voxel_intensities(): the stored points' intensities in voxel_points() order.  Raises on a map whose points came
+        without intensities, and on an iVoxCovarianceEstimation, which keeps none."""
+        out = np.zeros(self.size())
+        capi.check(capi.lib().b2_ivox_download_intensities(self.h, capi.dptr(out)))
+        return out
 
     def voxel_covs(self) -> np.ndarray:
         """iVox::voxel_covs(): the stored covariances in voxel_points() order (N x 4 x 4)."""
@@ -534,10 +584,11 @@ def merge_frames_gpu(poses, frames, downsample_resolution: float, ctx: "Context 
     return PointCloud(xyz[: m.value].copy(), cov[: m.value].reshape(-1, 3, 3).copy(), ctx=ctx)
 
 
-def voxelgrid_sampling(points, resolution: float, covs=None, normals=None, ctx: Context | None = None, flags: int = capi.B2_CLOUD_DEFAULT) -> PointCloud:
+def voxelgrid_sampling(points, resolution: float, covs=None, normals=None, ctx: Context | None = None, flags: int = capi.B2_CLOUD_DEFAULT,
+                       intensities=None) -> PointCloud:
     """voxelgrid_sampling (types/point_cloud_cpu.hpp:136) of a host scan into a device cloud: one point per occupied voxel of
     `resolution`, in ascending voxel-key order, each value the mean of the voxel's points in input order (covs N x 3 x 3 /
-    N x 4 x 4 and normals N x 3 / N x 4 averaged alongside).  Points with a non-finite coordinate or outside the 21-bit voxel
+    N x 4 x 4, normals N x 3 / N x 4 and intensities N averaged alongside).  Points with a non-finite coordinate or outside the 21-bit voxel
     key range are dropped.  flags: capi.B2_CLOUD_* storage of the result.  See b2_cloud_create_voxelgrid for the differences from
     the reference."""
     ctx = ctx or default_context()
@@ -555,11 +606,15 @@ def voxelgrid_sampling(points, resolution: float, covs=None, normals=None, ctx: 
         if normals.ndim != 2 or normals.shape[1] not in (3, 4) or len(normals) != len(p):
             raise ValueError("normals must be N x 3 or N x 4, one per point")
         nrm_stride = normals.shape[1]
+    if intensities is not None:
+        intensities = np.ascontiguousarray(intensities, dtype=np.float64)
+        if intensities.shape != (len(p),):
+            raise ValueError("intensities must be N values, one per point")
     h = C.c_void_p()
     capi.check(
-        capi.lib().b2_cloud_create_voxelgrid(
+        capi.lib().b2_cloud_create_voxelgrid_with_intensities(
             ctx.h, float(resolution), capi.dptr(p), p.shape[1], None if covs is None else capi.dptr(covs), cov_stride, None if normals is None else capi.dptr(normals),
-            nrm_stride, len(p), flags, C.byref(h)
+            nrm_stride, None if intensities is None else capi.dptr(intensities), len(p), flags, C.byref(h)
         )
     )
     return PointCloud._from_handle(h, ctx)

@@ -134,6 +134,27 @@ B2_API b2_status b2_cloud_create(b2_ctx* ctx, const double* points, int point_st
  * b2_icp_factor_create (target cloud). */
 B2_API b2_status b2_cloud_create_with_normals(b2_ctx* ctx, const double* points, int point_stride, const double* covs, int cov_stride,
                                               const double* normals, int normal_stride, size_t n, unsigned flags, b2_cloud** out);
+/* The same with per-point intensities (PointCloud::intensities, point_cloud.hpp:109; uploaded like PointCloudGPU::add_intensities,
+ * point_cloud_gpu.hpp:113-119): n doubles in caller order, any values (NaN and infinities included: they are stored, never computed
+ * on).  They are kept in the stored (Morton) order of the points in an array of their own that no factor reads, float32 when every
+ * value is exactly float32-representable (NaN is not) and float64 otherwise; B2_CLOUD_COMPACT_F32 / B2_CLOUD_FORCE_F64 apply.
+ * intensities == NULL is b2_cloud_create_with_normals.  Every producer of a device cloud carries them when its input has them:
+ * b2_cloud_create_transformed copies them unchanged (transform(), point_cloud_cpu_funcs.cpp:469-488), the samplers and
+ * b2_cloud_create_inliers gather them, b2_cloud_create_voxelgrid_with_intensities averages them, b2_merge_frames_to_cloud keeps the
+ * per-voxel maximum, b2_cloud_create_estimated keeps them (estimate_covariances leaves a frame's intensities in place); each result
+ * stores them under its own `flags` by the rule above. */
+B2_API b2_status b2_cloud_create_with_intensities(b2_ctx* ctx, const double* points, int point_stride, const double* covs, int cov_stride,
+                                                  const double* normals, int normal_stride, const double* intensities, size_t n, unsigned flags,
+                                                  b2_cloud** out);
+/* PointCloudGPU::add_intensities as a NEW cloud, the input untouched (factors and trees may hold it): the input's stored points,
+ * covariances and normals, Morton order and bounding-box centre, copied on the device as they are, with `intensities` (n doubles,
+ * caller order) stored by the rule above under `flags` (B2_CLOUD_COMPACT_F32 / B2_CLOUD_FORCE_F64; nothing else applies).  The
+ * input's own intensities, if any, are not carried over.  So every factor computes on the new cloud what it computes on the input. */
+B2_API b2_status b2_cloud_create_with_added_intensities(const b2_cloud* cloud, const double* intensities, unsigned flags, b2_cloud** out);
+/* *out = the storage of the cloud's intensities: 4 or 8 bytes, 0 = none */
+B2_API b2_status b2_cloud_intensity_bytes(const b2_cloud* cloud, int* out);
+/* The stored intensities (after any float32 rounding) in caller order: host, n doubles.  B2_ERR_INVALID_STATE if the cloud has none. */
+B2_API b2_status b2_cloud_download_intensities(const b2_cloud* cloud, double* out_intensities);
 /* The stored normals as the kernels read them (after any float32 rounding): host, n x 3, caller order.
  * B2_ERR_INVALID_STATE if the cloud has none. */
 B2_API b2_status b2_cloud_download_normals(const b2_cloud* cloud, double* out_normals);
@@ -157,6 +178,12 @@ B2_API b2_status b2_cloud_download(const b2_cloud* cloud, double* out_points, do
  * dropped.  (Its w component enters its range test only for resolution < ~1e-6; not reproduced.) */
 B2_API b2_status b2_cloud_create_voxelgrid(b2_ctx* ctx, double resolution, const double* points, int point_stride, const double* covs, int cov_stride,
                                            const double* normals, int normal_stride, size_t n, unsigned flags, b2_cloud** out);
+/* The same with per-point intensities (n doubles, may be NULL): each voxel's intensity is the float64 sum of its kept points'
+ * intensities in caller order divided by their count, as the other arrays are averaged (voxelgrid_sampling's Averager,
+ * point_cloud_cpu_funcs.cpp:237-242), stored as b2_cloud_create_with_intensities stores them. */
+B2_API b2_status b2_cloud_create_voxelgrid_with_intensities(b2_ctx* ctx, double resolution, const double* points, int point_stride, const double* covs,
+                                                            int cov_stride, const double* normals, int normal_stride, const double* intensities, size_t n,
+                                                            unsigned flags, b2_cloud** out);
 /* transform(frame, T) (src/gtsam_points/types/point_cloud_cpu_funcs.cpp:469-488) of a device cloud into a NEW device cloud, without a
  * host copy.  T: 16 doubles, row-major 4x4, every entry finite; only its rigid part [R | t] is read.  The new cloud's caller index i
  * is the input's caller index i, and it has covariances / normals iff the input has them:
@@ -190,6 +217,16 @@ B2_API b2_status b2_voxelmap_create_from_points(b2_ctx* ctx, double resolution, 
 B2_API b2_status b2_voxelmap_create(b2_ctx* ctx, double resolution, b2_voxelmap** out);
 B2_API b2_status b2_voxelmap_set_lru(b2_voxelmap* vm, size_t lru_horizon, size_t lru_clear_cycle);
 B2_API b2_status b2_voxelmap_insert(b2_voxelmap* vm, const double* points, int point_stride, const double* covs, int cov_stride, size_t n);
+/* Voxel intensities (GaussianVoxel::intensity, gaussian_voxelmap_cpu.cpp:23-37).  Every voxel holds an intensity v, 0.0 when it is
+ * created; each inserted point with intensity x sets v = (v < x) ? x : v, std::max(v, x) as GaussianVoxel::add uses it.  So NaN and
+ * -0.0 never change v, negative values never take it below 0, and v is the same whatever the order of the points (the device equals
+ * the CPU rule bit for bit).  An insert without intensities leaves every v as it is.  v survives re-opening and finalizing; it goes
+ * with its voxel on LRU eviction and moves with it when ids are re-indexed.  It is kept beside the voxel records, which do not
+ * change: the factors never read it.  Deliberate difference: the reference's GPU map (gaussian_voxelmap_gpu.cu:99-175) takes an
+ * atomicMax over the raw bits of a float, which orders negative values wrongly; here the CPU map's rule holds for every value.
+ * intensities: n doubles, or NULL (b2_voxelmap_insert).  b2_voxelmap_insert_cloud reads the frame's intensities when it has them. */
+B2_API b2_status b2_voxelmap_insert_with_intensities(b2_voxelmap* vm, const double* points, int point_stride, const double* covs, int cov_stride,
+                                                     const double* intensities, size_t n);
 /* GaussianVoxelMapGPU::insert(const PointCloud& frame) from a device cloud (src/gtsam_points/types/gaussian_voxelmap_gpu.cu:211-227),
  * with the incremental semantics of b2_voxelmap_insert; T_map_frame: 16 doubles row-major (every entry finite), or NULL = the frame as
  * stored.  The map afterwards equals b2_voxelmap_insert over b2_cloud_download's arrays posed as b2_cloud_create_transformed poses them
@@ -201,6 +238,13 @@ B2_API b2_status b2_voxelmap_insert_cloud(b2_voxelmap* vm, const b2_cloud* frame
  * include/gtsam_points/types/gaussian_voxel_data.hpp:11-54): coords V x 3, means V x 3, covs V x 9, num_points V. */
 B2_API b2_status b2_voxelmap_create_from_voxels(b2_ctx* ctx, double resolution, const int32_t* coords, const double* means, const double* covs,
                                                 const int32_t* num_points, size_t num_voxels, b2_voxelmap** out);
+/* The same with each voxel's intensity v (num_voxels doubles, stored as given; NULL: every v = 0), as GaussianVoxelData::uncompact
+ * sets it (gaussian_voxel_data.hpp:27-46).  Later inserts apply b2_voxelmap_insert_with_intensities's rule from there. */
+B2_API b2_status b2_voxelmap_create_from_voxels_with_intensities(b2_ctx* ctx, double resolution, const int32_t* coords, const double* means,
+                                                                 const double* covs, const int32_t* num_points, const double* intensities,
+                                                                 size_t num_voxels, b2_voxelmap** out);
+/* Each voxel's intensity v in id order: num_voxels doubles (all 0 for a map that never received intensities). */
+B2_API b2_status b2_voxelmap_download_intensities(const b2_voxelmap* vm, double* intensities);
 B2_API b2_status b2_voxelmap_destroy(b2_voxelmap* vm);
 B2_API b2_status b2_voxelmap_get_info(const b2_voxelmap* vm, b2_voxelmap_info* info);
 /* download_voxel_means / _covs / _num_points / buckets (gaussian_voxelmap_gpu.hpp:110-114); any pointer may be NULL */
@@ -208,7 +252,8 @@ B2_API b2_status b2_voxelmap_download(const b2_voxelmap* vm, int32_t* coords, do
 /* GaussianVoxelMapCPU::save_compact / ::load (src/gtsam_points/types/gaussian_voxelmap_cpu.cpp:79-135): the reference's wire
  * format -- 7 text header lines, then num_voxels packed 56-byte GaussianVoxelData records (types/gaussian_voxel_data.hpp:11-54:
  * int32 coord[3], int32 num_points, float mean[3], float cov[6] = (00,01,02,11,12,22), float intensity).  Files written by either
- * side load on the other. */
+ * side load on the other.  save_compact writes (float)v of each voxel; load reads the field back into v, so a file loaded and saved
+ * again gives the same records.  A file whose intensity fields are all +0.0f loads as a map without intensities (all v = 0). */
 B2_API b2_status b2_voxelmap_save_compact(const b2_voxelmap* vm, const char* path);
 B2_API b2_status b2_voxelmap_load(b2_ctx* ctx, const char* path, b2_voxelmap** out);
 /* overlap_gpu (include/gtsam_points/types/gaussian_voxelmap_gpu.hpp:116-125, src/.../gaussian_voxelmap_gpu_funcs.cu:65-194):
@@ -227,7 +272,9 @@ B2_API b2_status b2_merge_frames(b2_ctx* ctx, const double* poses, const b2_clou
 /* b2_merge_frames with the result assembled into a device cloud instead of copied to the host (merge_frames_gpu returns a GPU frame,
  * gaussian_voxelmap_gpu_funcs.cu:65-152): the cloud b2_cloud_create(points, 3, covs, 9, m, flags) makes of b2_merge_frames's output --
  * the same storage, the same stored values.  It always has covariances (zeros where the frames have none); the upper triangle of
- * each merged 3x3 is kept.  No input points give an empty cloud. */
+ * each merged 3x3 is kept.  No input points give an empty cloud.  When every frame has intensities (empty frames included), the
+ * cloud has intensities: per voxel the maximum of its points' intensities from 0.0, v = (v < x) ? x : v in the order of the sums
+ * (merge_frames, gaussian_voxelmap_cpu_funcs.cpp:83-101); else it has none.  b2_merge_frames returns no intensities. */
 B2_API b2_status b2_merge_frames_to_cloud(b2_ctx* ctx, const double* poses, const b2_cloud* const* frames, size_t num_frames, double downsample_resolution,
                                           unsigned flags, b2_cloud** out);
 /* voxel_coord + lookup_voxel_index for n host points (gaussian_voxelmap_cpu.cpp:59-69); out_index[i] = id or -1 */
@@ -254,7 +301,7 @@ typedef struct b2_ivox_info {
 B2_API b2_status b2_ivox_create(b2_ctx* ctx, double resolution, b2_ivox** out);
 B2_API b2_status b2_ivox_destroy(b2_ivox* ivox);
 /* IncrementalVoxelMap::clear (incremental_voxelmap_impl.hpp:24-28): no voxels, lru_counter = 0; the next insert may again
- * choose to carry covariances or not.  The point slots per voxel fixed by the first insert are kept. */
+ * choose to carry covariances and intensities or not.  The point slots per voxel fixed by the first insert are kept. */
 B2_API b2_status b2_ivox_clear(b2_ivox* ivox);
 /* set_lru_horizon / set_lru_clear_cycle (incremental_voxelmap.hpp:48-50); defaults 10 / 10 */
 B2_API b2_status b2_ivox_set_lru(b2_ivox* ivox, size_t lru_horizon, size_t lru_clear_cycle);
@@ -267,6 +314,13 @@ B2_API b2_status b2_ivox_set_insertion_setting(b2_ivox* ivox, double min_dist_in
 /* IncrementalVoxelMap::insert (incremental_voxelmap_impl.hpp:31-68) with FlatContainer::add (flat_container.hpp:33-50); covs may
  * be NULL, but every insert into one map must agree on whether covariances are given. */
 B2_API b2_status b2_ivox_insert(b2_ivox* ivox, const double* points, int point_stride, const double* covs, int cov_stride, size_t n);
+/* The same with per-point intensities (n doubles, may be NULL): each kept point's intensity is stored in its slot, as FlatContainer::add
+ * appends it (flat_container.hpp:51-52); b2_ivox_insert_cloud stores the frame's when it has them.  Every non-empty insert into one map
+ * must agree on whether intensities are given, as for covariances: a mix is B2_ERR_INVALID_ARGUMENT, raised before the map changes.
+ * (Deliberate difference: the reference appends intensities only for the frames that have them, so a mix misaligns its slots'
+ * vectors.)  An iVoxCovarianceEstimation keeps no intensities (incremental_covariance_container.hpp:101,106) and ignores them. */
+B2_API b2_status b2_ivox_insert_with_intensities(b2_ivox* ivox, const double* points, int point_stride, const double* covs, int cov_stride,
+                                                 const double* intensities, size_t n);
 /* IncrementalVoxelMap<FlatContainer>::insert of a device cloud posed by T_map_frame -- the map update of frame-to-map odometry
  * (src/example/advanced_scan_matching.cpp:84-95: transform the aligned frame into the map frame, insert it) in one call.
  * T_map_frame: 16 doubles row-major (every entry finite), or NULL = the frame as stored.  The map afterwards equals b2_ivox_insert over
@@ -278,6 +332,10 @@ B2_API b2_status b2_ivox_get_info(const b2_ivox* ivox, b2_ivox_info* info);
 /* Contents in id / slot order (voxel_points() / voxel_covs(), ivox.hpp): coords V x 3, counts V, points num_points x 3,
  * covs num_points x 9 (zeros if the map has none).  Any pointer may be NULL. */
 B2_API b2_status b2_ivox_download(const b2_ivox* ivox, int32_t* coords, int32_t* counts, double* points, double* covs);
+/* voxel_intensities() (incremental_voxelmap_impl.hpp:183-189): the stored points' intensities in b2_ivox_download's slot order,
+ * num_points doubles.  B2_ERR_INVALID_STATE on a map whose points were inserted without intensities, and on an
+ * iVoxCovarianceEstimation. */
+B2_API b2_status b2_ivox_download_intensities(const b2_ivox* ivox, double* intensities);
 /* IncrementalVoxelMap::knn_search (incremental_voxelmap_impl.hpp:71-92) for nq host queries, 1 <= k <= B2_KNN_MAX_K:
  * out_index = voxel_id << 32 | point_id (calc_index, incremental_voxelmap.hpp:84), KnnResult order and padding (-1, max_sq).
  * On an iVoxCovarianceEstimation map only points with a valid covariance are found (knn_search, incremental_covariance_voxelmap.hpp:46). */
@@ -393,7 +451,8 @@ B2_API b2_status b2_kdtree_estimate_normals(const b2_kdtree* tree, int k_neighbo
 /* estimate_covariances / estimate_normals (covariance_estimation.cpp:18-77, normal_estimation.cpp:52-55) of a device cloud into a NEW
  * cloud: the same points (storage type, stored order and permutation copied on the device, no host trip) with the covariances
  * b2_kdtree_estimate_covariances computes over them and, if with_normals, the normals of b2_kdtree_estimate_normals from the same
- * neighbour search.  The input's own covariances and normals are not carried over.  tree: NULL builds a temporary one; otherwise
+ * neighbour search.  The input's own covariances and normals are not carried over; its intensities are (stored under `flags` by
+ * b2_cloud_create_with_intensities's rule).  tree: NULL builds a temporary one; otherwise
  * it must come from b2_kdtree_create_from_cloud(cloud) (B2_ERR_INVALID_ARGUMENT).  flags pick only the storage of the estimated
  * arrays (B2_CLOUD_NO_REORDER: B2_ERR_INVALID_ARGUMENT).  The new cloud does not depend on the input cloud or the tree. */
 B2_API b2_status b2_cloud_create_estimated(const b2_cloud* cloud, const b2_kdtree* tree, int k_neighbors, const double* eigen_values, int with_normals,
@@ -410,7 +469,8 @@ B2_API b2_status b2_cloud_create_estimated(const b2_cloud* cloud, const b2_kdtre
  *             gathered and assembled on the device; no point data goes to the host.
  *   K:        depends only on caller indices and stored values, so a cloud made with and without B2_CLOUD_NO_REORDER gives the same K
  *             and the same bits.  out_indices (where taken) may be NULL; else it is a host array with room for n entries (n = the
- *             input's size) and receives K -- clouds carry no times or intensities, so this is how a caller samples side arrays.
+ *             input's size) and receives K -- clouds carry no times, so this is how a caller samples side arrays.  Intensities,
+ *             where the input has them, are gathered with the rows.
  *   edges:    an empty input gives an empty cloud.  Every argument check runs before any device work.
  * The random stream of the two random samplers: each point has two 64-bit priorities, s = 0 and 1, with i its caller index and
  * arithmetic mod 2^64 (SplitMix64):

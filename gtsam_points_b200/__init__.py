@@ -25,7 +25,9 @@ from .types import (  # noqa: F401
     Context,
     GaussianVoxelMapGPU,
     KdTree,
+    OffloadableGPU,
     PointCloud,
+    current_access_time,
     default_context,
     estimate_covariances,
     estimate_normals,

@@ -36,6 +36,10 @@ class VoxelMapInfo(C.Structure):
     _fields_ = [("num_voxels", C.c_uint64), ("num_buckets", C.c_uint64), ("resolution", C.c_double), ("device_bytes", C.c_uint64)]
 
 
+class Residency(C.Structure):
+    _fields_ = [("loaded_on_gpu", C.c_int32), ("reserved", C.c_int32), ("last_access", C.c_uint64), ("device_bytes", C.c_uint64), ("host_bytes", C.c_uint64)]
+
+
 class IvoxInfo(C.Structure):
     _fields_ = [("num_voxels", C.c_uint64), ("num_points", C.c_uint64), ("resolution", C.c_double), ("device_bytes", C.c_uint64)]
 
@@ -135,6 +139,15 @@ SIGNATURES = {
     "b2_merge_frames": (C.c_int, [_vp, _dp, C.POINTER(C.c_void_p), C.c_size_t, C.c_double, _dp, _dp, C.POINTER(C.c_size_t)]),
     "b2_merge_frames_to_cloud": (C.c_int, [_vp, _dp, C.POINTER(C.c_void_p), C.c_size_t, C.c_double, C.c_uint, _pp]),
     "b2_voxelmap_lookup": (C.c_int, [_vp, _dp, C.c_int, C.c_size_t, _ip]),
+    "b2_cloud_offload": (C.c_int, [_vp, _ip]),
+    "b2_cloud_reload": (C.c_int, [_vp, _ip]),
+    "b2_cloud_touch": (C.c_int, [_vp, _ip]),
+    "b2_cloud_residency": (C.c_int, [_vp, C.POINTER(Residency)]),
+    "b2_voxelmap_offload": (C.c_int, [_vp, _ip]),
+    "b2_voxelmap_reload": (C.c_int, [_vp, _ip]),
+    "b2_voxelmap_touch": (C.c_int, [_vp, _ip]),
+    "b2_voxelmap_residency": (C.c_int, [_vp, C.POINTER(Residency)]),
+    "b2_access_time_current": (C.c_int, [C.POINTER(C.c_uint64)]),
     "b2_ivox_create": (C.c_int, [_vp, C.c_double, _pp]),
     "b2_ivox_destroy": (C.c_int, [_vp]),
     "b2_ivox_clear": (C.c_int, [_vp]),
@@ -203,6 +216,8 @@ SIGNATURES = {
     "b2_factor_set_correspondence_update_tolerance": (C.c_int, [_vp, C.c_double, C.c_double]),
     "b2_factor_set_enable_surface_validation": (C.c_int, [_vp, C.c_int]),
     "b2_factor_num_points": (C.c_size_t, [_vp]),
+    "b2_factor_set_enable_offloading": (C.c_int, [_vp, C.c_int]),
+    "b2_factor_device_bytes": (C.c_int, [_vp, C.POINTER(C.c_uint64)]),
     "b2_factor_correspondences": (C.c_int, [_vp, _lp]),
     "b2_factor_linearize": (C.c_int, [_vp, _dp, _dp]),
     "b2_factor_error": (C.c_int, [_vp, _dp, _dp]),

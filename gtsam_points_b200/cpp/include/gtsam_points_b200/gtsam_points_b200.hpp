@@ -64,6 +64,9 @@
 #endif
 #endif
 
+// cudaStream_t is ::CUstream_st*: the offloading methods take the reference's stream argument (types/offloadable.hpp) without CUDA headers
+struct CUstream_st;
+
 namespace gtsam_points_b200 {
 
 inline void check(b2_status st, const char* what) {
@@ -148,7 +151,34 @@ template <typename Frame>
 const double* frame_intensities(const Frame&, long) { return nullptr; }
 }  // namespace detail
 
-class PointCloudGPU {
+// types/offloadable.hpp: an object whose device copy can be moved to host memory and back (b2points.h: GPU memory offloading).
+// offload_gpu / reload_gpu return whether they moved anything; touch() records an access (last_access = clock++) and reloads if
+// needed.  The stream arguments are accepted for source compatibility; the copies run on the object's context stream.  While an
+// object is offloaded, calls that read it throw -- except overlap_gpu and factors with set_enable_offloading(true), which touch
+// what they read.
+class OffloadableGPU {
+public:
+  using Ptr = std::shared_ptr<OffloadableGPU>;
+  using ConstPtr = std::shared_ptr<const OffloadableGPU>;
+  virtual ~OffloadableGPU() {}
+
+  static std::uint64_t current_access_time() {
+    std::uint64_t t = 0;
+    check(b2_access_time_current(&t), "b2_access_time_current");
+    return t;
+  }
+  std::uint64_t last_accessed_time() const { return residency().last_access; }
+  virtual std::size_t memory_usage_gpu() const { return residency().device_bytes; }
+  virtual bool loaded_on_gpu() const { return residency().loaded_on_gpu != 0; }
+  virtual bool touch(CUstream_st* stream = 0) = 0;
+  virtual bool offload_gpu(CUstream_st* stream = 0) = 0;
+  virtual bool reload_gpu(CUstream_st* stream = 0) = 0;
+
+protected:
+  virtual b2_residency residency() const = 0;
+};
+
+class PointCloudGPU : public OffloadableGPU {
 public:
   using Ptr = std::shared_ptr<PointCloudGPU>;
   using ConstPtr = std::shared_ptr<const PointCloudGPU>;
@@ -230,9 +260,17 @@ public:
     check(b2_cloud_download_intensities(cloud_, out.data()), "b2_cloud_download_intensities");
     return out;
   }
-  ~PointCloudGPU() {
+  ~PointCloudGPU() override {
     b2_cloud_destroy(cloud_);
     for (b2_cloud* c : retired_) b2_cloud_destroy(c);
+  }
+  // OffloadableGPU: the handles add_intensities retired move with the current one (factors made earlier may read them)
+  bool offload_gpu(CUstream_st* = 0) override { return each_handle(b2_cloud_offload, "b2_cloud_offload"); }
+  bool reload_gpu(CUstream_st* = 0) override { return each_handle(b2_cloud_reload, "b2_cloud_reload"); }
+  bool touch(CUstream_st* = 0) override {
+    int changed = 0;
+    check(b2_cloud_touch(cloud_, &changed), "b2_cloud_touch");
+    return each_handle(b2_cloud_reload, "b2_cloud_reload") || changed != 0;
   }
   PointCloudGPU(const PointCloudGPU&) = delete;
 
@@ -244,8 +282,31 @@ public:
   b2_cloud* handle() const { return cloud_; }
   Context::Ptr context() const { return ctx_; }
 
+protected:
+  b2_residency residency() const override {
+    b2_residency r{};
+    check(b2_cloud_residency(cloud_, &r), "b2_cloud_residency");
+    for (b2_cloud* c : retired_) {
+      b2_residency o{};
+      check(b2_cloud_residency(c, &o), "b2_cloud_residency");
+      r.device_bytes += o.device_bytes;
+      r.host_bytes += o.host_bytes;
+    }
+    return r;
+  }
+
 private:
   PointCloudGPU() = default;
+  bool each_handle(b2_status (*op)(b2_cloud*, int*), const char* what) {
+    int changed = 0, any = 0;
+    check(op(cloud_, &changed), what);
+    any |= changed;
+    for (b2_cloud* c : retired_) {
+      check(op(c, &changed), what);
+      any |= changed;
+    }
+    return any != 0;
+  }
   // frame->normals where the frame type has such a member, else null
   template <typename Frame>
   static auto frame_normals(const Frame& f, int) -> decltype(reinterpret_cast<const double*>(f.normals)) { return reinterpret_cast<const double*>(f.normals); }
@@ -271,12 +332,13 @@ public:
   virtual void save_compact(const std::string& path) const = 0;
 };
 
-class GaussianVoxelMapGPU : public GaussianVoxelMap {
+class GaussianVoxelMapGPU : public GaussianVoxelMap, public OffloadableGPU {
 public:
   using Ptr = std::shared_ptr<GaussianVoxelMapGPU>;
   using ConstPtr = std::shared_ptr<const GaussianVoxelMapGPU>;
 
-  explicit GaussianVoxelMapGPU(double resolution, Context::Ptr ctx = Context::default_context()) : ctx_(ctx), resolution_(resolution) {}
+  explicit GaussianVoxelMapGPU(double resolution, Context::Ptr ctx = Context::default_context())
+  : ctx_(ctx), resolution_(resolution), created_at_(OffloadableGPU::current_access_time()) {}
   ~GaussianVoxelMapGPU() override { b2_voxelmap_destroy(vm_); }
   GaussianVoxelMapGPU(const GaussianVoxelMapGPU&) = delete;
 
@@ -331,9 +393,35 @@ public:
   b2_voxelmap* handle() const { return vm_; }
   Context::Ptr context() const { return ctx_; }
 
+  // OffloadableGPU.  The device map is made by the first insert (or set_lru / touch).  Until then the map holds no device memory,
+  // so offload / reload move nothing, and last_accessed_time() is the clock's value at construction (the reference's creation
+  // stamp); the device map, once made, records the clock's value at its own creation, as every new device object does.  touch()
+  // makes the device map, so that it has an object to record the access on.
+  bool offload_gpu(CUstream_st* = 0) override { return call(b2_voxelmap_offload, "b2_voxelmap_offload"); }
+  bool reload_gpu(CUstream_st* = 0) override { return call(b2_voxelmap_reload, "b2_voxelmap_reload"); }
+  bool touch(CUstream_st* = 0) override {
+    if (!vm_) check(b2_voxelmap_create(ctx_->get(), resolution_, &vm_), "b2_voxelmap_create");
+    return call(b2_voxelmap_touch, "b2_voxelmap_touch");
+  }
+
+protected:
+  b2_residency residency() const override {
+    b2_residency r{};
+    r.loaded_on_gpu = 1;
+    r.last_access = created_at_;
+    if (vm_) check(b2_voxelmap_residency(vm_, &r), "b2_voxelmap_residency");
+    return r;
+  }
+
 private:
+  bool call(b2_status (*op)(b2_voxelmap*, int*), const char* what) {
+    int changed = 0;
+    if (vm_) check(op(vm_, &changed), what);
+    return changed != 0;
+  }
   Context::Ptr ctx_;
   double resolution_;
+  std::uint64_t created_at_ = 0;  // the access clock at construction: last_accessed_time() while there is no device map
   b2_voxelmap* vm_ = nullptr;
 };
 
@@ -1195,7 +1283,25 @@ public:
   }
   b2_factor* handle() const { return factor_; }
 
+  // IntegratedVGICPFactorGPU::set_enable_offloading, on every factor kind: each linearize / error first touches what the factor
+  // reads (a VGICP factor's target map, then its source cloud), reloading what was offloaded.  clone() carries it over.
+  void set_enable_offloading(bool enable) {
+    check(b2_factor_set_enable_offloading(factor_, enable ? 1 : 0), "b2_factor_set_enable_offloading");
+    offloading_ = enable;
+  }
+  // device bytes the factor owns itself (correspondences, gathered kd-tree target records, linearization point)
+  std::size_t memory_usage_gpu() const {
+    std::uint64_t b = 0;
+    check(b2_factor_device_bytes(factor_, &b), "b2_factor_device_bytes");
+    return b;
+  }
+
 protected:
+  // clone(): the copy takes this factor's offloading setting
+  FactorBasePtr carry_settings(IntegratedMatchingCostFactorB200* f) const {
+    if (offloading_) f->set_enable_offloading(true);
+    return FactorBasePtr(f);
+  }
   IntegratedMatchingCostFactorB200(Key target_key, Key source_key) : NonlinearFactorGPU(std::vector<Key>{target_key, source_key}), is_binary_(true) {
     fixed_target_pose_ = Mat4{1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
   }
@@ -1246,6 +1352,7 @@ protected:
   bool is_binary_;
   Mat4 fixed_target_pose_;
   b2_factor* factor_ = nullptr;
+  bool offloading_ = false;
   mutable b2_linearized linearized_{};
   mutable bool has_linearization_ = false;
   mutable double evaluation_ = 0.0;
@@ -1304,7 +1411,7 @@ public:
     IntegratedVGICPFactor* f = new IntegratedVGICPFactor(this->keys()[0], this->keys()[is_binary_ ? 1 : 0], target_voxels_, source_);
     if (!is_binary_) f->make_unary(fixed_target_pose_);
     if (surface_validation_) f->set_enable_surface_validation(true);
-    return FactorBasePtr(f);
+    return carry_settings(f);
   }
   // device bytes this factor owns itself (correspondence array + linearization point); clouds / maps are shared
   std::size_t memory_usage() const { return b2_factor_num_points(factor_) * sizeof(std::int32_t) + 16 * sizeof(double) + sizeof(*this); }
@@ -1390,12 +1497,12 @@ public:
     check(b2_factor_set_correspondence_update_tolerance(factor_, angle, trans), "b2_factor_set_correspondence_update_tolerance");
   }
   FactorBasePtr clone() const override {
-    if (is_binary_) return FactorBasePtr(ivox_ ? new IntegratedGICPFactor(this->keys()[0], this->keys()[1], ivox_, source_) : new IntegratedGICPFactor(this->keys()[0], this->keys()[1], target_, source_, tree_));
+    if (is_binary_) return carry_settings(ivox_ ? new IntegratedGICPFactor(this->keys()[0], this->keys()[1], ivox_, source_) : new IntegratedGICPFactor(this->keys()[0], this->keys()[1], target_, source_, tree_));
     IntegratedGICPFactor* f = ivox_ ? new IntegratedGICPFactor(this->keys()[0], this->keys()[0], ivox_, source_) : new IntegratedGICPFactor(this->keys()[0], this->keys()[0], target_, source_, tree_);
     f->is_binary_ = false;
     f->fixed_target_pose_ = fixed_target_pose_;
     f->keys_.erase(f->keys_.begin());
-    return FactorBasePtr(f);
+    return carry_settings(f);
   }
   std::size_t memory_usage() const {
     return b2_factor_num_points(factor_) * sizeof(std::int32_t) + 16 * sizeof(double) + (ivox_ ? 0 : target_->size() * 10 * sizeof(double)) + sizeof(*this);
@@ -1472,12 +1579,12 @@ public:
     auto make = [&](Key target_key, Key source_key) {
       return ivox_ ? new IntegratedICPFactor(target_key, source_key, ivox_, source_, plane_) : new IntegratedICPFactor(target_key, source_key, target_, source_, tree_, plane_, nrm);
     };
-    if (is_binary_) return FactorBasePtr(make(this->keys()[0], this->keys()[1]));
+    if (is_binary_) return carry_settings(make(this->keys()[0], this->keys()[1]));
     IntegratedICPFactor* f = make(this->keys()[0], this->keys()[0]);
     f->is_binary_ = false;
     f->fixed_target_pose_ = fixed_target_pose_;
     f->keys_.erase(f->keys_.begin());
-    return FactorBasePtr(f);
+    return carry_settings(f);
   }
   iVoxGPU::ConstPtr get_target_ivox() const { return ivox_; }
 

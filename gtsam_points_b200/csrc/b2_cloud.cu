@@ -348,6 +348,7 @@ b2_status merge_frames_check(b2_ctx* ctx, const double* poses, const b2_cloud* c
   *have_covs = true;
   *have_ints = true;
   for (size_t f = 0; f < num_frames; f++) {
+    B2_TRY(require_resident(frames[f], who, "a frame"));
     B2_REQUIRE(frames[f] != nullptr && (frames[f]->n == 0 || frames[f]->d_points), "error: frame %zu has no points", f);
     B2_REQUIRE(frames[f]->ctx->device == ctx->device, "%s: frame %zu lives on another device", who, f);
     B2_TRY(check_pose(poses + 16 * f, who));
@@ -613,6 +614,27 @@ b2_status cloud_arrays_to_device(const b2_cloud* c, cudaStream_t st, const doubl
   return B2_OK;
 }
 
+namespace {
+// Reload of an offloaded cloud on `st`: every array back from the host copy, which the cloud keeps.  On a failed allocation the cloud
+// stays offloaded.
+b2_status cloud_reload(b2_cloud* c, cudaStream_t st) {
+  B2_TRY(reload_arrays({&c->d_points, &c->d_covs, &c->d_normals, &c->d_perm, &c->d_intensities}, {false, false, false, false, false}, st, c->host));
+  B2_TRY(stream_after(c->ctx->stream, st));
+  c->offloaded = false;
+  c->residency_gen++;
+  return B2_OK;
+}
+}  // namespace
+
+b2_status cloud_touch(b2_cloud* c, cudaStream_t st, bool* changed) {
+  c->last_access = access_clock_tick();
+  if (changed) *changed = false;
+  if (!c->offloaded) return B2_OK;
+  B2_TRY(cloud_reload(c, st));
+  if (changed) *changed = true;
+  return B2_OK;
+}
+
 b2_status cloud_intensities_to_device(const b2_cloud* c, cudaStream_t st, double* d_out) {
   with_storage(c->intensity_bytes, [&](auto t) {
     using IT = decltype(t);
@@ -678,6 +700,7 @@ b2_status b2_cloud_intensity_bytes(const b2_cloud* cloud, int* out) {
 
 b2_status b2_cloud_download_intensities(const b2_cloud* c, double* out) {
   B2_REQUIRE(c != nullptr && (out != nullptr || c->n == 0), "b2_cloud_download_intensities: NULL argument");
+  B2_TRY(require_resident(c, "b2_cloud_download_intensities"));
   if (!c->d_intensities) return fail(B2_ERR_INVALID_STATE, "b2_cloud_download_intensities: the cloud has no intensities");
   if (c->n == 0) return B2_OK;
   B2_ON_DEVICE(c->ctx);
@@ -698,6 +721,7 @@ b2_status b2_cloud_create_with_added_intensities(const b2_cloud* cloud, const do
   *out = nullptr;
   B2_REQUIRE(cloud != nullptr, "%s: cloud is NULL", who);
   B2_REQUIRE(intensities != nullptr, "%s: intensities is NULL", who);
+  B2_TRY(require_resident(cloud, who));
   B2_ON_DEVICE(cloud->ctx);
   cudaStream_t st = cloud->ctx->stream;
   DeviceBuffer d_i;
@@ -785,6 +809,7 @@ b2_status b2_cloud_create_transformed(const b2_cloud* cloud, const double* T, un
   *out = nullptr;
   B2_REQUIRE(cloud != nullptr, "b2_cloud_create_transformed: cloud is NULL");
   B2_TRY(check_pose(T, "b2_cloud_create_transformed"));
+  B2_TRY(require_resident(cloud, "b2_cloud_create_transformed"));
   B2_ON_DEVICE(cloud->ctx);
   const size_t n = cloud->n, rows = std::max<size_t>(n, 1);  // n == 0: the buffers only mark which arrays the cloud has
   DeviceBuffer d_p, d_c, d_n, d_i;
@@ -855,6 +880,58 @@ b2_status b2_cloud_destroy(b2_cloud* c) {
   return B2_OK;
 }
 
+// PointCloudGPU::offload_gpu: the device arrays into one pinned host block (once: a cloud never changes, so the block is kept for
+// later offloads), then the device buffers are freed.
+b2_status b2_cloud_offload(b2_cloud* c, int* changed) {
+  B2_REQUIRE(c != nullptr, "b2_cloud_offload: cloud is NULL");
+  if (changed) *changed = 0;
+  if (c->offloaded) return B2_OK;
+  B2_ON_DEVICE(c->ctx);
+  cudaStream_t st = c->ctx->stream;
+  if (c->host.empty()) {
+    B2_TRY(offload_arrays({&c->d_points, &c->d_covs, &c->d_normals, &c->d_perm, &c->d_intensities},
+                          {c->d_points.bytes(), c->d_covs.bytes(), c->d_normals.bytes(), c->d_perm.bytes(), c->d_intensities.bytes()}, st, c->host));
+  } else {
+    B2_CUDA(cudaStreamSynchronize(st));  // queued work may still read the arrays
+  }
+  c->d_points.reset(), c->d_covs.reset(), c->d_normals.reset(), c->d_perm.reset(), c->d_intensities.reset();
+  c->offloaded = true;
+  if (changed) *changed = 1;
+  return B2_OK;
+}
+
+b2_status b2_cloud_reload(b2_cloud* c, int* changed) {
+  B2_REQUIRE(c != nullptr, "b2_cloud_reload: cloud is NULL");
+  if (changed) *changed = 0;
+  if (!c->offloaded) return B2_OK;
+  B2_ON_DEVICE(c->ctx);
+  B2_TRY(cloud_reload(c, c->ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(c->ctx->stream));
+  if (changed) *changed = 1;
+  return B2_OK;
+}
+
+b2_status b2_cloud_touch(b2_cloud* c, int* changed) {
+  B2_REQUIRE(c != nullptr, "b2_cloud_touch: cloud is NULL");
+  if (changed) *changed = 0;
+  B2_ON_DEVICE(c->ctx);
+  bool reloaded = false;
+  B2_TRY(cloud_touch(c, c->ctx->stream, &reloaded));
+  if (reloaded) B2_CUDA(cudaStreamSynchronize(c->ctx->stream));
+  if (changed) *changed = reloaded ? 1 : 0;
+  return B2_OK;
+}
+
+b2_status b2_cloud_residency(const b2_cloud* c, b2_residency* out) {
+  B2_REQUIRE(c && out, "b2_cloud_residency: NULL argument");
+  out->loaded_on_gpu = c->offloaded ? 0 : 1;
+  out->reserved = 0;
+  out->last_access = c->last_access;
+  out->device_bytes = c->device_bytes();
+  out->host_bytes = c->host.block.bytes();
+  return B2_OK;
+}
+
 b2_status b2_cloud_get_info(const b2_cloud* c, b2_cloud_info* info) {
   B2_REQUIRE(c && info, "b2_cloud_get_info: NULL argument");
   info->num_points = c->n;
@@ -868,6 +945,7 @@ b2_status b2_cloud_get_info(const b2_cloud* c, b2_cloud_info* info) {
 
 b2_status b2_cloud_download(const b2_cloud* c, double* out_points, double* out_covs, double* out_normals) {
   B2_REQUIRE(c != nullptr, "b2_cloud_download: cloud is NULL");
+  B2_TRY(require_resident(c, "b2_cloud_download"));
   if (out_covs && !c->d_covs) return fail(B2_ERR_INVALID_STATE, "b2_cloud_download: the cloud has no covariances");
   if (out_normals && !c->d_normals) return fail(B2_ERR_INVALID_STATE, "b2_cloud_download: the cloud has no normals");
   if (c->n == 0) return B2_OK;
@@ -889,6 +967,7 @@ b2_status b2_cloud_download(const b2_cloud* c, double* out_points, double* out_c
 
 b2_status b2_cloud_download_normals(const b2_cloud* c, double* out_normals) {
   B2_REQUIRE(c != nullptr && (out_normals != nullptr || c->n == 0), "b2_cloud_download_normals: NULL argument");
+  B2_TRY(require_resident(c, "b2_cloud_download_normals"));
   if (!c->d_normals) return fail(B2_ERR_INVALID_STATE, "b2_cloud_download_normals: the cloud has no normals");
   return b2_cloud_download(c, nullptr, nullptr, out_normals);
 }

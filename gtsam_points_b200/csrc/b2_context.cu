@@ -1,4 +1,5 @@
 // b2_context.cu -- library state, error reporting, context (device + stream + staging).
+#include <atomic>
 #include <cstring>
 
 #include "b2_internal.hpp"
@@ -60,6 +61,66 @@ DeviceScope::DeviceScope(int device) {
 
 DeviceScope::~DeviceScope() {
   if (restore_) ctx_calls()->set(saved_);
+}
+
+// ---- residency ----
+
+namespace {
+std::atomic<uint64_t> g_access_clock{0};
+}  // namespace
+
+uint64_t access_clock_now() { return g_access_clock.load(); }
+uint64_t access_clock_tick() { return g_access_clock.fetch_add(1); }
+
+b2_status offload_arrays(std::initializer_list<DeviceBuffer*> bufs, std::initializer_list<size_t> sizes, cudaStream_t st, HostCopy& host) {
+  size_t total = 0;
+  for (size_t s : sizes) total += s;
+  HostCopy h;
+  B2_TRY(h.block.alloc(total));
+  size_t off = 0;
+  auto s = sizes.begin();
+  for (DeviceBuffer* b : bufs) {
+    const size_t bytes = *b ? *s : 0;
+    if (bytes) B2_CUDA(cudaMemcpyAsync(h.block.get() + off, b->get(), bytes, cudaMemcpyDeviceToHost, st));
+    h.sizes.push_back(bytes);
+    h.alloc.push_back(b->bytes());
+    off += bytes;
+    ++s;
+  }
+  B2_CUDA(cudaStreamSynchronize(st));
+  host.block = std::move(h.block);
+  host.sizes = std::move(h.sizes);
+  host.alloc = std::move(h.alloc);
+  return B2_OK;
+}
+
+b2_status reload_arrays(std::initializer_list<DeviceBuffer*> bufs, std::initializer_list<bool> zero, cudaStream_t st, const HostCopy& host) {
+  // everything is allocated and queued before any buffer is handed over: on failure `fresh` frees what was allocated here
+  std::vector<DeviceBuffer> fresh(bufs.size());
+  size_t off = 0;
+  auto z = zero.begin();
+  for (size_t k = 0; k < fresh.size(); k++, ++z) {
+    if (host.alloc[k] > 0) {
+      B2_TRY(fresh[k].alloc(host.alloc[k]));
+      if (*z) B2_CUDA(cudaMemsetAsync(fresh[k].get(), 0, host.alloc[k], st));
+      if (host.sizes[k]) B2_CUDA(cudaMemcpyAsync(fresh[k].get(), host.block.get() + off, host.sizes[k], cudaMemcpyHostToDevice, st));
+    }
+    off += host.sizes[k];
+  }
+  size_t k = 0;
+  for (DeviceBuffer* b : bufs) *b = std::move(fresh[k++]);
+  return B2_OK;
+}
+
+b2_status stream_after(cudaStream_t other, cudaStream_t st) {
+  if (other == st) return B2_OK;
+  cudaEvent_t ev = nullptr;
+  B2_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  cudaError_t e = cudaEventRecord(ev, st);
+  if (e == cudaSuccess) e = cudaStreamWaitEvent(other, ev, 0);
+  cudaEventDestroy(ev);  // released once the wait has been satisfied
+  B2_CUDA(e);
+  return B2_OK;
 }
 
 }  // namespace b2
@@ -160,6 +221,12 @@ b2_status b2_ctx_synchronize(b2_ctx* ctx) {
 }
 
 void* b2_ctx_stream(b2_ctx* ctx) { return ctx ? static_cast<void*>(ctx->stream) : nullptr; }
+
+b2_status b2_access_time_current(uint64_t* out) {
+  B2_REQUIRE(out != nullptr, "b2_access_time_current: out is NULL");
+  *out = b2::access_clock_now();
+  return B2_OK;
+}
 
 b2_status b2_device_malloc(b2_ctx* ctx, size_t bytes, void** out) {
   B2_REQUIRE(ctx && out, "b2_device_malloc: NULL argument");

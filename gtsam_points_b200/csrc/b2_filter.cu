@@ -175,6 +175,7 @@ b2_status b2_cloud_create_sampled(const b2_cloud* cloud, const int64_t* indices,
   B2_REQUIRE(out != nullptr, "%s: out is NULL", who);
   *out = nullptr;
   B2_REQUIRE(cloud != nullptr, "%s: cloud is NULL", who);
+  B2_TRY(require_resident(cloud, who));
   B2_REQUIRE(indices != nullptr || num_indices == 0, "%s: indices is NULL", who);
   B2_REQUIRE(num_indices < (1ull << 31), "%s: at most 2^31-1 indices", who);
   const size_t n = cloud->n;
@@ -198,6 +199,7 @@ b2_status b2_cloud_create_random_sampled(const b2_cloud* cloud, double sampling_
   B2_REQUIRE(out != nullptr, "%s: out is NULL", who);
   *out = nullptr;
   B2_REQUIRE(cloud != nullptr, "%s: cloud is NULL", who);
+  B2_TRY(require_resident(cloud, who));
   B2_TRY(check_rate(sampling_rate, who));
   B2_ON_DEVICE(cloud->ctx);
   cudaStream_t st = cloud->ctx->stream;
@@ -219,6 +221,7 @@ b2_status b2_cloud_create_randomgrid(const b2_cloud* cloud, double resolution, d
   B2_REQUIRE(out != nullptr, "%s: out is NULL", who);
   *out = nullptr;
   B2_REQUIRE(cloud != nullptr, "%s: cloud is NULL", who);
+  B2_TRY(require_resident(cloud, who));
   B2_REQUIRE(resolution > 0.0 && std::isfinite(resolution), "%s: resolution must be positive and finite (got %g)", who, resolution);
   B2_TRY(check_rate(sampling_rate, who));
   B2_ON_DEVICE(cloud->ctx);
@@ -280,6 +283,7 @@ b2_status b2_cloud_create_inliers(const b2_cloud* cloud, const b2_kdtree* tree, 
   B2_REQUIRE(out != nullptr, "%s: out is NULL", who);
   *out = nullptr;
   B2_REQUIRE(cloud != nullptr, "%s: cloud is NULL", who);
+  B2_TRY(require_resident(cloud, who));
   B2_REQUIRE(k >= 1 && k <= B2_KNN_MAX_K, "%s: k must be in [1, %d] (got %d)", who, B2_KNN_MAX_K, k);
   B2_REQUIRE(std::isfinite(std_thresh), "%s: std_thresh must be finite (got %g)", who, std_thresh);
   B2_REQUIRE(tree == nullptr || tree->cloud_uid == cloud->uid, "%s: the tree was not built by b2_kdtree_create_from_cloud from this cloud", who);

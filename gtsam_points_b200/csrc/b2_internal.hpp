@@ -129,6 +129,76 @@ class DeviceBuffer {
   size_t bytes_ = 0;
 };
 
+// ---- pinned host memory ---------------------------------------------------------------------------
+// One cudaHostAlloc allocation and its size in bytes: the host copy of an offloaded cloud or map.  Move-only, like DeviceBuffer.
+class HostBuffer {
+ public:
+  HostBuffer() = default;
+  HostBuffer(const HostBuffer&) = delete;
+  HostBuffer& operator=(const HostBuffer&) = delete;
+  HostBuffer(HostBuffer&& o) noexcept : p_(std::exchange(o.p_, nullptr)), bytes_(std::exchange(o.bytes_, 0)) {}
+  HostBuffer& operator=(HostBuffer&& o) noexcept {
+    if (this != &o) {
+      reset();
+      p_ = std::exchange(o.p_, nullptr);
+      bytes_ = std::exchange(o.bytes_, 0);
+    }
+    return *this;
+  }
+  ~HostBuffer() { reset(); }
+  // frees what the buffer holds, then allocates `bytes` (at least 1); B2_ERR_OUT_OF_MEMORY / B2_ERR_CUDA on failure (then empty)
+  b2_status alloc(size_t bytes) {
+    reset();
+    const cudaError_t e = cudaHostAlloc(&p_, std::max<size_t>(bytes, 1), cudaHostAllocDefault);
+    if (e != cudaSuccess) {
+      p_ = nullptr;
+      return fail(e == cudaErrorMemoryAllocation ? B2_ERR_OUT_OF_MEMORY : B2_ERR_CUDA, "cudaHostAlloc(%zu bytes) -> %s", bytes, cudaGetErrorString(e));
+    }
+    bytes_ = bytes;
+    return B2_OK;
+  }
+  void reset() {
+    if (p_) cudaFreeHost(p_);
+    p_ = nullptr;
+    bytes_ = 0;
+  }
+  char* get() const { return static_cast<char*>(p_); }
+  size_t bytes() const { return bytes_; }
+  explicit operator bool() const { return p_ != nullptr; }
+
+ private:
+  void* p_ = nullptr;
+  size_t bytes_ = 0;
+};
+
+// ---- residency: offload / reload of device clouds and Gaussian voxel maps ---------------------------------------------------
+// The process-wide access clock (OffloadableGPU::access_counter): an object records its value at creation, and touch() takes
+// last_access = clock++ before it reloads.
+uint64_t access_clock_now();
+uint64_t access_clock_tick();  // clock++, returns the value before the increment
+
+// The device arrays of an object as one pinned host block: array k occupies `sizes[k]` bytes of `block` at the sum of the sizes
+// before it.  `alloc[k]` is the device allocation the array is reloaded into (>= sizes[k]: a map's arrays keep their capacity).
+struct HostCopy {
+  HostBuffer block;
+  std::vector<size_t> sizes, alloc;
+  bool empty() const { return !block; }
+  void reset() {
+    block.reset();
+    sizes.clear();
+    alloc.clear();
+  }
+};
+// Copies bytes [0, sizes[k]) of every non-empty array bufs[k] into a fresh host block on `st`, then synchronises `st`.  The copy
+// is left empty and the status returned when the block cannot be allocated.
+b2_status offload_arrays(std::initializer_list<DeviceBuffer*> bufs, std::initializer_list<size_t> sizes, cudaStream_t st, HostCopy& host);
+// Allocates every array of `host` (alloc[k] bytes, nothing for alloc[k] == 0) and copies its sizes[k] bytes back, asynchronously on
+// `st`; `zero[k]` clears array k first.  On a failed allocation every array allocated here is freed again, bufs are left empty and
+// the status (B2_ERR_OUT_OF_MEMORY) is returned.
+b2_status reload_arrays(std::initializer_list<DeviceBuffer*> bufs, std::initializer_list<bool> zero, cudaStream_t st, const HostCopy& host);
+// Makes `other` wait for the work queued on `st` so far (a reload issued on one stream, read on another).  Nothing if they are equal.
+b2_status stream_after(cudaStream_t other, cudaStream_t st);
+
 // ---- CUB two-phase calls ---------------------------------------------------------------------------
 // A CUB device algorithm is written once, as `call(void* temp, size_t& temp_bytes) -> cudaError_t`: called with temp == nullptr
 // it only reports the temporary storage it needs.
@@ -440,6 +510,13 @@ struct b2_cloud {
   // planes above: no factor reads it.
   b2::DeviceBuffer d_intensities;
   size_t device_bytes() const { return d_points.bytes() + d_covs.bytes() + d_normals.bytes() + d_perm.bytes() + d_intensities.bytes(); }
+  // residency (b2_cloud_offload / b2_cloud_reload / b2_cloud_touch).  While offloaded every device buffer above is empty and the
+  // arrays live in `host` only; the metadata above (sizes, storage types, centre) stays.  A cloud never changes, so its host copy is
+  // kept until it is destroyed and a second offload only frees the device buffers.
+  bool offloaded = false;
+  uint64_t last_access = b2::access_clock_now();
+  uint64_t residency_gen = 0;  // bumped by every reload: the device addresses changed, factor sets refresh their descriptors
+  b2::HostCopy host;
 };
 
 // A voxel-keyed map: a bucket table (integer voxel coordinate -> voxel id) over per-voxel arrays in id order.  `slots` is the
@@ -475,7 +552,31 @@ struct b2_voxelmap {
     return d_buckets.bytes() + d_records.bytes() + d_coords.bytes() + d_lru.bytes() + d_counts.bytes() + d_flags.bytes() + d_normals.bytes() +
            d_intensities.bytes();
   }
+  // residency of a Gaussian voxel map (b2_voxelmap_offload / _reload / _touch; an iVox's map is never offloaded).  Offloading keeps
+  // the records, coordinates, LRU stamps and intensities of the num_voxels voxels in `host` and frees every device buffer, the
+  // bucket table included (num_buckets = 0): a reload rebuilds the table from the coordinates.  The first insert after a reload
+  // drops the host copy; the next offload copies again.
+  bool offloaded = false;
+  uint64_t last_access = b2::access_clock_now();
+  b2::HostCopy host;
 };
+
+namespace b2 {
+// The one residency check of every entry point that reads a cloud's or map's device arrays: B2_ERR_INVALID_STATE, naming `who`
+// and `what`, if the object is offloaded.  A NULL handle passes (the caller's own checks report it).
+inline b2_status require_resident(const b2_cloud* c, const char* who, const char* what = "the cloud") {
+  if (c && c->offloaded) return fail(B2_ERR_INVALID_STATE, "%s: %s is offloaded from the GPU (reload or touch it first)", who, what);
+  return B2_OK;
+}
+inline b2_status require_resident(const b2_voxelmap* vm, const char* who, const char* what = "the voxel map") {
+  if (vm && vm->offloaded) return fail(B2_ERR_INVALID_STATE, "%s: %s is offloaded from the GPU (reload or touch it first)", who, what);
+  return B2_OK;
+}
+// touch(): last_access = clock++, then a reload if the object is offloaded, issued on `st` (the caller's device is the object's).
+// *changed (may be NULL): whether it reloaded.
+b2_status cloud_touch(b2_cloud* c, cudaStream_t st, bool* changed);
+b2_status voxelmap_touch(b2_voxelmap* vm, cudaStream_t st, bool* changed);
+}  // namespace b2
 
 // Running eigenvalue statistics of one insert (RunningStatistics<Eigen::Array3d>, util/runnning_statistics.hpp: count, sum, sum_sq;
 // min / max are never read by the map).
@@ -574,4 +675,7 @@ struct b2_factor {
   uint64_t corr_gen = 0;  // iVox factors: map generation the stored correspondences were associated against
   double lin_delta[16] = {0};
   b2_factor_set* self_set = nullptr;  // lazily created set of size 1 for the single-factor entry points
+  // b2_factor_set_enable_offloading: every launch touches what it reads (a VGICP target map, then the source cloud), reloading
+  // what is offloaded; off, a launch that would read an offloaded object fails
+  bool offloading = false;
 };

@@ -502,6 +502,7 @@ b2_status b2_kdtree_create_from_cloud(const b2_cloud* cloud, b2_kdtree** out) {
   B2_REQUIRE(out != nullptr, "b2_kdtree_create_from_cloud: out is NULL");
   *out = nullptr;
   B2_REQUIRE(cloud != nullptr, "b2_kdtree_create_from_cloud: cloud is NULL");
+  B2_TRY(require_resident(cloud, "b2_kdtree_create_from_cloud"));
   b2_ctx* ctx = cloud->ctx;
   B2_ON_DEVICE(ctx);
   DeviceBuffer d_pts;
@@ -724,6 +725,7 @@ b2_status b2_cloud_create_estimated(const b2_cloud* cloud, const b2_kdtree* tree
   B2_REQUIRE(out != nullptr, "b2_cloud_create_estimated: out is NULL");
   *out = nullptr;
   B2_REQUIRE(cloud != nullptr, "b2_cloud_create_estimated: cloud is NULL");
+  B2_TRY(require_resident(cloud, "b2_cloud_create_estimated"));
   B2_REQUIRE(k_neighbors >= 1 && k_neighbors <= B2_KNN_MAX_K, "b2_cloud_create_estimated: k_neighbors must be in [1, %d]", B2_KNN_MAX_K);
   B2_REQUIRE(!(flags & B2_CLOUD_NO_REORDER), "b2_cloud_create_estimated: B2_CLOUD_NO_REORDER does not apply (the points keep the input cloud's order)");
   B2_REQUIRE(tree == nullptr || tree->cloud_uid == cloud->uid, "b2_cloud_create_estimated: the tree was not built by b2_kdtree_create_from_cloud from this cloud");

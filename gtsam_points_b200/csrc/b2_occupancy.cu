@@ -381,6 +381,7 @@ b2_status grow(b2_occgrid& g, size_t cap) {
 b2_status check_cloud(const b2_occgrid* g, const b2_cloud* cloud, const double* T, const char* who) {
   B2_REQUIRE(g != nullptr, "%s: grid is NULL", who);
   B2_REQUIRE(cloud != nullptr, "%s: cloud is NULL", who);
+  B2_TRY(require_resident(cloud, who));
   B2_REQUIRE(cloud->ctx->device == g->ctx->device, "%s: the cloud lives on device %d, the grid on device %d", who, cloud->ctx->device, g->ctx->device);
   if (T) B2_TRY(check_pose(T, who));
   return B2_OK;

@@ -896,6 +896,7 @@ b2_status create_features(bool pfh, const char* who, const b2_cloud* cloud, cons
   B2_REQUIRE(out != nullptr, "%s: out is NULL", who);
   *out = nullptr;
   B2_REQUIRE(cloud != nullptr, "%s: cloud is NULL", who);
+  B2_TRY(require_resident(cloud, who));
   if (!cloud->d_normals) return fail(B2_ERR_INVALID_STATE, "%s: the cloud has no normals", who);
   B2_REQUIRE(search_radius >= 0.0 && std::isfinite(search_radius), "%s: search_radius must be finite and >= 0 (got %g)", who, search_radius);
   B2_REQUIRE(tree == nullptr || tree->cloud_uid == cloud->uid, "%s: the tree was not built by b2_kdtree_create_from_cloud from this cloud", who);
@@ -1053,6 +1054,8 @@ b2_status b2_estimate_pose_ransac(const b2_cloud* target, const b2_cloud* source
                                   const b2_ransac_params* params, b2_registration_result* out, int32_t* out_hypothesis_inliers) {
   const char* who = "b2_estimate_pose_ransac";
   B2_REQUIRE(target && source && params && out, "%s: NULL argument", who);
+  B2_TRY(require_resident(target, who, "the target cloud"));
+  B2_TRY(require_resident(source, who, "the source cloud"));
   B2_TRY(check_features(target_features, who));
   B2_TRY(check_features(source_features, who));
   const b2_ransac_params& p = *params;
@@ -1178,6 +1181,8 @@ b2_status b2_estimate_pose_gnc(const b2_cloud* target, const b2_cloud* source, c
                                const b2_gnc_params* params, b2_registration_result* out, int64_t* out_correspondences, size_t capacity, size_t* out_num_correspondences) {
   const char* who = "b2_estimate_pose_gnc";
   B2_REQUIRE(target && source && params && out, "%s: NULL argument", who);
+  B2_TRY(require_resident(target, who, "the target cloud"));
+  B2_TRY(require_resident(source, who, "the source cloud"));
   B2_TRY(check_features(target_features, who));
   B2_TRY(check_features(source_features, who));
   const b2_gnc_params& p = *params;

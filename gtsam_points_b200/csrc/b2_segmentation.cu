@@ -614,6 +614,7 @@ b2_status b2_region_growing_create(const b2_cloud* cloud, const b2_kdtree* tree,
   B2_REQUIRE(out != nullptr, "%s: out is NULL", who);
   *out = nullptr;
   B2_REQUIRE(cloud != nullptr, "%s: cloud is NULL", who);
+  B2_TRY(require_resident(cloud, who));
   B2_REQUIRE(seed_point != nullptr, "%s: seed_point is NULL", who);
   B2_REQUIRE(cloud->d_normals, "%s: the cloud has no normals", who);
   B2_REQUIRE(std::isfinite(seed_point[0]) && std::isfinite(seed_point[1]) && std::isfinite(seed_point[2]), "%s: seed_point must be finite", who);
@@ -676,6 +677,7 @@ b2_status b2_min_cut(const b2_cloud* cloud, const b2_kdtree* tree, int64_t sourc
                      b2_min_cut_result* info, int64_t* out_indices, int64_t* out_capacities) {
   const char* who = "b2_min_cut";
   B2_REQUIRE(cloud != nullptr, "%s: cloud is NULL", who);
+  B2_TRY(require_resident(cloud, who));
   B2_REQUIRE(params != nullptr && info != nullptr, "%s: params or info is NULL", who);
   B2_REQUIRE(cloud->d_normals, "%s: the cloud has no normals", who);
   const b2_min_cut_params& p = *params;

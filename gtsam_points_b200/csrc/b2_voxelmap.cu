@@ -385,14 +385,14 @@ b2_status reserve_voxels(b2_voxelmap* vm, size_t want) {
   });
 }
 
-// (re)build the bucket table over the current voxels; resized when the load factor bound asks for it
-b2_status rebuild_table(b2_voxelmap* vm) {
-  cudaStream_t st = vm->ctx->stream;
+// (re)build the bucket table over the current voxels on `st`; resized when the load factor bound asks for it
+b2_status rebuild_table(b2_voxelmap* vm, cudaStream_t st) {
   const size_t nb = bucket_count_for(vm->num_voxels);
   if (nb != vm->num_buckets) {
     DeviceBuffer fresh;
     B2_TRY(fresh.alloc(nb * sizeof(VoxelBucket)));
-    B2_CUDA(cudaStreamSynchronize(st));
+    // queued work may still read the table that is replaced; a reloaded map has none, so its reload does not drain the stream
+    if (vm->d_buckets) B2_CUDA(cudaStreamSynchronize(st));
     vm->d_buckets = std::move(fresh);
     vm->num_buckets = nb;
   }
@@ -405,6 +405,7 @@ b2_status rebuild_table(b2_voxelmap* vm) {
   vm->generation++;
   return B2_OK;
 }
+b2_status rebuild_table(b2_voxelmap* vm) { return rebuild_table(vm, vm->ctx->stream); }
 
 
 // ---- voxel-keyed insertion, shared by the Gaussian voxel map and the iVox ----
@@ -550,6 +551,10 @@ template <typename Cell, typename OnChange>
 b2_status insert_batch(b2_voxelmap* vm, int slots, const Cell& cell, OnChange&& on_change, const double* d_points, int point_stride, const double* d_covs, int cov_stride,
                        const double* d_ints, size_t n, const char* who) {
   cudaStream_t st = vm->ctx->stream;
+  if (!vm->host.empty()) {  // the map changes: a host copy from an earlier offload no longer describes it
+    B2_CUDA(cudaStreamSynchronize(st));  // a reload issued on another stream may still copy from it (this stream waits for that)
+    vm->host.reset();
+  }
   if (n > 0) {
     const size_t V_old = vm->num_voxels;
     BatchSegments sg;
@@ -618,6 +623,7 @@ b2_status insert_cloud(b2_voxelmap* vm, int slots, const Cell& cell, OnChange&& 
 // The checks every *_insert_cloud makes before the map changes: the frame handle, its device, the pose (NULL allowed).
 b2_status check_insert_cloud(const b2_voxelmap& vm, const b2_cloud* frame, const double* T, const char* who) {
   B2_REQUIRE(frame != nullptr, "%s: frame is NULL", who);
+  B2_TRY(require_resident(frame, who, "the frame"));
   B2_REQUIRE(frame->ctx->device == vm.ctx->device, "%s: the frame lives on device %d, the map on device %d", who, frame->ctx->device, vm.ctx->device);
   if (T) B2_TRY(check_pose(T, who));
   return B2_OK;
@@ -944,7 +950,91 @@ b2_status ivox_enable_plane_view(const b2_ivox* iv) {
   return B2_OK;
 }
 
+namespace b2 {
+namespace {
+// Reload of an offloaded Gaussian map on `st`: the per-voxel arrays back at their capacity (intensities beyond num_voxels zeroed, as
+// growth leaves them), then the bucket table rebuilt from the coordinates (a generation bump).  On a failed allocation the map
+// stays offloaded with its host copy.
+b2_status voxelmap_reload(b2_voxelmap* vm, cudaStream_t st) {
+  B2_TRY(reload_arrays({&vm->d_records, &vm->d_coords, &vm->d_lru, &vm->d_intensities}, {false, false, false, true}, st, vm->host));
+  const b2_status s = rebuild_table(vm, st);
+  if (s != B2_OK) {
+    vm->d_records.reset(), vm->d_coords.reset(), vm->d_lru.reset(), vm->d_intensities.reset(), vm->d_buckets.reset();
+    vm->num_buckets = 0;
+    return s;
+  }
+  B2_TRY(stream_after(vm->ctx->stream, st));
+  vm->offloaded = false;
+  return B2_OK;
+}
+}  // namespace
+
+b2_status voxelmap_touch(b2_voxelmap* vm, cudaStream_t st, bool* changed) {
+  vm->last_access = access_clock_tick();
+  if (changed) *changed = false;
+  if (!vm->offloaded) return B2_OK;
+  B2_TRY(voxelmap_reload(vm, st));
+  if (changed) *changed = true;
+  return B2_OK;
+}
+
+}  // namespace b2
+
 extern "C" {
+
+// GaussianVoxelMapGPU::offload_gpu: the records, coordinates, LRU stamps and intensities of the map's voxels into one pinned host
+// block (kept until the next insert), then every device buffer is freed, the bucket table included.
+b2_status b2_voxelmap_offload(b2_voxelmap* vm, int* changed) {
+  B2_REQUIRE(vm != nullptr, "b2_voxelmap_offload: vm is NULL");
+  if (changed) *changed = 0;
+  if (vm->offloaded) return B2_OK;
+  B2_ON_DEVICE(vm->ctx);
+  cudaStream_t st = vm->ctx->stream;
+  const size_t V = vm->num_voxels;
+  if (vm->host.empty()) {
+    B2_TRY(offload_arrays({&vm->d_records, &vm->d_coords, &vm->d_lru, &vm->d_intensities},
+                          {V * kRecordDoubles * sizeof(double), V * 3 * sizeof(int32_t), V * sizeof(uint32_t), V * sizeof(double)}, st, vm->host));
+  } else {
+    B2_CUDA(cudaStreamSynchronize(st));  // queued work may still read the arrays
+  }
+  vm->d_records.reset(), vm->d_coords.reset(), vm->d_lru.reset(), vm->d_intensities.reset(), vm->d_buckets.reset();
+  vm->num_buckets = 0;  // rebuild_table reallocates the table only when the bucket count changes
+  vm->offloaded = true;
+  if (changed) *changed = 1;
+  return B2_OK;
+}
+
+b2_status b2_voxelmap_reload(b2_voxelmap* vm, int* changed) {
+  B2_REQUIRE(vm != nullptr, "b2_voxelmap_reload: vm is NULL");
+  if (changed) *changed = 0;
+  if (!vm->offloaded) return B2_OK;
+  B2_ON_DEVICE(vm->ctx);
+  B2_TRY(voxelmap_reload(vm, vm->ctx->stream));
+  B2_CUDA(cudaStreamSynchronize(vm->ctx->stream));
+  if (changed) *changed = 1;
+  return B2_OK;
+}
+
+b2_status b2_voxelmap_touch(b2_voxelmap* vm, int* changed) {
+  B2_REQUIRE(vm != nullptr, "b2_voxelmap_touch: vm is NULL");
+  if (changed) *changed = 0;
+  B2_ON_DEVICE(vm->ctx);
+  bool reloaded = false;
+  B2_TRY(voxelmap_touch(vm, vm->ctx->stream, &reloaded));
+  if (reloaded) B2_CUDA(cudaStreamSynchronize(vm->ctx->stream));
+  if (changed) *changed = reloaded ? 1 : 0;
+  return B2_OK;
+}
+
+b2_status b2_voxelmap_residency(const b2_voxelmap* vm, b2_residency* out) {
+  B2_REQUIRE(vm && out, "b2_voxelmap_residency: NULL argument");
+  out->loaded_on_gpu = vm->offloaded ? 0 : 1;
+  out->reserved = 0;
+  out->last_access = vm->last_access;
+  out->device_bytes = vm->device_bytes();
+  out->host_bytes = vm->host.block.bytes();
+  return B2_OK;
+}
 
 b2_status b2_voxelmap_create_from_voxels(b2_ctx* ctx, double resolution, const int32_t* coords, const double* means, const double* covs,
                                          const int32_t* num_points, size_t V, b2_voxelmap** out) {
@@ -1036,6 +1126,7 @@ b2_status b2_voxelmap_insert(b2_voxelmap* vm, const double* points, int point_st
 b2_status b2_voxelmap_insert_with_intensities(b2_voxelmap* vm, const double* points, int point_stride, const double* covs, int cov_stride, const double* intensities,
                                               size_t n) {
   B2_REQUIRE(vm != nullptr, "b2_voxelmap_insert: vm is NULL");
+  B2_TRY(require_resident(vm, intensities ? "b2_voxelmap_insert_with_intensities" : "b2_voxelmap_insert"));
   B2_REQUIRE(point_stride == 3 || point_stride == 4, "b2_voxelmap_insert: point_stride must be 3 or 4");
   B2_REQUIRE(cov_stride == 9 || cov_stride == 16, "b2_voxelmap_insert: cov_stride must be 9 or 16");
   B2_REQUIRE(n == 0 || (points && covs), "error: points/covs have not been allocated!!");  // GaussianVoxel::add reads covs
@@ -1050,6 +1141,7 @@ b2_status b2_voxelmap_insert_with_intensities(b2_voxelmap* vm, const double* poi
 // intensities when it has them.
 b2_status b2_voxelmap_insert_cloud(b2_voxelmap* vm, const b2_cloud* frame, const double* T_map_frame) {
   B2_REQUIRE(vm != nullptr, "b2_voxelmap_insert_cloud: vm is NULL");
+  B2_TRY(require_resident(vm, "b2_voxelmap_insert_cloud"));
   B2_TRY(check_insert_cloud(*vm, frame, T_map_frame, "b2_voxelmap_insert_cloud"));
   B2_REQUIRE(frame->n == 0 || frame->d_covs, "b2_voxelmap_insert_cloud: the frame has no covariances");  // GaussianVoxel::add reads covs
   B2_ON_DEVICE(vm->ctx);
@@ -1093,6 +1185,7 @@ b2_status b2_voxelmap_get_info(const b2_voxelmap* vm, b2_voxelmap_info* info) {
 
 b2_status b2_voxelmap_download(const b2_voxelmap* vm, int32_t* coords, double* means, double* covs, int32_t* num_points) {
   B2_REQUIRE(vm != nullptr, "b2_voxelmap_download: vm is NULL");
+  B2_TRY(require_resident(vm, "b2_voxelmap_download"));
   const size_t V = vm->num_voxels;
   if (V == 0) return B2_OK;
   B2_ON_DEVICE(vm->ctx);
@@ -1113,6 +1206,7 @@ b2_status b2_voxelmap_download(const b2_voxelmap* vm, int32_t* coords, double* m
 
 b2_status b2_voxelmap_download_intensities(const b2_voxelmap* vm, double* intensities) {
   B2_REQUIRE(vm != nullptr && (intensities != nullptr || vm->num_voxels == 0), "b2_voxelmap_download_intensities: NULL argument");
+  B2_TRY(require_resident(vm, "b2_voxelmap_download_intensities"));
   const size_t V = vm->num_voxels;
   if (V == 0) return B2_OK;
   if (!vm->d_intensities) {  // no insert brought intensities: every voxel holds the initial 0
@@ -1139,6 +1233,7 @@ static_assert(sizeof(GaussianVoxelData) == 56, "GaussianVoxelData layout");
 
 b2_status b2_voxelmap_save_compact(const b2_voxelmap* vm, const char* path) {
   B2_REQUIRE(vm && path, "b2_voxelmap_save_compact: NULL argument");
+  B2_TRY(require_resident(vm, "b2_voxelmap_save_compact"));
   const size_t V = vm->num_voxels;
   std::vector<int32_t> coords(V * 3), cnt(V);
   std::vector<double> means(V * 3), covs(V * 9), ints(V);
@@ -1205,14 +1300,19 @@ b2_status b2_voxelmap_load(b2_ctx* ctx, const char* path, b2_voxelmap** out) {
 
 b2_status b2_overlap(const b2_voxelmap* const* targets, size_t num_targets, const b2_cloud* source, const double* Ts_target_source, double* out_overlap) {
   B2_REQUIRE(targets && source && Ts_target_source && out_overlap && num_targets > 0, "b2_overlap: NULL / empty argument");
-  B2_REQUIRE(source->d_points, "error: source points have not been allocated!!");
+  B2_REQUIRE(source->offloaded || source->d_points, "error: source points have not been allocated!!");
   b2_ctx* ctx = source->ctx;
-  B2_ON_DEVICE(ctx);
-  cudaStream_t st = ctx->stream;
-  std::vector<OverlapMap> maps(num_targets);
   for (size_t j = 0; j < num_targets; j++) {
     B2_REQUIRE(targets[j] != nullptr, "error: Failed to cast target voxelmap to GaussianVoxelMapGPU!!");  // gaussian_voxelmap_gpu_funcs.cu:70-75
     B2_REQUIRE(targets[j]->ctx->device == ctx->device, "b2_overlap: map %zu lives on another device", j);
+  }
+  B2_ON_DEVICE(ctx);
+  cudaStream_t st = ctx->stream;
+  // overlap_gpu touches what it reads, the targets and then the source (gaussian_voxelmap_gpu_funcs.cu), reloading what is offloaded
+  for (size_t j = 0; j < num_targets; j++) B2_TRY(voxelmap_touch(const_cast<b2_voxelmap*>(targets[j]), st, nullptr));
+  B2_TRY(cloud_touch(const_cast<b2_cloud*>(source), st, nullptr));
+  std::vector<OverlapMap> maps(num_targets);
+  for (size_t j = 0; j < num_targets; j++) {
     maps[j].table = targets[j]->table();
     std::memcpy(maps[j].T, Ts_target_source + 16 * j, 12 * sizeof(double));
   }
@@ -1239,6 +1339,7 @@ b2_status b2_overlap(const b2_voxelmap* const* targets, size_t num_targets, cons
 
 b2_status b2_voxelmap_lookup(const b2_voxelmap* vm, const double* points, int point_stride, size_t n, int32_t* out_index) {
   B2_REQUIRE(vm && (n == 0 || (points && out_index)), "b2_voxelmap_lookup: NULL argument");
+  B2_TRY(require_resident(vm, "b2_voxelmap_lookup"));
   B2_REQUIRE(point_stride == 3 || point_stride == 4, "b2_voxelmap_lookup: point_stride must be 3 or 4");
   if (n == 0) return B2_OK;
   B2_ON_DEVICE(vm->ctx);

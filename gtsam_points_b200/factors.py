@@ -126,6 +126,26 @@ class IntegratedMatchingCostFactor:
         """Device bytes the factor owns itself (correspondence array + linearization point); clouds / maps are shared."""
         return self.source.size() * 4 + 16 * 8
 
+    def memory_usage_gpu(self) -> int:
+        """Device bytes the factor owns itself (b2_factor_device_bytes): correspondences, gathered kd-tree target records and the
+        linearization point; the clouds and maps it reads report their own (memory_usage_gpu)."""
+        out = C.c_uint64()
+        capi.check(capi.lib().b2_factor_device_bytes(self.h, C.byref(out)))
+        return out.value
+
+    def set_enable_offloading(self, enable: bool):
+        """IntegratedVGICPFactorGPU::set_enable_offloading, on every factor kind: each linearize / error touches what the factor
+        reads (a VGICP factor's target map, then the source cloud), reloading what was offloaded.  Off (the default), a call that
+        would read an offloaded object raises."""
+        capi.check(capi.lib().b2_factor_set_enable_offloading(self.h, 1 if enable else 0))
+        self._offloading = bool(enable)
+
+    def _carry_settings(self, f):
+        """clone(): the copy takes this factor's offloading setting"""
+        if getattr(self, "_offloading", False):
+            f.set_enable_offloading(True)
+        return f
+
     # -- tuning knobs of the reference, accepted for drop-in compatibility ------------------------------------------
     def set_num_threads(self, n: int):
         """The device path has no thread knob (integrated_vgicp_factor.hpp:71-73, integrated_gicp_factor.hpp:95-97)."""
@@ -174,7 +194,7 @@ class IntegratedVGICPFactor(IntegratedMatchingCostFactor):
         f = IntegratedVGICPFactor(a0, a1, self.target_voxels, self.source, ctx=self.ctx)
         if getattr(self, "_surface_validation", False):
             f.set_enable_surface_validation(True)
-        return f
+        return self._carry_settings(f)
 
 
 IntegratedVGICPFactorGPU = IntegratedVGICPFactor
@@ -222,7 +242,7 @@ class IntegratedGICPFactor(IntegratedMatchingCostFactor):
     def clone(self):
         a0 = self._keys[0] if self.is_binary else self.fixed_target_pose
         a1 = self._keys[1] if self.is_binary else self._keys[0]
-        return IntegratedGICPFactor(a0, a1, self.target, self.source, target_tree=self.target_tree, ctx=self.ctx)
+        return self._carry_settings(IntegratedGICPFactor(a0, a1, self.target, self.source, target_tree=self.target_tree, ctx=self.ctx))
 
 
 class IntegratedICPFactor(IntegratedMatchingCostFactor):
@@ -273,7 +293,7 @@ class IntegratedICPFactor(IntegratedMatchingCostFactor):
     def clone(self):
         a0 = self._keys[0] if self.is_binary else self.fixed_target_pose
         a1 = self._keys[1] if self.is_binary else self._keys[0]
-        return IntegratedICPFactor(a0, a1, self.target, self.source, target_tree=self.target_tree, use_point_to_plane=self.use_point_to_plane, ctx=self.ctx)
+        return self._carry_settings(IntegratedICPFactor(a0, a1, self.target, self.source, target_tree=self.target_tree, use_point_to_plane=self.use_point_to_plane, ctx=self.ctx))
 
 
 class IntegratedPointToPlaneICPFactor(IntegratedICPFactor):

@@ -56,13 +56,61 @@ def default_context(device: int = 0) -> Context:
         return _default_ctx[device]
 
 
-class PointCloud:
+def current_access_time() -> int:
+    """OffloadableGPU::current_access_time: the process-wide access clock that touch() advances."""
+    out = C.c_uint64()
+    capi.check(capi.lib().b2_access_time_current(C.byref(out)))
+    return out.value
+
+
+class OffloadableGPU:
+    """OffloadableGPU (include/gtsam_points/types/offloadable.hpp): the device copy can be moved to pinned host memory
+    (offload_gpu) and back (reload_gpu), and touch() records an access and reloads if needed.  Each returns whether it moved
+    anything.  While offloaded, calls that read the device copy raise B2Error (B2_ERR_INVALID_STATE) -- except overlap_gpu and
+    factor launches with set_enable_offloading(True), which touch what they read.  Which objects to offload is the caller's
+    choice; nothing is evicted automatically."""
+
+    _residency_api = ""  # the C ABI prefix of the handle: b2_cloud / b2_voxelmap
+
+    def _residency_call(self, op: str) -> bool:
+        changed = C.c_int32()
+        capi.check(getattr(capi.lib(), f"{self._residency_api}_{op}")(self.h, C.byref(changed)))
+        return bool(changed.value)
+
+    def offload_gpu(self) -> bool:
+        return self._residency_call("offload")
+
+    def reload_gpu(self) -> bool:
+        return self._residency_call("reload")
+
+    def touch(self) -> bool:
+        return self._residency_call("touch")
+
+    def residency(self) -> capi.Residency:
+        out = capi.Residency()
+        capi.check(getattr(capi.lib(), f"{self._residency_api}_residency")(self.h, C.byref(out)))
+        return out
+
+    def loaded_on_gpu(self) -> bool:
+        return bool(self.residency().loaded_on_gpu)
+
+    def last_accessed_time(self) -> int:
+        return int(self.residency().last_access)
+
+    def memory_usage_gpu(self) -> int:
+        """Device bytes the object holds now: 0 while offloaded."""
+        return int(self.residency().device_bytes)
+
+
+class PointCloud(OffloadableGPU):
     """Points (N x 3 or N x 4 float64) with optional covariances (N x 3 x 3 or N x 4 x 4 float64), normals (N x 3 or N x 4) and
     intensities (N).
 
     The device copy (`points_gpu` / `covs_gpu` / `normals_gpu` / `intensities_gpu` in the reference) is created on construction.
     flags: capi.B2_CLOUD_* (default lossless storage, Morton-ordered on the device).
     """
+
+    _residency_api = "b2_cloud"
 
     def __init__(self, points, covs=None, ctx: Context | None = None, flags: int = capi.B2_CLOUD_DEFAULT, normals=None, intensities=None):
         self.ctx = ctx or default_context()
@@ -176,14 +224,33 @@ class PointCloud:
             pass
 
 
-class GaussianVoxelMapGPU:
+class GaussianVoxelMapGPU(OffloadableGPU):
     """Gaussian voxel map on the device with the CPU map's index semantics (first-touch ids, exact lookups)."""
+
+    _residency_api = "b2_voxelmap"
+
+    # The device map is made by the first insert (or set_lru / touch).  Until then the map holds no device memory, so offload_gpu /
+    # reload_gpu move nothing, and last_accessed_time() is the clock's value at construction (the reference's creation stamp); the
+    # device map, once made, records the clock's value at its own creation, as every new device object does.  touch() makes the
+    # device map, so that it has an object to record the access on.
+    def _residency_call(self, op: str) -> bool:
+        if op == "touch":
+            self._ensure()
+        if self.h is None:
+            return False
+        return super()._residency_call(op)
+
+    def residency(self) -> capi.Residency:
+        if self.h is None:
+            return capi.Residency(loaded_on_gpu=1, last_access=self._created_at)
+        return super().residency()
 
     def __init__(self, resolution: float, ctx: Context | None = None):
         self.ctx = ctx or default_context()
         self._resolution = float(resolution)
         self.h = None
         self._lru = None
+        self._created_at = current_access_time()
 
     def voxel_resolution(self) -> float:
         return self._resolution

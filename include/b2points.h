@@ -281,6 +281,58 @@ B2_API b2_status b2_merge_frames_to_cloud(b2_ctx* ctx, const double* poses, cons
 B2_API b2_status b2_voxelmap_lookup(const b2_voxelmap* vm, const double* points, int point_stride, size_t n, int32_t* out_index);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * GPU memory offloading.  OffloadableGPU (include/gtsam_points/types/offloadable.hpp) for device clouds and Gaussian voxel maps:
+ * a caller that holds more clouds and maps than it wants resident moves some of them to host memory and back.  Which objects to
+ * offload and when is the caller's choice; the library has no eviction policy.
+ *
+ *   offload  copies every device array of the object into one pinned host block (cudaHostAlloc) on the object's context stream,
+ *            synchronises that stream and frees the device buffers.  A cloud: points, covariances, normals, permutation and
+ *            intensities.  A map: the records, coordinates, LRU stamps and intensities of its voxels; its bucket table is not
+ *            copied but freed.  *changed = 1 if the object was resident.
+ *   reload   allocates the arrays again and copies them back; a map rebuilds its bucket table from the coordinates.  Voxel ids,
+ *            correspondences and every factor result are the same as before the offload, bit for bit; only device addresses
+ *            change.  If an allocation fails, whatever was allocated is freed and B2_ERR_OUT_OF_MEMORY is returned: the object
+ *            stays offloaded with its host copy.  *changed = 1 if the object was offloaded.
+ *   touch    last_access = clock++ (one process-wide counter), then reload if offloaded (OffloadableGPU::touch); *changed = 1 if
+ *            it reloaded.
+ * Each object records the clock's value at creation as its last_access.  offload / reload / touch return once the object's
+ * stream has finished the copies.  `changed` may be NULL.
+ *
+ * A cloud never changes, so its host copy is kept until it is destroyed, and a second offload only frees device memory.  A map's
+ * host copy is dropped by the first insert after a reload; the next offload copies again.
+ *
+ * Differences from the reference:
+ *   - The reference reads NULL device pointers when an offloaded object is used without a touch.  Here every entry point that
+ *     reads the device arrays of an offloaded cloud or map returns B2_ERR_INVALID_STATE and changes nothing: downloads, inserts,
+ *     insert_cloud, kd-tree builds, every cloud producer and filter, features, segmentation, occupancy grids, save_compact,
+ *     lookup, correspondences and factor creation.  Only the reference's touch points reload: b2_overlap (it touches its targets,
+ *     then its source) and factor launches with offloading on (b2_factor_set_enable_offloading).  get_info works on an offloaded
+ *     object and reports device_bytes = 0; destroy works in either state.
+ *   - The reference copies a map's bucket table to the host and back; this map rebuilds the table on reload, which saves the
+ *     table's host memory and copy bytes.  Lookups are exact, so no result depends on where a voxel sits in the table.
+ *   - The host copy is pinned memory, so the copies run at full bus bandwidth.
+ *   - Offloading in factor launches is available on every factor kind, not on the VGICP factor only.
+ * Only Gaussian voxel maps and device clouds offload: kd-trees, iVox maps, features, occupancy grids and factor-owned buffers stay
+ * on the device. */
+typedef struct b2_residency {
+  int32_t loaded_on_gpu; /* 1 = resident, 0 = offloaded */
+  int32_t reserved;
+  uint64_t last_access;  /* OffloadableGPU::last_accessed_time */
+  uint64_t device_bytes; /* device memory the object holds now (0 while offloaded); OffloadableGPU::memory_usage_gpu */
+  uint64_t host_bytes;   /* pinned host memory its host copy holds (0 if none) */
+} b2_residency;
+B2_API b2_status b2_cloud_offload(b2_cloud* cloud, int* changed);
+B2_API b2_status b2_cloud_reload(b2_cloud* cloud, int* changed);
+B2_API b2_status b2_cloud_touch(b2_cloud* cloud, int* changed);
+B2_API b2_status b2_cloud_residency(const b2_cloud* cloud, b2_residency* out);
+B2_API b2_status b2_voxelmap_offload(b2_voxelmap* vm, int* changed);
+B2_API b2_status b2_voxelmap_reload(b2_voxelmap* vm, int* changed);
+B2_API b2_status b2_voxelmap_touch(b2_voxelmap* vm, int* changed);
+B2_API b2_status b2_voxelmap_residency(const b2_voxelmap* vm, b2_residency* out);
+/* OffloadableGPU::current_access_time: the clock's current value */
+B2_API b2_status b2_access_time_current(uint64_t* out);
+
+/* ------------------------------------------------------------------------------------------------------------
  * iVox.  Replaces IncrementalVoxelMap<FlatContainer> / iVox (include/gtsam_points/ann/ivox.hpp,
  * ann/incremental_voxelmap.hpp:36-130, ann/impl/incremental_voxelmap_impl.hpp, ann/flat_container.hpp:14-80): an incremental
  * point map for frame-to-map odometry.  Points are kept (up to max_num_points_in_cell per voxel, at least min_dist_in_cell
@@ -938,6 +990,19 @@ B2_API b2_status b2_factor_set_correspondence_update_tolerance(b2_factor* f, dou
  * carry normals (B2_ERR_INVALID_STATE); default off.  Takes effect at the next correspondence update. */
 B2_API b2_status b2_factor_set_enable_surface_validation(b2_factor* f, int enable);
 B2_API size_t b2_factor_num_points(const b2_factor* f);
+/* IntegratedVGICPFactorGPU::set_enable_offloading (integrated_vgicp_factor_gpu.hpp), for every factor kind.  When on, every launch
+ * of a set holding the factor -- the set calls, the single-factor calls, issue_* and the b2_exchange_* calls -- first touches what
+ * the factor reads, in set order: a VGICP factor's target map, then the source cloud.  What is offloaded is reloaded on the set's
+ * context stream (a context with another stream waits for it).  kd-tree factors read the target records they gathered at
+ * creation, so their target cloud may stay offloaded.  When off (the default), a launch of a set in which such a factor would
+ * read an offloaded object returns B2_ERR_INVALID_STATE naming the member, launches nothing and touches nothing.  This check
+ * looks at the objects as they are when the call starts, before any touch: it fails even when another member of the set, with
+ * offloading on, would have reloaded the same shared map or cloud earlier in the set order.  Turn offloading on for every
+ * member that shares an object that may be offloaded. */
+B2_API b2_status b2_factor_set_enable_offloading(b2_factor* f, int enable);
+/* Device memory the factor owns itself (correspondences, gathered kd-tree target records, linearization point); the clouds and
+ * maps it reads are counted on those objects. */
+B2_API b2_status b2_factor_device_bytes(const b2_factor* f, uint64_t* out);
 /* Correspondences frozen at the last linearize, in the caller's point order: VGICP voxel id / GICP target index, -1 = none
  * (IntegratedVGICPFactor_::correspondences, integrated_vgicp_factor.hpp:107; IntegratedGICPFactor_::correspondences :147). */
 B2_API b2_status b2_factor_correspondences(const b2_factor* f, int64_t* out);

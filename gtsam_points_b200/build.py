@@ -16,7 +16,7 @@ LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(HERE, "build")
 LIB = os.path.join(LIBDIR, "libb2points.so")
 
-SOURCES = ["b2_context.cu", "b2_cloud.cu", "b2_voxelmap.cu", "b2_kdtree.cu", "b2_factors.cu", "b2_registration.cu", "b2_filter.cu", "b2_segmentation.cu", "b2_occupancy.cu"]
+SOURCES = ["b2_context.cu", "b2_cloud.cu", "b2_voxelmap.cu", "b2_kdtree.cu", "b2_factors.cu", "b2_registration.cu", "b2_filter.cu", "b2_segmentation.cu", "b2_occupancy.cu", "b2_optimize.cu"]
 HEADERS = ["b2_internal.hpp", "b2_device.cuh", "b2_kdtree.cuh", "b2_factor_kernel_ws.cuh", os.path.join("..", "..", "include", "b2points.h")]
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
@@ -29,6 +29,9 @@ NVCC_FLAGS = [
     "-Xcudafe", "--diag_suppress=177",
 ]
 
+# The pose optimizer's loop arithmetic is restated on the host bit for bit: no fused multiply-adds, on the device or the host.
+EXTRA_FLAGS = {"b2_optimize.cu": ["-fmad=false", "-Xcompiler", "-ffp-contract=off"]}
+
 
 def _mtime(p):
     return os.path.getmtime(p) if os.path.exists(p) else 0.0
@@ -39,7 +42,7 @@ def _compile(src, verbose):
     deps = [os.path.join(CSRC, src)] + [os.path.join(CSRC, h) for h in HEADERS]
     if _mtime(obj) > max(_mtime(d) for d in deps):
         return obj, False
-    cmd = [NVCC] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-c", os.path.join(CSRC, src), "-o", obj]
+    cmd = [NVCC] + NVCC_FLAGS + EXTRA_FLAGS.get(src, []) + (["-Xptxas", "-v"] if verbose else []) + ["-c", os.path.join(CSRC, src), "-o", obj]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"nvcc failed for {src}:\n{r.stdout}\n{r.stderr}")

@@ -87,6 +87,26 @@ class RegistrationResultC(C.Structure):
     _fields_ = [("T_target_source", C.c_double * 16), ("inlier_rate", C.c_double), ("num_inliers", C.c_int64), ("hypothesis", C.c_int64)]
 
 
+class LmParamsC(C.Structure):
+    _fields_ = [("max_iterations", C.c_int32), ("reserved", C.c_int32), ("relative_error_tol", C.c_double), ("absolute_error_tol", C.c_double),
+                ("error_tol", C.c_double), ("lambda_initial", C.c_double), ("lambda_factor", C.c_double), ("lambda_upper_bound", C.c_double),
+                ("lambda_lower_bound", C.c_double), ("min_model_fidelity", C.c_double)]
+
+
+class LmSummaryC(C.Structure):
+    _fields_ = [("iterations", C.c_int64), ("outer_iterations", C.c_int64), ("inner_iterations", C.c_int64), ("linearizations", C.c_int64),
+                ("error_evaluations", C.c_int64), ("error0", C.c_double), ("error", C.c_double), ("lambda_", C.c_double), ("termination", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
+class LmTraceEntryC(C.Structure):
+    _fields_ = [("outer", C.c_int32), ("solved", C.c_int32), ("success", C.c_int32), ("stop", C.c_int32), ("lambda_", C.c_double),
+                ("T_lin", C.c_double * 16), ("G", C.c_double * 36), ("g", C.c_double * 6), ("error", C.c_double), ("half_f", C.c_double),
+                ("d", C.c_double * 6), ("lin_change", C.c_double), ("T_trial", C.c_double * 16), ("error_trial", C.c_double), ("fidelity", C.c_double)]
+
+
+B2_LM_TERMINATION = {0: "none", 1: "max_iterations", 2: "non_finite", 3: "absolute_error_tol", 4: "relative_error_tol", 5: "error_tol", 6: "try_limit"}
+
 _lib = None
 
 # name -> (restype, argtypes); every symbol include/b2points.h declares
@@ -249,6 +269,8 @@ SIGNATURES = {
     "b2_exchange_errors": (_vp, [_vp, C.c_uint]),
     "b2_exchange_barrier": (C.c_int, [_vp]),
     "b2_factor_set_launch_count": (C.c_uint64, [_vp]),
+    "b2_lm_params_default": (None, [C.POINTER(LmParamsC)]),
+    "b2_factor_set_optimize_pose": (C.c_int, [_vp, _dp, _dp, C.POINTER(LmParamsC), _dp, C.POINTER(LmSummaryC), C.POINTER(LmTraceEntryC), C.c_size_t, C.POINTER(C.c_size_t)]),
 }
 
 

@@ -1282,6 +1282,8 @@ public:
     return c;
   }
   b2_factor* handle() const { return factor_; }
+  bool is_binary() const { return is_binary_; }
+  const Mat4& fixed_target_pose() const { return fixed_target_pose_; }  // identity for a binary factor
 
   // IntegratedVGICPFactorGPU::set_enable_offloading, on every factor kind: each linearize / error first touches what the factor
   // reads (a VGICP factor's target map, then its source cloud), reloading what was offloaded.  clone() carries it over.
@@ -1732,6 +1734,9 @@ public:
     for (std::size_t i = 0; i < factors_.size(); i++) factors_[i]->store_computed_error(&errors_[i]);
   }
 
+  // optimize_pose_gpu over this set's members (unary factors on one source key), reusing the set and its cached graph from call to call
+  Mat4 optimize_pose(const Mat4& T_init, const b2_lm_params* params = nullptr, b2_lm_summary* summary = nullptr);
+
   std::vector<LinearFactorPtr> calc_linear_factors(const Values& linearization_point) override {
     linearize(linearization_point);
     std::vector<LinearFactorPtr> out(factors_.size());
@@ -1763,5 +1768,47 @@ private:
 
 // what user code hands to LinearizationHook::register_hook (src/demo/demo_matching_cost_factors.cpp:52)
 inline std::shared_ptr<FactorSetBase> create_nonlinear_factor_set_gpu() { return std::make_shared<NonlinearFactorSetGPU>(); }
+
+namespace detail {
+// b2_factor_set_optimize_pose on `set`, whose members are `factors` in order (unary, one source key)
+template <class Factors>
+Mat4 optimize_pose_on(b2_factor_set* set, const Factors& factors, const Mat4& T_init, const b2_lm_params* params, b2_lm_summary* summary) {
+  if (factors.empty()) throw std::invalid_argument("optimize_pose_gpu: no factors");
+  std::vector<double> targets;
+  for (const auto& f : factors) {
+    if (f->is_binary()) throw std::invalid_argument("optimize_pose_gpu: binary factors are not supported");
+    if (f->keys()[0] != factors[0]->keys()[0]) throw std::invalid_argument("optimize_pose_gpu: the factors act on different source keys");
+    targets.insert(targets.end(), f->fixed_target_pose().begin(), f->fixed_target_pose().end());
+  }
+  b2_lm_params p;
+  if (params) p = *params;
+  else b2_lm_params_default(&p);
+  Mat4 out{};
+  check(b2_factor_set_optimize_pose(set, targets.data(), T_init.data(), &p, out.data(), summary, nullptr, 0, nullptr), "b2_factor_set_optimize_pose");
+  return out;
+}
+}  // namespace detail
+
+inline Mat4 NonlinearFactorSetGPU::optimize_pose(const Mat4& T_init, const b2_lm_params* params, b2_lm_summary* summary) {
+  if (factors_.empty()) throw std::invalid_argument("optimize_pose_gpu: no factors");
+  ensure();
+  return detail::optimize_pose_on(set_, factors_, T_init, params, summary);
+}
+
+// LevenbergMarquardtOptimizerExt::optimize() over the pose of unary factors, run on the device as one graph launch
+// (b2_factor_set_optimize_pose; its header comment states the rules and the differences from GTSAM).  Every factor must be unary
+// (constructed with a fixed target pose) and act on the same source key.  params: NULL takes GTSAM's defaults.  Returns the optimized
+// source pose (row-major); summary may be NULL.  This form creates a factor set for the one call, so the call also captures and
+// instantiates the set's graph; a caller that optimizes every frame keeps a NonlinearFactorSetGPU and calls its optimize_pose.
+inline Mat4 optimize_pose_gpu(const std::vector<std::shared_ptr<IntegratedMatchingCostFactorB200>>& factors, const Mat4& T_init, const b2_lm_params* params = nullptr,
+                              b2_lm_summary* summary = nullptr, Context::Ptr ctx = Context::default_context()) {
+  if (factors.empty()) throw std::invalid_argument("optimize_pose_gpu: no factors");
+  std::vector<b2_factor*> hs;
+  for (const auto& f : factors) hs.push_back(f->handle());
+  b2_factor_set* set = nullptr;
+  check(b2_factor_set_create(ctx->get(), hs.data(), hs.size(), &set), "b2_factor_set_create");
+  const std::unique_ptr<b2_factor_set, b2_status (*)(b2_factor_set*)> owned(set, b2_factor_set_destroy);
+  return detail::optimize_pose_on(set, factors, T_init, params, summary);
+}
 
 }  // namespace gtsam_points_b200

@@ -12,6 +12,7 @@
 #include <cstdio>
 #include <cstring>
 #include <initializer_list>
+#include <memory>
 #include <string>
 #include <utility>
 #include <vector>
@@ -467,6 +468,45 @@ inline b2_status check_pose(const double* T, const char* who) {
   return B2_OK;
 }
 
+// ---- correspondence-update tolerance (integrated_gicp_factor_impl.hpp:135-147) ------------------------------------------------
+// Eigen::AngleAxisd(R).angle() the way Eigen computes it (through the quaternion: 2 atan2(|vec|, |w|)) of a row-major 4x4.
+__host__ __device__ inline double rotation_angle_rm(const double* T) {
+  const double m00 = T[0], m11 = T[5], m22 = T[10];
+  double w, q[3];
+  const double tr = m00 + m11 + m22;
+  if (tr > 0.0) {
+    double t = sqrt(tr + 1.0);
+    w = 0.5 * t;
+    t = 0.5 / t;
+    q[0] = (T[9] - T[6]) * t, q[1] = (T[2] - T[8]) * t, q[2] = (T[4] - T[1]) * t;
+  } else {
+    int i = 0;
+    if (m11 > m00) i = 1;
+    if (m22 > T[i * 5]) i = 2;
+    const int j = (i + 1) % 3, k = (j + 1) % 3;
+    double t = sqrt(T[i * 5] - T[j * 5] - T[k * 5] + 1.0);
+    q[i] = 0.5 * t;
+    t = 0.5 / t;
+    w = (T[k * 4 + j] - T[j * 4 + k]) * t;
+    q[j] = (T[j * 4 + i] + T[i * 4 + j]) * t;
+    q[k] = (T[k * 4 + i] + T[i * 4 + k]) * t;
+  }
+  const double n = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2]);
+  return n != 0.0 ? 2.0 * atan2(n, fabs(w)) : 0.0;
+}
+// The pose d (row-major 4x4) is within (tol_rot, tol_trans) of L, the pose of the last correspondence update: diff = d^-1 L.  The
+// host-pose linearize and the device pose optimizer both decide with this.
+__host__ __device__ inline bool within_corr_tolerance(const double* d, const double* L, double tol_rot, double tol_trans) {
+  double diff[16] = {0};
+  for (int r = 0; r < 3; r++) {
+    for (int c = 0; c < 3; c++) diff[r * 4 + c] = d[0 * 4 + r] * L[0 * 4 + c] + d[1 * 4 + r] * L[1 * 4 + c] + d[2 * 4 + r] * L[2 * 4 + c];
+    diff[r * 4 + 3] = d[0 * 4 + r] * (L[3] - d[3]) + d[1 * 4 + r] * (L[7] - d[7]) + d[2 * 4 + r] * (L[11] - d[11]);
+  }
+  const double diff_rot = rotation_angle_rm(diff);
+  const double diff_trans = sqrt(diff[3] * diff[3] + diff[7] * diff[7] + diff[11] * diff[11]);
+  return diff_rot < tol_rot && diff_trans < tol_trans;
+}
+
 }  // namespace b2
 
 // ---- opaque handle definitions -----------------------------------------------------------------
@@ -679,3 +719,39 @@ struct b2_factor {
   // what is offloaded; off, a launch that would read an offloaded object fails
   bool offloading = false;
 };
+
+// ---- factor-set internals the device pose optimizer (b2_optimize.cu) drives -------------------------------------------------
+namespace b2 {
+// The optimizer's cached graph and buffers of one set (b2_optimize.cu); the set owns it and frees it through lm_free.
+struct LmCache;
+void lm_free(LmCache* c);
+struct LmCacheDeleter {
+  void operator()(LmCache* c) const { lm_free(c); }
+};
+
+constexpr int kModeLinearize = 0, kModeError = 1;  // MODE_LINEARIZE / MODE_ERROR of the factor kernels
+
+// The host preparation of a set's launch: residency (make_resident), regrouping after a surface-validation switch, and the refresh
+// of descriptors whose factor, map or source changed since they were built.  Stream-ordered on the context's stream.
+b2_status set_prepare_launch(b2_factor_set* s);
+// The group kernels of one call with device poses (F x 16, read as linearization and evaluation poses in linearize mode, as
+// evaluation poses in error mode) on stream `st`, results to d_out; d_frozen as the kernels read it (NULL: re-associate).  Nothing
+// else: no staging, no synchronisation, and the set's launch count is not changed.  Capturable into a graph.
+b2_status set_launch_groups(b2_factor_set* s, int mode, const double* d_poses, double* d_out, const uint32_t* d_frozen, cudaStream_t st);
+// The set's context, members, its per-member frozen-flag array (F uint32), whether some member has a correspondence-update tolerance,
+// and a counter that moves whenever the groups are rebuilt (descriptors, tile lists, partial-sum slots and kernels change).
+b2_ctx* set_ctx(const b2_factor_set* s);
+const std::vector<b2_factor*>& set_factors(const b2_factor_set* s);
+uint32_t* set_frozen(const b2_factor_set* s);
+bool set_any_tolerance(const b2_factor_set* s);
+uint64_t set_layout_gen(const b2_factor_set* s);
+std::unique_ptr<LmCache, LmCacheDeleter>& set_lm_cache(b2_factor_set* s);
+// b2_factor_set_error's rule for the host evaluation poses `deltas` (F x 16): a member without current correspondences establishes
+// them at its pose first.
+b2_status set_ready_for_error(b2_factor_set* s, const double* deltas, const char* fn);
+// Stored correspondences exist and still index the factor's target (corr_current); the factor has a correspondence-update
+// tolerance rule at all (not VGICP); the record of a linearize (mark_linearized; delta: the linearization pose, may be NULL).
+bool factor_corr_current(const b2_factor* f);
+bool factor_tolerance_kind(const b2_factor* f);
+void factor_mark_linearized(b2_factor* f, const double* delta);
+}  // namespace b2

@@ -1105,6 +1105,96 @@ B2_API b2_status b2_exchange_barrier(b2_exchange* ex);
 /* Number of kernel launches issued by this set since creation (for bench.py's gpu_launches). */
 B2_API uint64_t b2_factor_set_launch_count(const b2_factor_set* set);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Pose optimization on the device: LevenbergMarquardtOptimizerExt::optimize() (src/gtsam_points/optimizers/
+ * levenberg_marquardt_ext.cpp:180-434) on the graph of ONE Pose3 variable T made of the set's members, each a UNARY matching-cost
+ * factor with a fixed target pose T_target[i] (delta_i = T_target[i]^-1 T, integrated_matching_cost_factor.cpp:55-69).  The whole
+ * loop runs on the device as one CUDA graph launch with conditional (WHILE) nodes; the host waits once, for the result.
+ *
+ * Rules (GTSAM's useFixedLambdaFactor = true, diagonalDamping = false):
+ *   start:  error0 = the set's error at the initial deltas (b2_factor_set_error's rule: a member without current correspondences
+ *           associates at its evaluation pose first); lambda = lambda_initial; E_prev = error0.
+ *   outer:  linearize every member at the current deltas; E = the set's error at the same deltas; G = sum H_source, g = -sum b_source
+ *           (set order); then tryLambda until it returns true.  After it: stop when accepted > max_iterations, E is not finite,
+ *           |E_prev - E| < absolute_error_tol, |E_prev - E| / |E_prev| < relative_error_tol or E < error_tol; E_prev = E.
+ *   tryLambda: Cholesky of G + lambda I (not positive definite: not solved); lin_change = d'g - 0.5 d'Gd; if solved and
+ *           lin_change >= 0: T' = T Exp(d) (tangent [w, v]), E' = the set's error at T' with the correspondences of the linearize,
+ *           success iff lin_change > DBL_EPSILON * 0.5 sum f and (E - E') / lin_change > min_model_fidelity, stop iff |E - E'| <
+ *           relative_error_tol * E.  Success: T = T', E = E', lambda = max(lambda / lambda_factor, lambda_lower_bound), accepted++,
+ *           true.  Otherwise if !stop: lambda *= lambda_factor, true iff lambda >= lambda_upper_bound.  Otherwise true.
+ *   A member's correspondence-update tolerance (b2_factor_set_correspondence_update_tolerance) is applied before every linearize,
+ *   on the device, as the host-pose linearize applies it.  On return every member's host-side state (linearization point,
+ *   correspondences, the pose of the last correspondence update) is what the same sequence of b2_factor_set_linearize /
+ *   b2_factor_set_error calls would have left.
+ * Deliberate differences from the reference: unary factors only; one pose variable; only the fixed lambda factor; no diagonal
+ * damping; no callbacks and no termination_criteria; error0 (not DBL_MAX) is the first E_prev.  So that the device loop always
+ * ends, absolute_error_tol must be positive, lambda must stay a normal positive double through max_iterations + 1 decreases, and
+ * the parameters must allow at most 2^22 tryLambda calls (2 (max_iterations + 2) outer iterations times the rejected steps from the
+ * smallest reachable lambda to lambda_upper_bound, DESIGN.md 4.9); the device stops at that bound (B2_LM_TRY_LIMIT).
+ * All arithmetic of the loop is float64 without fused multiply-adds (DESIGN.md 4.9), so it can be restated on the host bit for bit
+ * except for Exp's sin / cos / sqrt.  The tolerance test's rotation angle uses atan2 and sqrt, on the device here and on the host in
+ * the host-pose linearize: for a pose whose angle or distance to the last correspondence update lies within a few ulps of the
+ * tolerance, the two may decide differently, and only then does the state left differ from the host sequence's. */
+typedef struct b2_lm_params {
+  int32_t max_iterations;     /* >= 0 (100) */
+  int32_t reserved;
+  double relative_error_tol;  /* >= 0 (1e-5) */
+  double absolute_error_tol;  /* > 0 (1e-5) */
+  double error_tol;           /* (0) */
+  double lambda_initial;      /* > 0 (1e-5) */
+  double lambda_factor;       /* > 1 (10) */
+  double lambda_upper_bound;  /* > 0 (1e5) */
+  double lambda_lower_bound;  /* >= 0 (0) */
+  double min_model_fidelity;  /* (1e-3) */
+} b2_lm_params;
+B2_API void b2_lm_params_default(b2_lm_params* params);
+
+typedef enum b2_lm_termination {
+  B2_LM_MAX_ITERATIONS = 1,   /* accepted > max_iterations */
+  B2_LM_NON_FINITE = 2,       /* the error is not finite */
+  B2_LM_ABSOLUTE_TOL = 3,
+  B2_LM_RELATIVE_TOL = 4,
+  B2_LM_ERROR_TOL = 5,
+  B2_LM_TRY_LIMIT = 6         /* a guard the rules never reach: the tryLambda calls hit the bound the parameter check derived */
+} b2_lm_termination;
+
+typedef struct b2_lm_summary {
+  int64_t iterations;         /* accepted steps (GTSAM's iterations()) */
+  int64_t outer_iterations;   /* linearizations */
+  int64_t inner_iterations;   /* tryLambda calls */
+  int64_t linearizations;     /* set linearize evaluations */
+  int64_t error_evaluations;  /* set error evaluations run: error0, one per outer and one per inner iteration */
+  double error0, error, lambda;
+  int32_t termination;        /* b2_lm_termination */
+  int32_t reserved;
+} b2_lm_summary;
+
+/* One tryLambda.  A step that was not tried (not solved, or lin_change < 0) has T_trial = T_lin and error_trial = NaN. */
+typedef struct b2_lm_trace_entry {
+  int32_t outer;              /* 0-based outer iteration */
+  int32_t solved, success, stop;
+  double lambda;              /* lambda the step was solved with */
+  double T_lin[16];           /* linearization pose (row-major) */
+  double G[36], g[6];         /* as reduced on the device */
+  double error;               /* E */
+  double half_f;              /* 0.5 sum f of the linearize */
+  double d[6];
+  double lin_change;
+  double T_trial[16];
+  double error_trial;         /* E' */
+  double fidelity;            /* 0 unless lin_change > DBL_EPSILON * half_f */
+} b2_lm_trace_entry;
+
+/* T_targets: host, F x 16 (member i's fixed target pose); T_init, T_out: host, 16.  Blocks until T_out is on the host.  summary
+ * may be NULL.  trace may be NULL; otherwise it receives the first trace_capacity entries and *trace_len (may be NULL) the full
+ * count.  Errors before any device work (B2_ERR_INVALID_ARGUMENT): NULL pointers, non-finite poses or parameters, parameters
+ * out of range (checked before the set is read).  The first call on a set captures and instantiates its graph and allocates its
+ * buffers; later calls reuse them, so a caller that optimizes every frame keeps one set per factor configuration.  The set's offloading rule applies (b2_factor_set_enable_offloading).  A driver without conditional graph nodes
+ * (older than CUDA 12.4) is B2_ERR_INVALID_STATE; there is no host path.  b2_factor_set_launch_count does not count the call. */
+B2_API b2_status b2_factor_set_optimize_pose(b2_factor_set* set, const double* T_targets, const double* T_init, const b2_lm_params* params,
+                                             double* T_out, b2_lm_summary* summary, b2_lm_trace_entry* trace, size_t trace_capacity,
+                                             size_t* trace_len);
+
 #ifdef __cplusplus
 }
 #endif

@@ -19,7 +19,8 @@ from .factors import (  # noqa: F401
     pose_inverse,
 )
 from .occupancy import FastOccupancyGrid, raycast  # noqa: F401
-from .optimize import LevenbergMarquardtExtParams, PoseOptimizationResult, optimize_pose_gpu  # noqa: F401
+from .optimize import (GraphOptimizationResult, LevenbergMarquardtExtParams, PoseOptimizationResult, PriorFactorPose3, optimize_graph_gpu,  # noqa: F401
+                       optimize_pose_gpu)
 from .registration import Features, GNCParams, RANSACParams, RegistrationResult, estimate_fpfh, estimate_pfh, estimate_pose_gnc, estimate_pose_ransac  # noqa: F401
 from .segmentation import MinCutParams, MinCutResult, RegionGrowing, RegionGrowingParams, min_cut, region_growing_init, region_growing_update  # noqa: F401
 from .types import (  # noqa: F401

@@ -105,6 +105,16 @@ class LmTraceEntryC(C.Structure):
                 ("d", C.c_double * 6), ("lin_change", C.c_double), ("T_trial", C.c_double * 16), ("error_trial", C.c_double), ("fidelity", C.c_double)]
 
 
+class PosePriorC(C.Structure):
+    _fields_ = [("var", C.c_int32), ("reserved", C.c_int32), ("T_prior", C.c_double * 16), ("precision", C.c_double * 6)]
+
+
+class LmGraphTraceEntryC(C.Structure):
+    _fields_ = [("outer", C.c_int32), ("solved", C.c_int32), ("success", C.c_int32), ("stop", C.c_int32), ("lambda_", C.c_double),
+                ("error", C.c_double), ("half_f", C.c_double), ("lin_change", C.c_double), ("error_trial", C.c_double), ("fidelity", C.c_double)]
+
+
+B2_LM_MAX_POSES = 32
 B2_LM_TERMINATION = {0: "none", 1: "max_iterations", 2: "non_finite", 3: "absolute_error_tol", 4: "relative_error_tol", 5: "error_tol", 6: "try_limit"}
 
 _lib = None
@@ -271,6 +281,10 @@ SIGNATURES = {
     "b2_factor_set_launch_count": (C.c_uint64, [_vp]),
     "b2_lm_params_default": (None, [C.POINTER(LmParamsC)]),
     "b2_factor_set_optimize_pose": (C.c_int, [_vp, _dp, _dp, C.POINTER(LmParamsC), _dp, C.POINTER(LmSummaryC), C.POINTER(LmTraceEntryC), C.c_size_t, C.POINTER(C.c_size_t)]),
+    "b2_lm_graph_trace_doubles": (C.c_size_t, [C.c_size_t]),
+    "b2_factor_set_optimize_poses": (C.c_int, [_vp, C.c_size_t, _ip, _dp, C.POINTER(PosePriorC), C.c_size_t, _dp, C.POINTER(LmParamsC), _dp, C.POINTER(LmSummaryC),
+                                               C.POINTER(LmGraphTraceEntryC), _dp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "b2_factor_set_lm_graph_builds": (C.c_uint64, [_vp]),
 }
 
 

@@ -1203,6 +1203,7 @@ public:
 };
 
 class NonlinearFactorSetGPU;
+struct PosePriorB200;
 
 // factors/integrated_gicp_factor.hpp:20-24.  The device path recomputes M = (C_B + R C_A R^T)^-1 from the rotation of the
 // linearization point inside the kernel (the reference's NONE behaviour: no cache to keep in HBM).  FULL gives the same
@@ -1736,6 +1737,9 @@ public:
 
   // optimize_pose_gpu over this set's members (unary factors on one source key), reusing the set and its cached graph from call to call
   Mat4 optimize_pose(const Mat4& T_init, const b2_lm_params* params = nullptr, b2_lm_summary* summary = nullptr);
+  // optimize_poses_gpu over this set's members, reusing the set and its cached graph from call to call (and across graph shapes)
+  std::map<Key, Mat4> optimize_poses(const std::vector<PosePriorB200>& priors, const std::map<Key, Mat4>& values, const b2_lm_params* params = nullptr,
+                                     b2_lm_summary* summary = nullptr);
 
   std::vector<LinearFactorPtr> calc_linear_factors(const Values& linearization_point) override {
     linearize(linearization_point);
@@ -1788,6 +1792,86 @@ Mat4 optimize_pose_on(b2_factor_set* set, const Factors& factors, const Mat4& T_
   return out;
 }
 }  // namespace detail
+
+// gtsam::PriorFactor<Pose3>(key, pose, noise) with a diagonal precision over the tangent [w, v] (GTSAM's Isotropic::Precision(6, p)
+// is p six times)
+struct PosePriorB200 {
+  Key key;
+  Mat4 pose;
+  std::array<double, 6> precision;
+};
+
+namespace detail {
+// b2_factor_set_optimize_poses on `set`, whose members are `factors` in order; the variables are the keys of `values` in order
+template <class Factors>
+std::map<Key, Mat4> optimize_poses_on(b2_factor_set* set, const Factors& factors, const std::vector<PosePriorB200>& priors, const std::map<Key, Mat4>& values,
+                                      const b2_lm_params* params, b2_lm_summary* summary) {
+  const char* fn = "optimize_poses_gpu";
+  if (factors.empty()) throw std::invalid_argument(std::string(fn) + ": no factors");
+  if (values.empty() || values.size() > B2_LM_MAX_POSES) throw std::invalid_argument(std::string(fn) + ": 1 to B2_LM_MAX_POSES values are optimized");
+  std::map<Key, int32_t> index;
+  std::vector<double> T_init;
+  for (const auto& kv : values) {
+    index.emplace(kv.first, static_cast<int32_t>(index.size()));
+    T_init.insert(T_init.end(), kv.second.begin(), kv.second.end());
+  }
+  auto var = [&](Key k) {
+    const auto it = index.find(k);
+    if (it == index.end()) throw std::invalid_argument(std::string(fn) + ": a factor or prior acts on a key that has no value");
+    return it->second;
+  };
+  std::vector<int32_t> member_vars;
+  std::vector<double> targets;
+  for (const auto& f : factors) {
+    member_vars.push_back(f->is_binary() ? var(f->keys()[0]) : -1);
+    member_vars.push_back(var(f->keys()[f->is_binary() ? 1 : 0]));
+    targets.insert(targets.end(), f->fixed_target_pose().begin(), f->fixed_target_pose().end());
+  }
+  std::vector<b2_pose_prior> pri(priors.size());
+  for (std::size_t j = 0; j < priors.size(); j++) {
+    pri[j] = b2_pose_prior{};
+    pri[j].var = var(priors[j].key);
+    std::copy(priors[j].pose.begin(), priors[j].pose.end(), pri[j].T_prior);
+    std::copy(priors[j].precision.begin(), priors[j].precision.end(), pri[j].precision);
+  }
+  b2_lm_params p;
+  if (params) p = *params;
+  else b2_lm_params_default(&p);
+  std::vector<double> out(T_init.size());
+  const b2_status st = b2_factor_set_optimize_poses(set, values.size(), member_vars.data(), targets.data(), pri.data(), pri.size(), T_init.data(), &p, out.data(), summary,
+                                                    nullptr, nullptr, 0, nullptr);
+  if (st == B2_ERR_INVALID_ARGUMENT) throw std::invalid_argument(b2_last_error());
+  check(st, "b2_factor_set_optimize_poses");
+  std::map<Key, Mat4> result;
+  for (const auto& kv : index) std::copy(out.begin() + kv.second * 16, out.begin() + kv.second * 16 + 16, result[kv.first].begin());
+  return result;
+}
+}  // namespace detail
+
+inline std::map<Key, Mat4> NonlinearFactorSetGPU::optimize_poses(const std::vector<PosePriorB200>& priors, const std::map<Key, Mat4>& values, const b2_lm_params* params,
+                                                                 b2_lm_summary* summary) {
+  if (factors_.empty()) throw std::invalid_argument("optimize_poses_gpu: no factors");
+  ensure();
+  return detail::optimize_poses_on(set_, factors_, priors, values, params, summary);
+}
+
+// LevenbergMarquardtOptimizerExt::optimize() over a graph of up to B2_LM_MAX_POSES Pose3 variables made of unary and binary
+// matching-cost factors and Pose3 priors, run on the device as one graph launch (b2_factor_set_optimize_poses; its header comment
+// states the rules and the differences from GTSAM).  The variables are the keys of `values`; binary factors act on their keys,
+// unary factors on their source key against their fixed target pose.  params: NULL takes GTSAM's defaults.  Returns the optimized
+// values; summary may be NULL.  Argument errors throw std::invalid_argument.  This form creates a factor set for the one call; a
+// caller that optimizes repeatedly keeps a NonlinearFactorSetGPU and calls its optimize_poses.
+inline std::map<Key, Mat4> optimize_poses_gpu(const std::vector<std::shared_ptr<IntegratedMatchingCostFactorB200>>& factors, const std::vector<PosePriorB200>& priors,
+                                              const std::map<Key, Mat4>& values, const b2_lm_params* params = nullptr, b2_lm_summary* summary = nullptr,
+                                              Context::Ptr ctx = Context::default_context()) {
+  if (factors.empty()) throw std::invalid_argument("optimize_poses_gpu: no factors");
+  std::vector<b2_factor*> hs;
+  for (const auto& f : factors) hs.push_back(f->handle());
+  b2_factor_set* set = nullptr;
+  check(b2_factor_set_create(ctx->get(), hs.data(), hs.size(), &set), "b2_factor_set_create");
+  const std::unique_ptr<b2_factor_set, b2_status (*)(b2_factor_set*)> owned(set, b2_factor_set_destroy);
+  return detail::optimize_poses_on(set, factors, priors, values, params, summary);
+}
 
 inline Mat4 NonlinearFactorSetGPU::optimize_pose(const Mat4& T_init, const b2_lm_params* params, b2_lm_summary* summary) {
   if (factors_.empty()) throw std::invalid_argument("optimize_pose_gpu: no factors");

@@ -1195,6 +1195,80 @@ B2_API b2_status b2_factor_set_optimize_pose(b2_factor_set* set, const double* T
                                              double* T_out, b2_lm_summary* summary, b2_lm_trace_entry* trace, size_t trace_capacity,
                                              size_t* trace_len);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Multi-pose optimization on the device: the same loop on a graph of N Pose3 variables T_0..T_{N-1} (1 <= N <= B2_LM_MAX_POSES)
+ * made of the set's members, unary or binary, and PriorFactor<Pose3>s -- the graphs of the reference's scan-matching examples
+ * (a prior on pose 0 and a binary factor), of demo_matching_cost_factors.cpp (a window of frames) and of its AlignmentTest.
+ * b2_factor_set_optimize_pose is this call's N = 1 case with unary members and no prior, and computes the same bits.
+ *
+ * Rules (those of b2_factor_set_optimize_pose, with):
+ *   variables: member i has (target_var, source_var) = member_vars[2i], member_vars[2i + 1]; target_var = -1 makes it unary with
+ *           the fixed target pose T_targets[i]; its delta is T[target]^-1 T[source] (T_targets[i]^-1 T[source] when unary), with the
+ *           optimizer's pose products.  source_var in [0, N); target_var in [-1, N) and != source_var.
+ *   priors: PriorFactor<Pose3>(var, T_prior, diagonal precision p[6]) (GTSAM's Isotropic::Precision(6, 1e6) is p = 1e6 six times):
+ *           r = Logmap(T_prior^-1 T_var), tangent [w, v] as Exp's, right for rotation angles in [0, pi] (through atan2 of the
+ *           rotation's sine and cosine; above pi / 2 the axis comes from the symmetric part; below 1e-10 rad v = t - 0.5 w x t);
+ *           J = Pose3::LogmapDerivative(r), the inverse right Jacobian of SE(3) -- the exact derivative of r under T Exp(d) (series
+ *           coefficients below 1e-3 rad for Jw and below 0.1 rad for Q, closed forms above);  H = J' diag(p) J, b = J' diag(p) r,
+ *           f = sum_k p_k r_k^2, error = 0.5 f (GTSAM's error; 0.5 f is also its linearized error at zero, as a member's 0.5 f is).
+ *           The operation order is stated at prior_eval in b2_optimize.cu.
+ *   assembly: the dense 6N x 6N system G, g.  Each block of G and segment of g is the sum of its contributions in set order, then
+ *           in prior order, from 0.0: a member adds H_source to (s, s), H_target to (t, t), H_target_source to (t, s) and its
+ *           transpose to (s, t), b_target and b_source to segments t and s; a prior adds H to (var, var) and b to segment var;
+ *           g = -(sum).  E = the members' errors in set order, then the priors' errors; half_f = 0.5 (sum of f) in the same order.
+ *           error0 and E' are sums of the same form.
+ *   solve:  Cholesky of G + lambda I on G's lower triangle (not positive definite: not solved), forward and back substitution;
+ *           every inner sum runs over ascending index (a right-looking factorization keeps that order); lin_change = d'g - 0.5 d'Gd
+ *           over the full G; T'_v = T_v Exp(d_v) for every variable v.
+ *   The loop, termination, the parameter check, the tryLambda bound and the correspondence-update tolerance (applied per member, on
+ *   its delta) are b2_factor_set_optimize_pose's; so is the host state each member is left in.
+ *   A graph without a prior (or one that leaves a gauge free) has a G that is only positive semidefinite: lambda I makes the damped
+ *   system solvable, g has no component along the free directions, so the steps leave the gauge in place up to rounding, and the
+ *   loop ends under the same rules with finite poses; only the relative poses are determined.
+ * Deliberate differences from GTSAM, besides those of b2_factor_set_optimize_pose: a dense Cholesky in variable-index order instead
+ * of GTSAM's sparse elimination under COLAMD, so rounding differs; diagonal prior precisions only; no other factor types (no
+ * BetweenFactor, IMU or other families). */
+#define B2_LM_MAX_POSES 32  /* a 192 x 192 system: its packed lower triangle fits one CTA's shared memory */
+
+typedef struct b2_pose_prior {
+  int32_t var;
+  int32_t reserved;
+  double T_prior[16];  /* row-major */
+  double precision[6]; /* diagonal, over [w, v]; finite and > 0 */
+} b2_pose_prior;
+
+/* One tryLambda of the graph; its arrays follow in trace_data */
+typedef struct b2_lm_graph_trace_entry {
+  int32_t outer;              /* 0-based outer iteration */
+  int32_t solved, success, stop;
+  double lambda;              /* lambda the step was solved with */
+  double error;               /* E */
+  double half_f;              /* 0.5 sum f of the linearize (priors included) */
+  double lin_change;
+  double error_trial;         /* E' (NaN when the step was not tried) */
+  double fidelity;            /* 0 unless lin_change > DBL_EPSILON * half_f */
+} b2_lm_graph_trace_entry;
+/* Doubles per trace entry in trace_data, in this order: T_lin (N x 16), G ((6N)^2, full, row-major), g (6N), d (6N),
+ * T_trial (N x 16).  A step that was not tried has T_trial = T_lin. */
+B2_API size_t b2_lm_graph_trace_doubles(size_t num_poses);
+
+/* member_vars: host, F x 2 int32 (F = the set's size).  T_targets: host, F x 16, read only for unary members (may be NULL when
+ * every member is binary).  priors: host, num_priors (may be NULL when num_priors = 0).  T_init, T_out: host, N x 16.  summary may
+ * be NULL.  trace may be NULL; otherwise trace (trace_capacity entries) and trace_data (trace_capacity x
+ * b2_lm_graph_trace_doubles(N) doubles) receive the first trace_capacity entries and *trace_len (may be NULL) the full count.
+ * Errors before any device work (B2_ERR_INVALID_ARGUMENT): NULL pointers, N out of range, a var index out of range, target_var ==
+ * source_var, a variable that no member or prior references, non-finite poses, precisions or parameters, a precision that is not
+ * positive, parameters out of range (checked before the set is read, as are the priors and T_init).  The set's graph depends only
+ * on its layout and on its buffers' capacities (poses, priors): a call with another topology, other target poses or other priors
+ * reuses it unless it needs more poses or priors than an earlier call on the set.  A driver without conditional graph nodes is
+ * B2_ERR_INVALID_STATE.  b2_factor_set_launch_count does not count the call. */
+B2_API b2_status b2_factor_set_optimize_poses(b2_factor_set* set, size_t num_poses, const int32_t* member_vars, const double* T_targets,
+                                              const b2_pose_prior* priors, size_t num_priors, const double* T_init, const b2_lm_params* params,
+                                              double* T_out, b2_lm_summary* summary, b2_lm_graph_trace_entry* trace, double* trace_data,
+                                              size_t trace_capacity, size_t* trace_len);
+/* How many times the set's optimizer graph has been captured and instantiated (0 before the first optimize call). */
+B2_API uint64_t b2_factor_set_lm_graph_builds(b2_factor_set* set);
+
 #ifdef __cplusplus
 }
 #endif

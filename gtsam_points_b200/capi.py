@@ -99,12 +99,6 @@ class LmSummaryC(C.Structure):
                 ("reserved", C.c_int32)]
 
 
-class LmTraceEntryC(C.Structure):
-    _fields_ = [("outer", C.c_int32), ("solved", C.c_int32), ("success", C.c_int32), ("stop", C.c_int32), ("lambda_", C.c_double),
-                ("T_lin", C.c_double * 16), ("G", C.c_double * 36), ("g", C.c_double * 6), ("error", C.c_double), ("half_f", C.c_double),
-                ("d", C.c_double * 6), ("lin_change", C.c_double), ("T_trial", C.c_double * 16), ("error_trial", C.c_double), ("fidelity", C.c_double)]
-
-
 class PosePriorC(C.Structure):
     _fields_ = [("var", C.c_int32), ("reserved", C.c_int32), ("T_prior", C.c_double * 16), ("precision", C.c_double * 6)]
 
@@ -280,7 +274,6 @@ SIGNATURES = {
     "b2_exchange_barrier": (C.c_int, [_vp]),
     "b2_factor_set_launch_count": (C.c_uint64, [_vp]),
     "b2_lm_params_default": (None, [C.POINTER(LmParamsC)]),
-    "b2_factor_set_optimize_pose": (C.c_int, [_vp, _dp, _dp, C.POINTER(LmParamsC), _dp, C.POINTER(LmSummaryC), C.POINTER(LmTraceEntryC), C.c_size_t, C.POINTER(C.c_size_t)]),
     "b2_lm_graph_trace_doubles": (C.c_size_t, [C.c_size_t]),
     "b2_factor_set_optimize_poses": (C.c_int, [_vp, C.c_size_t, _ip, _dp, C.POINTER(PosePriorC), C.c_size_t, _dp, C.POINTER(LmParamsC), _dp, C.POINTER(LmSummaryC),
                                                C.POINTER(LmGraphTraceEntryC), _dp, C.c_size_t, C.POINTER(C.c_size_t)]),

@@ -1773,26 +1773,6 @@ private:
 // what user code hands to LinearizationHook::register_hook (src/demo/demo_matching_cost_factors.cpp:52)
 inline std::shared_ptr<FactorSetBase> create_nonlinear_factor_set_gpu() { return std::make_shared<NonlinearFactorSetGPU>(); }
 
-namespace detail {
-// b2_factor_set_optimize_pose on `set`, whose members are `factors` in order (unary, one source key)
-template <class Factors>
-Mat4 optimize_pose_on(b2_factor_set* set, const Factors& factors, const Mat4& T_init, const b2_lm_params* params, b2_lm_summary* summary) {
-  if (factors.empty()) throw std::invalid_argument("optimize_pose_gpu: no factors");
-  std::vector<double> targets;
-  for (const auto& f : factors) {
-    if (f->is_binary()) throw std::invalid_argument("optimize_pose_gpu: binary factors are not supported");
-    if (f->keys()[0] != factors[0]->keys()[0]) throw std::invalid_argument("optimize_pose_gpu: the factors act on different source keys");
-    targets.insert(targets.end(), f->fixed_target_pose().begin(), f->fixed_target_pose().end());
-  }
-  b2_lm_params p;
-  if (params) p = *params;
-  else b2_lm_params_default(&p);
-  Mat4 out{};
-  check(b2_factor_set_optimize_pose(set, targets.data(), T_init.data(), &p, out.data(), summary, nullptr, 0, nullptr), "b2_factor_set_optimize_pose");
-  return out;
-}
-}  // namespace detail
-
 // gtsam::PriorFactor<Pose3>(key, pose, noise) with a diagonal precision over the tangent [w, v] (GTSAM's Isotropic::Precision(6, p)
 // is p six times)
 struct PosePriorB200 {
@@ -1846,6 +1826,18 @@ std::map<Key, Mat4> optimize_poses_on(b2_factor_set* set, const Factors& factors
   for (const auto& kv : index) std::copy(out.begin() + kv.second * 16, out.begin() + kv.second * 16 + 16, result[kv.first].begin());
   return result;
 }
+
+// the N = 1 graph of optimize_poses_on: `factors` are unary on one source key, optimized from T_init without priors
+template <class Factors>
+Mat4 optimize_pose_on(b2_factor_set* set, const Factors& factors, const Mat4& T_init, const b2_lm_params* params, b2_lm_summary* summary) {
+  if (factors.empty()) throw std::invalid_argument("optimize_pose_gpu: no factors");
+  const Key key = factors[0]->keys()[0];
+  for (const auto& f : factors) {
+    if (f->is_binary()) throw std::invalid_argument("optimize_pose_gpu: binary factors are not supported");
+    if (f->keys()[0] != key) throw std::invalid_argument("optimize_pose_gpu: the factors act on different source keys");
+  }
+  return optimize_poses_on(set, factors, {}, {{key, T_init}}, params, summary).begin()->second;
+}
 }  // namespace detail
 
 inline std::map<Key, Mat4> NonlinearFactorSetGPU::optimize_poses(const std::vector<PosePriorB200>& priors, const std::map<Key, Mat4>& values, const b2_lm_params* params,
@@ -1879,11 +1871,13 @@ inline Mat4 NonlinearFactorSetGPU::optimize_pose(const Mat4& T_init, const b2_lm
   return detail::optimize_pose_on(set_, factors_, T_init, params, summary);
 }
 
-// LevenbergMarquardtOptimizerExt::optimize() over the pose of unary factors, run on the device as one graph launch
-// (b2_factor_set_optimize_pose; its header comment states the rules and the differences from GTSAM).  Every factor must be unary
-// (constructed with a fixed target pose) and act on the same source key.  params: NULL takes GTSAM's defaults.  Returns the optimized
-// source pose (row-major); summary may be NULL.  This form creates a factor set for the one call, so the call also captures and
-// instantiates the set's graph; a caller that optimizes every frame keeps a NonlinearFactorSetGPU and calls its optimize_pose.
+// LevenbergMarquardtOptimizerExt::optimize() over the pose of unary factors, run on the device as one graph launch: the one-pose
+// graph of optimize_poses_gpu (b2_factor_set_optimize_poses; its header comment states the rules and the differences from GTSAM).
+// Every factor must be unary (constructed with a fixed target pose) and act on the same source key.  params: NULL takes GTSAM's
+// defaults.  Returns the optimized source pose (row-major); summary may be NULL.  Argument errors throw std::invalid_argument,
+// those the C ABI detects included (a non-finite T_init or target pose, parameters out of range).  This form creates a factor set
+// for the one call, so the call also captures and instantiates the set's graph; a caller that optimizes every frame keeps a
+// NonlinearFactorSetGPU and calls its optimize_pose.
 inline Mat4 optimize_pose_gpu(const std::vector<std::shared_ptr<IntegratedMatchingCostFactorB200>>& factors, const Mat4& T_init, const b2_lm_params* params = nullptr,
                               b2_lm_summary* summary = nullptr, Context::Ptr ctx = Context::default_context()) {
   if (factors.empty()) throw std::invalid_argument("optimize_pose_gpu: no factors");

@@ -10,9 +10,9 @@
 // single-CTA float64 code.  The topology, the target poses, the priors and N are per-call device inputs, so a call with another
 // graph shape reuses the captured graph unless it needs more room than the buffers have.  This translation unit is compiled with
 // FMA contraction off (device: -fmad=false, host: -ffp-contract=off), so the pose products, the assembly, damping, Cholesky,
-// substitutions and lin_change below are plain IEEE operations in the order written, which the host restatements
-// (tests/lm_ext_np.py, tests/lm_graph_np.py) reproduce bit for bit.  Only sin / cos / tan / atan2 / sqrt of Exp, of the priors'
-// Logmap and of its derivative may differ from a host's in the last bits.
+// substitutions and lin_change below are plain IEEE operations in the order written, which the host restatement tests/lm_graph_np.py
+// reproduces bit for bit.  Only sin / cos / tan / atan2 / sqrt of Exp, of the priors' Logmap and of its derivative may differ from a
+// host's in the last bits.
 #include <cfloat>
 #include <vector>
 
@@ -933,42 +933,6 @@ void b2_lm_params_default(b2_lm_params* p) {
 }
 
 size_t b2_lm_graph_trace_doubles(size_t num_poses) { return 36 * num_poses * num_poses + 44 * num_poses; }
-
-b2_status b2_factor_set_optimize_pose(b2_factor_set* s, const double* T_targets, const double* T_init, const b2_lm_params* params, double* T_out,
-                                      b2_lm_summary* summary, b2_lm_trace_entry* trace, size_t trace_capacity, size_t* trace_len) {
-  const char* fn = "b2_factor_set_optimize_pose";
-  B2_REQUIRE(s && T_targets && T_init && params && T_out, "%s: NULL argument", fn);
-  uint64_t max_tries = 0;
-  B2_TRY(check_params(params, &max_tries, fn));
-  B2_TRY(check_pose(T_init, fn));
-  const size_t F = set_factors(s).size();
-  B2_REQUIRE(F > 0, "%s: the set has no members", fn);
-  for (size_t i = 0; i < F; i++) B2_TRY(check_pose(T_targets + i * 16, fn));
-  // the N = 1 graph of unary members without priors; its trace entries are the graph entries with their arrays inlined
-  std::vector<int32_t> topo(2 * F);
-  for (size_t i = 0; i < F; i++) topo[2 * i] = -1, topo[2 * i + 1] = 0;
-  const size_t cap = trace ? trace_capacity : 0;
-  std::vector<b2_lm_graph_trace_entry> entries(cap);
-  std::vector<double> data(cap * b2_lm_graph_trace_doubles(1));
-  size_t n = 0;
-  B2_TRY(run_optimizer(s, 1, topo.data(), T_targets, nullptr, 0, T_init, params, max_tries, T_out, summary, entries.data(), data.data(), cap, &n, fn));
-  for (size_t k = 0; k < std::min(cap, n); k++) {
-    const b2_lm_graph_trace_entry& e = entries[k];
-    const double* x = data.data() + k * b2_lm_graph_trace_doubles(1);
-    b2_lm_trace_entry& t = trace[k];
-    t = b2_lm_trace_entry{};
-    t.outer = e.outer, t.solved = e.solved, t.success = e.success, t.stop = e.stop;
-    t.lambda = e.lambda;
-    std::copy(x, x + 16, t.T_lin);
-    std::copy(x + 16, x + 52, t.G);
-    std::copy(x + 52, x + 58, t.g);
-    std::copy(x + 58, x + 64, t.d);
-    std::copy(x + 64, x + 80, t.T_trial);
-    t.error = e.error, t.half_f = e.half_f, t.lin_change = e.lin_change, t.error_trial = e.error_trial, t.fidelity = e.fidelity;
-  }
-  if (trace_len) *trace_len = n;
-  return B2_OK;
-}
 
 b2_status b2_factor_set_optimize_poses(b2_factor_set* s, size_t num_poses, const int32_t* member_vars, const double* T_targets, const b2_pose_prior* priors,
                                        size_t num_priors, const double* T_init, const b2_lm_params* params, double* T_out, b2_lm_summary* summary,

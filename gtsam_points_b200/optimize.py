@@ -1,6 +1,6 @@
 """Pose optimization on the device: LevenbergMarquardtOptimizerExt (src/gtsam_points/optimizers/levenberg_marquardt_ext.cpp) run
-as one CUDA graph launch, on one Pose3 variable made of unary matching-cost factors (b2_factor_set_optimize_pose), or on a graph
-of up to 32 Pose3 variables made of unary and binary matching-cost factors and Pose3 priors (b2_factor_set_optimize_poses).
+as one CUDA graph launch (b2_factor_set_optimize_poses), on one Pose3 variable made of unary matching-cost factors, or on a graph
+of up to 32 Pose3 variables made of unary and binary matching-cost factors and Pose3 priors.
 
   params = LevenbergMarquardtExtParams(maxIterations=30)
   result = optimize_pose_gpu([IntegratedVGICPFactor(T_target, 1, target_voxels, source)], T_init, params)
@@ -9,8 +9,7 @@ of up to 32 Pose3 variables made of unary and binary matching-cost factors and P
   result = optimize_graph_gpu([IntegratedVGICPFactor(0, 1, voxels0, cloud1)], {0: T0, 1: T1}, [PriorFactorPose3(0, T0, 1e6)])
   result.values  # {0: pose, 1: pose}
 
-The rules, and where they differ from GTSAM's, are documented at b2_factor_set_optimize_pose and b2_factor_set_optimize_poses in
-include/b2points.h.
+The rules, and where they differ from GTSAM's, are documented at b2_factor_set_optimize_poses in include/b2points.h.
 """
 from __future__ import annotations
 
@@ -69,14 +68,6 @@ class PoseOptimizationResult:
     trace_len: int = 0       # tryLambda calls, traced or not
 
 
-def _trace_dict(e: capi.LmTraceEntryC) -> dict:
-    return dict(
-        outer=e.outer, solved=bool(e.solved), success=bool(e.success), stop=bool(e.stop), lam=e.lambda_,
-        T_lin=np.array(e.T_lin[:]).reshape(4, 4), G=np.array(e.G[:]).reshape(6, 6), g=np.array(e.g[:]), error=e.error, half_f=e.half_f,
-        d=np.array(e.d[:]), lin_change=e.lin_change, T_trial=np.array(e.T_trial[:]).reshape(4, 4), error_trial=e.error_trial, fidelity=e.fidelity,
-    )
-
-
 def _members(factors):
     """The factor list of `factors` (a NonlinearFactorSetGPU or a sequence of factors), checked to be unary on one source key."""
     fs = factors.factors if isinstance(factors, NonlinearFactorSetGPU) else list(factors)
@@ -99,33 +90,17 @@ def optimize_pose_gpu(factors, T_init, params: LevenbergMarquardtExtParams | Non
     them (reused, with its cached graph: what a per-frame caller wants).  trace: False, True
     (up to DEFAULT_TRACE_CAPACITY tryLambda entries) or a capacity."""
     fs = _members(factors)
-    T_init = np.ascontiguousarray(np.asarray(T_init, dtype=np.float64))
+    T_init = np.asarray(T_init, dtype=np.float64)
     if T_init.shape != (4, 4) or not np.all(np.isfinite(T_init)):
         raise ValueError("optimize_pose_gpu: T_init must be a finite 4x4 pose")
-    if isinstance(factors, NonlinearFactorSetGPU):
-        fset = factors
-    else:
-        fset = NonlinearFactorSetGPU(fs[0].ctx)
-        fset.add(fs)
-    fset._ensure()
-    targets = np.ascontiguousarray(np.stack([f.fixed_target_pose for f in fs]).astype(np.float64))
-    p = (params or LevenbergMarquardtExtParams()).to_c()
+    # the N = 1 graph of unary members without priors
+    _, _, member_vars, targets, pri, T_init = _graph_inputs(factors, {fs[0].keys()[0]: T_init}, [])
     cap = 0 if trace is False else (DEFAULT_TRACE_CAPACITY if trace is True else int(trace))
-    entries = (capi.LmTraceEntryC * max(cap, 1))() if cap > 0 else None
-    T_out = np.zeros((4, 4))
-    summary = capi.LmSummaryC()
-    n = C.c_size_t(0)
-    capi.check(capi.lib().b2_factor_set_optimize_pose(
-        fset.h, capi.dptr(targets), capi.dptr(T_init), C.byref(p), capi.dptr(T_out), C.byref(summary),
-        C.cast(entries, C.POINTER(capi.LmTraceEntryC)) if entries is not None else None, cap, C.byref(n)))
-    fset.num_linearizations += summary.linearizations * len(fs)
-    fset.num_evaluations += summary.error_evaluations * len(fs)
-    tr = [_trace_dict(entries[i]) for i in range(min(cap, n.value))] if entries is not None else None
-    return PoseOptimizationResult(
-        pose=T_out, iterations=summary.iterations, outer_iterations=summary.outer_iterations, inner_iterations=summary.inner_iterations,
-        linearizations=summary.linearizations, error_evaluations=summary.error_evaluations, error0=summary.error0, error=summary.error,
-        lambda_=summary.lambda_, termination=capi.B2_LM_TERMINATION.get(summary.termination, str(summary.termination)), trace=tr, trace_len=n.value,
-    )
+    T_out, result = _optimize(factors, fs, member_vars, targets, pri, 0, T_init, params, cap)
+    if result["trace"] is not None:
+        for e in result["trace"]:
+            e["T_lin"], e["T_trial"] = e["T_lin"][0], e["T_trial"][0]
+    return PoseOptimizationResult(pose=T_out[0], **result)
 
 
 DEFAULT_GRAPH_TRACE_CAPACITY = 256
@@ -235,15 +210,22 @@ def optimize_graph_gpu(factors, values: dict, priors=(), params: LevenbergMarqua
     (reused, with its cached graph, across calls and graph shapes).  trace: False, True (up to DEFAULT_GRAPH_TRACE_CAPACITY
     tryLambda entries) or a capacity."""
     fs, keys, member_vars, targets, pri, T_init = _graph_inputs(factors, values, list(priors))
-    N = len(keys)
+    cap = 0 if trace is False else (DEFAULT_GRAPH_TRACE_CAPACITY if trace is True else int(trace))
+    T_out, result = _optimize(factors, fs, member_vars, targets, pri, len(priors), T_init, params, cap)
+    return GraphOptimizationResult(values={k: T_out[i].copy() for i, k in enumerate(keys)}, keys=keys, **result)
+
+
+def _optimize(factors, fs, member_vars, targets, pri, num_priors, T_init, params, cap):
+    """b2_factor_set_optimize_poses on checked inputs (those of _graph_inputs) -> (T_out N x 4 x 4, the result's summary and trace
+    fields).  `factors` is reused when it is a NonlinearFactorSetGPU; otherwise a set of `fs` is built for the call."""
     if isinstance(factors, NonlinearFactorSetGPU):
         fset = factors
     else:
         fset = NonlinearFactorSetGPU(fs[0].ctx)
         fset.add(fs)
     fset._ensure()
+    N = len(T_init)
     p = (params or LevenbergMarquardtExtParams()).to_c()
-    cap = 0 if trace is False else (DEFAULT_GRAPH_TRACE_CAPACITY if trace is True else int(trace))
     per = capi.lib().b2_lm_graph_trace_doubles(N)
     entries = (capi.LmGraphTraceEntryC * max(cap, 1))() if cap > 0 else None
     data = np.zeros(max(cap, 1) * per) if cap > 0 else None
@@ -254,15 +236,14 @@ def optimize_graph_gpu(factors, values: dict, priors=(), params: LevenbergMarqua
     summary = capi.LmSummaryC()
     n = C.c_size_t(0)
     capi.check(capi.lib().b2_factor_set_optimize_poses(
-        fset.h, N, member_vars.ctypes.data_as(C.POINTER(C.c_int32)), capi.dptr(targets), C.cast(pri, C.POINTER(capi.PosePriorC)), len(priors),
+        fset.h, N, member_vars.ctypes.data_as(C.POINTER(C.c_int32)), capi.dptr(targets), C.cast(pri, C.POINTER(capi.PosePriorC)), num_priors,
         capi.dptr(T_init), C.byref(p), capi.dptr(T_out), C.byref(summary),
         C.cast(entries, C.POINTER(capi.LmGraphTraceEntryC)) if entries is not None else None, capi.dptr(data) if data is not None else None, cap, C.byref(n)))
     fset.num_linearizations += summary.linearizations * len(fs)
     fset.num_evaluations += summary.error_evaluations * len(fs)
     tr = [_graph_trace_dict(entries[i], data[i * per:(i + 1) * per], N) for i in range(min(cap, n.value))] if entries is not None else None
-    return GraphOptimizationResult(
-        values={k: T_out[i].copy() for i, k in enumerate(keys)}, keys=keys, iterations=summary.iterations, outer_iterations=summary.outer_iterations,
-        inner_iterations=summary.inner_iterations, linearizations=summary.linearizations, error_evaluations=summary.error_evaluations,
-        error0=summary.error0, error=summary.error, lambda_=summary.lambda_,
-        termination=capi.B2_LM_TERMINATION.get(summary.termination, str(summary.termination)), trace=tr, trace_len=n.value,
+    return T_out, dict(
+        iterations=summary.iterations, outer_iterations=summary.outer_iterations, inner_iterations=summary.inner_iterations,
+        linearizations=summary.linearizations, error_evaluations=summary.error_evaluations, error0=summary.error0, error=summary.error,
+        lambda_=summary.lambda_, termination=capi.B2_LM_TERMINATION.get(summary.termination, str(summary.termination)), trace=tr, trace_len=n.value,
     )

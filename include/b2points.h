@@ -1107,34 +1107,61 @@ B2_API uint64_t b2_factor_set_launch_count(const b2_factor_set* set);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Pose optimization on the device: LevenbergMarquardtOptimizerExt::optimize() (src/gtsam_points/optimizers/
- * levenberg_marquardt_ext.cpp:180-434) on the graph of ONE Pose3 variable T made of the set's members, each a UNARY matching-cost
- * factor with a fixed target pose T_target[i] (delta_i = T_target[i]^-1 T, integrated_matching_cost_factor.cpp:55-69).  The whole
- * loop runs on the device as one CUDA graph launch with conditional (WHILE) nodes; the host waits once, for the result.
+ * levenberg_marquardt_ext.cpp:180-434) on a graph of N Pose3 variables T_0..T_{N-1} (1 <= N <= B2_LM_MAX_POSES) made of the set's
+ * members, unary or binary matching-cost factors, and PriorFactor<Pose3>s -- the graphs of the reference's scan-matching examples
+ * (one pose over unary factors, or a prior on pose 0 and a binary factor), of demo_matching_cost_factors.cpp (a window of frames)
+ * and of its AlignmentTest.  N = 1 with unary members and no prior is the one-pose optimization.  The whole loop runs on the
+ * device as one CUDA graph launch with conditional (WHILE) nodes; the host waits once, for the result.
  *
  * Rules (GTSAM's useFixedLambdaFactor = true, diagonalDamping = false):
- *   start:  error0 = the set's error at the initial deltas (b2_factor_set_error's rule: a member without current correspondences
+ *   variables: member i has (target_var, source_var) = member_vars[2i], member_vars[2i + 1]; target_var = -1 makes it unary with
+ *           the fixed target pose T_targets[i] (integrated_matching_cost_factor.cpp:55-69); its delta is T[target]^-1 T[source]
+ *           (T_targets[i]^-1 T[source] when unary), with the optimizer's pose products.  source_var in [0, N); target_var in
+ *           [-1, N) and != source_var.
+ *   priors: PriorFactor<Pose3>(var, T_prior, diagonal precision p[6]) (GTSAM's Isotropic::Precision(6, 1e6) is p = 1e6 six times):
+ *           r = Logmap(T_prior^-1 T_var), tangent [w, v] as Exp's, right for rotation angles in [0, pi] (through atan2 of the
+ *           rotation's sine and cosine; above pi / 2 the axis comes from the symmetric part; below 1e-10 rad v = t - 0.5 w x t);
+ *           J = Pose3::LogmapDerivative(r), the inverse right Jacobian of SE(3) -- the exact derivative of r under T Exp(d) (series
+ *           coefficients below 1e-3 rad for Jw and below 0.1 rad for Q, closed forms above);  H = J' diag(p) J, b = J' diag(p) r,
+ *           f = sum_k p_k r_k^2, error = 0.5 f (GTSAM's error; 0.5 f is also its linearized error at zero, as a member's 0.5 f is).
+ *           The operation order is stated at prior_eval in b2_optimize.cu.
+ *   start:  error0 = the graph's error at the initial poses (b2_factor_set_error's rule: a member without current correspondences
  *           associates at its evaluation pose first); lambda = lambda_initial; E_prev = error0.
- *   outer:  linearize every member at the current deltas; E = the set's error at the same deltas; G = sum H_source, g = -sum b_source
- *           (set order); then tryLambda until it returns true.  After it: stop when accepted > max_iterations, E is not finite,
- *           |E_prev - E| < absolute_error_tol, |E_prev - E| / |E_prev| < relative_error_tol or E < error_tol; E_prev = E.
- *   tryLambda: Cholesky of G + lambda I (not positive definite: not solved); lin_change = d'g - 0.5 d'Gd; if solved and
- *           lin_change >= 0: T' = T Exp(d) (tangent [w, v]), E' = the set's error at T' with the correspondences of the linearize,
- *           success iff lin_change > DBL_EPSILON * 0.5 sum f and (E - E') / lin_change > min_model_fidelity, stop iff |E - E'| <
- *           relative_error_tol * E.  Success: T = T', E = E', lambda = max(lambda / lambda_factor, lambda_lower_bound), accepted++,
- *           true.  Otherwise if !stop: lambda *= lambda_factor, true iff lambda >= lambda_upper_bound.  Otherwise true.
- *   A member's correspondence-update tolerance (b2_factor_set_correspondence_update_tolerance) is applied before every linearize,
- *   on the device, as the host-pose linearize applies it.  On return every member's host-side state (linearization point,
- *   correspondences, the pose of the last correspondence update) is what the same sequence of b2_factor_set_linearize /
- *   b2_factor_set_error calls would have left.
- * Deliberate differences from the reference: unary factors only; one pose variable; only the fixed lambda factor; no diagonal
- * damping; no callbacks and no termination_criteria; error0 (not DBL_MAX) is the first E_prev.  So that the device loop always
- * ends, absolute_error_tol must be positive, lambda must stay a normal positive double through max_iterations + 1 decreases, and
- * the parameters must allow at most 2^22 tryLambda calls (2 (max_iterations + 2) outer iterations times the rejected steps from the
- * smallest reachable lambda to lambda_upper_bound, DESIGN.md 4.9); the device stops at that bound (B2_LM_TRY_LIMIT).
+ *   outer:  linearize every member at the current deltas; E = the graph's error at the same deltas; assemble G, g (below); then
+ *           tryLambda until it returns true.  After it: stop when accepted > max_iterations, E is not finite, |E_prev - E| <
+ *           absolute_error_tol, |E_prev - E| / |E_prev| < relative_error_tol or E < error_tol; E_prev = E.
+ *   assembly: the dense 6N x 6N system G, g.  Each block of G and segment of g is the sum of its contributions in set order, then
+ *           in prior order, from 0.0: a member adds H_source to (s, s), H_target to (t, t), H_target_source to (t, s) and its
+ *           transpose to (s, t), b_target and b_source to segments t and s; a prior adds H to (var, var) and b to segment var;
+ *           g = -(sum).  E = the members' errors in set order, then the priors' errors; half_f = 0.5 (sum of f) in the same order.
+ *           error0 and E' are sums of the same form.
+ *   tryLambda: solve (G + lambda I) d = g by Cholesky on G's lower triangle (not positive definite: not solved), forward and back
+ *           substitution; every inner sum runs over ascending index (a right-looking factorization keeps that order);
+ *           lin_change = d'g - 0.5 d'Gd over the full G; if solved and lin_change >= 0: T'_v = T_v Exp(d_v) for every variable v
+ *           (tangent [w, v]), E' = the graph's error at T' with the correspondences of the linearize, success iff lin_change >
+ *           DBL_EPSILON * half_f and (E - E') / lin_change > min_model_fidelity, stop iff |E - E'| < relative_error_tol * E.
+ *           Success: T = T', E = E', lambda = max(lambda / lambda_factor, lambda_lower_bound), accepted++, true.  Otherwise if
+ *           !stop: lambda *= lambda_factor, true iff lambda >= lambda_upper_bound.  Otherwise true.
+ *   A member's correspondence-update tolerance (b2_factor_set_correspondence_update_tolerance) is applied to its delta before
+ *   every linearize, on the device, as the host-pose linearize applies it.  On return every member's host-side state
+ *   (linearization point, correspondences, the pose of the last correspondence update) is what the same sequence of
+ *   b2_factor_set_linearize / b2_factor_set_error calls would have left.
+ *   A graph without a prior (or one that leaves a gauge free) has a G that is only positive semidefinite: lambda I makes the damped
+ *   system solvable, g has no component along the free directions, so the steps leave the gauge in place up to rounding, and the
+ *   loop ends under the same rules with finite poses; only the relative poses are determined.
+ * Deliberate differences from the reference: only the fixed lambda factor; no diagonal damping; no callbacks and no
+ * termination_criteria; error0 (not DBL_MAX) is the first E_prev; a dense Cholesky in variable-index order instead of GTSAM's
+ * sparse elimination under COLAMD, so rounding differs; diagonal prior precisions only; no other factor types (no BetweenFactor,
+ * IMU or other families).
+ * So that the device loop always ends, absolute_error_tol must be positive, lambda must stay a normal positive double through
+ * max_iterations + 1 decreases, and the parameters must allow at most 2^22 tryLambda calls (2 (max_iterations + 2) outer
+ * iterations times the rejected steps from the smallest reachable lambda to lambda_upper_bound, DESIGN.md 4.9); the device stops
+ * at that bound (B2_LM_TRY_LIMIT).
  * All arithmetic of the loop is float64 without fused multiply-adds (DESIGN.md 4.9), so it can be restated on the host bit for bit
- * except for Exp's sin / cos / sqrt.  The tolerance test's rotation angle uses atan2 and sqrt, on the device here and on the host in
- * the host-pose linearize: for a pose whose angle or distance to the last correspondence update lies within a few ulps of the
- * tolerance, the two may decide differently, and only then does the state left differ from the host sequence's. */
+ * except for the sin / cos / tan / atan2 / sqrt of Exp, of the priors' Logmap and of its derivative.  The tolerance test's
+ * rotation angle uses atan2 and sqrt, on the device here and on the host in the host-pose linearize: for a pose whose angle or
+ * distance to the last correspondence update lies within a few ulps of the tolerance, the two may decide differently, and only
+ * then does the state left differ from the host sequence's. */
 typedef struct b2_lm_params {
   int32_t max_iterations;     /* >= 0 (100) */
   int32_t reserved;
@@ -1169,65 +1196,6 @@ typedef struct b2_lm_summary {
   int32_t reserved;
 } b2_lm_summary;
 
-/* One tryLambda.  A step that was not tried (not solved, or lin_change < 0) has T_trial = T_lin and error_trial = NaN. */
-typedef struct b2_lm_trace_entry {
-  int32_t outer;              /* 0-based outer iteration */
-  int32_t solved, success, stop;
-  double lambda;              /* lambda the step was solved with */
-  double T_lin[16];           /* linearization pose (row-major) */
-  double G[36], g[6];         /* as reduced on the device */
-  double error;               /* E */
-  double half_f;              /* 0.5 sum f of the linearize */
-  double d[6];
-  double lin_change;
-  double T_trial[16];
-  double error_trial;         /* E' */
-  double fidelity;            /* 0 unless lin_change > DBL_EPSILON * half_f */
-} b2_lm_trace_entry;
-
-/* T_targets: host, F x 16 (member i's fixed target pose); T_init, T_out: host, 16.  Blocks until T_out is on the host.  summary
- * may be NULL.  trace may be NULL; otherwise it receives the first trace_capacity entries and *trace_len (may be NULL) the full
- * count.  Errors before any device work (B2_ERR_INVALID_ARGUMENT): NULL pointers, non-finite poses or parameters, parameters
- * out of range (checked before the set is read).  The first call on a set captures and instantiates its graph and allocates its
- * buffers; later calls reuse them, so a caller that optimizes every frame keeps one set per factor configuration.  The set's offloading rule applies (b2_factor_set_enable_offloading).  A driver without conditional graph nodes
- * (older than CUDA 12.4) is B2_ERR_INVALID_STATE; there is no host path.  b2_factor_set_launch_count does not count the call. */
-B2_API b2_status b2_factor_set_optimize_pose(b2_factor_set* set, const double* T_targets, const double* T_init, const b2_lm_params* params,
-                                             double* T_out, b2_lm_summary* summary, b2_lm_trace_entry* trace, size_t trace_capacity,
-                                             size_t* trace_len);
-
-/* ------------------------------------------------------------------------------------------------------------
- * Multi-pose optimization on the device: the same loop on a graph of N Pose3 variables T_0..T_{N-1} (1 <= N <= B2_LM_MAX_POSES)
- * made of the set's members, unary or binary, and PriorFactor<Pose3>s -- the graphs of the reference's scan-matching examples
- * (a prior on pose 0 and a binary factor), of demo_matching_cost_factors.cpp (a window of frames) and of its AlignmentTest.
- * b2_factor_set_optimize_pose is this call's N = 1 case with unary members and no prior, and computes the same bits.
- *
- * Rules (those of b2_factor_set_optimize_pose, with):
- *   variables: member i has (target_var, source_var) = member_vars[2i], member_vars[2i + 1]; target_var = -1 makes it unary with
- *           the fixed target pose T_targets[i]; its delta is T[target]^-1 T[source] (T_targets[i]^-1 T[source] when unary), with the
- *           optimizer's pose products.  source_var in [0, N); target_var in [-1, N) and != source_var.
- *   priors: PriorFactor<Pose3>(var, T_prior, diagonal precision p[6]) (GTSAM's Isotropic::Precision(6, 1e6) is p = 1e6 six times):
- *           r = Logmap(T_prior^-1 T_var), tangent [w, v] as Exp's, right for rotation angles in [0, pi] (through atan2 of the
- *           rotation's sine and cosine; above pi / 2 the axis comes from the symmetric part; below 1e-10 rad v = t - 0.5 w x t);
- *           J = Pose3::LogmapDerivative(r), the inverse right Jacobian of SE(3) -- the exact derivative of r under T Exp(d) (series
- *           coefficients below 1e-3 rad for Jw and below 0.1 rad for Q, closed forms above);  H = J' diag(p) J, b = J' diag(p) r,
- *           f = sum_k p_k r_k^2, error = 0.5 f (GTSAM's error; 0.5 f is also its linearized error at zero, as a member's 0.5 f is).
- *           The operation order is stated at prior_eval in b2_optimize.cu.
- *   assembly: the dense 6N x 6N system G, g.  Each block of G and segment of g is the sum of its contributions in set order, then
- *           in prior order, from 0.0: a member adds H_source to (s, s), H_target to (t, t), H_target_source to (t, s) and its
- *           transpose to (s, t), b_target and b_source to segments t and s; a prior adds H to (var, var) and b to segment var;
- *           g = -(sum).  E = the members' errors in set order, then the priors' errors; half_f = 0.5 (sum of f) in the same order.
- *           error0 and E' are sums of the same form.
- *   solve:  Cholesky of G + lambda I on G's lower triangle (not positive definite: not solved), forward and back substitution;
- *           every inner sum runs over ascending index (a right-looking factorization keeps that order); lin_change = d'g - 0.5 d'Gd
- *           over the full G; T'_v = T_v Exp(d_v) for every variable v.
- *   The loop, termination, the parameter check, the tryLambda bound and the correspondence-update tolerance (applied per member, on
- *   its delta) are b2_factor_set_optimize_pose's; so is the host state each member is left in.
- *   A graph without a prior (or one that leaves a gauge free) has a G that is only positive semidefinite: lambda I makes the damped
- *   system solvable, g has no component along the free directions, so the steps leave the gauge in place up to rounding, and the
- *   loop ends under the same rules with finite poses; only the relative poses are determined.
- * Deliberate differences from GTSAM, besides those of b2_factor_set_optimize_pose: a dense Cholesky in variable-index order instead
- * of GTSAM's sparse elimination under COLAMD, so rounding differs; diagonal prior precisions only; no other factor types (no
- * BetweenFactor, IMU or other families). */
 #define B2_LM_MAX_POSES 32  /* a 192 x 192 system: its packed lower triangle fits one CTA's shared memory */
 
 typedef struct b2_pose_prior {
@@ -1237,7 +1205,8 @@ typedef struct b2_pose_prior {
   double precision[6]; /* diagonal, over [w, v]; finite and > 0 */
 } b2_pose_prior;
 
-/* One tryLambda of the graph; its arrays follow in trace_data */
+/* One tryLambda; its arrays follow in trace_data.  A step that was not tried (not solved, or lin_change < 0) has error_trial = NaN
+ * and T_trial = T_lin. */
 typedef struct b2_lm_graph_trace_entry {
   int32_t outer;              /* 0-based outer iteration */
   int32_t solved, success, stop;
@@ -1245,11 +1214,11 @@ typedef struct b2_lm_graph_trace_entry {
   double error;               /* E */
   double half_f;              /* 0.5 sum f of the linearize (priors included) */
   double lin_change;
-  double error_trial;         /* E' (NaN when the step was not tried) */
+  double error_trial;         /* E' */
   double fidelity;            /* 0 unless lin_change > DBL_EPSILON * half_f */
 } b2_lm_graph_trace_entry;
 /* Doubles per trace entry in trace_data, in this order: T_lin (N x 16), G ((6N)^2, full, row-major), g (6N), d (6N),
- * T_trial (N x 16).  A step that was not tried has T_trial = T_lin. */
+ * T_trial (N x 16). */
 B2_API size_t b2_lm_graph_trace_doubles(size_t num_poses);
 
 /* member_vars: host, F x 2 int32 (F = the set's size).  T_targets: host, F x 16, read only for unary members (may be NULL when
@@ -1260,8 +1229,11 @@ B2_API size_t b2_lm_graph_trace_doubles(size_t num_poses);
  * source_var, a variable that no member or prior references, non-finite poses, precisions or parameters, a precision that is not
  * positive, parameters out of range (checked before the set is read, as are the priors and T_init).  The set's graph depends only
  * on its layout and on its buffers' capacities (poses, priors): a call with another topology, other target poses or other priors
- * reuses it unless it needs more poses or priors than an earlier call on the set.  A driver without conditional graph nodes is
- * B2_ERR_INVALID_STATE.  b2_factor_set_launch_count does not count the call. */
+ * reuses it unless it needs more poses or priors than an earlier call on the set.  The first call on a set captures and
+ * instantiates its graph and allocates its buffers; later calls reuse them, so a caller that optimizes every frame keeps one set per
+ * factor configuration.  Blocks until T_out is on the host.  The set's offloading rule applies
+ * (b2_factor_set_enable_offloading).  A driver without conditional graph nodes (older than CUDA 12.4) is B2_ERR_INVALID_STATE;
+ * there is no host path.  b2_factor_set_launch_count does not count the call. */
 B2_API b2_status b2_factor_set_optimize_poses(b2_factor_set* set, size_t num_poses, const int32_t* member_vars, const double* T_targets,
                                               const b2_pose_prior* priors, size_t num_priors, const double* T_init, const b2_lm_params* params,
                                               double* T_out, b2_lm_summary* summary, b2_lm_graph_trace_entry* trace, double* trace_data,

@@ -1,8 +1,12 @@
 """What running the whole Levenberg-Marquardt loop of a pose graph on the device costs: b2_factor_set_optimize_poses (one CUDA graph
 launch per optimization) against the same rules as a compiled host loop over the C ABI (scripts/bench_align_graph_host.cpp: one
 blocking b2_factor_set_linearize per outer iteration, one blocking b2_factor_set_error for error0, each outer iteration's E and each
-tried step, and the same dense 6N solve), alternated in one run on three graphs:
+tried step, and the same dense 6N solve), alternated in one run on five graphs:
 
+  vgicp1m          one pose: one unary VGICP factor, 1M source points, 0.5 m Gaussian voxel map of a 1M-point target (synthetic
+                   clouds);
+  ivoxcov          one pose: one unary GICP factor of a 20k-point KITTI-07 frame (frame 1) against an iVoxCovarianceEstimation
+                   holding frames 0, 2, 3, 4 (the frame-to-map step of odometry);
   multi_frame      the five KITTI-07 frames, four binary VGICP factors (i - 1 -> i, 1.0 m voxels) and a Pose3 prior on frame 0
                    (the reference AlignmentTest's MULTI_FRAME graph);
   full_connection  the same frames with a binary VGICP factor between every pair (10 factors) and the prior: the full-connection
@@ -38,6 +42,7 @@ import gtsam_points_b200 as g  # noqa: E402
 import native  # noqa: E402
 from gtsam_points_b200 import capi  # noqa: E402
 from gtsam_points_b200 import synthetic as syn  # noqa: E402
+from gtsam_points_b200.optimize import _graph_inputs  # noqa: E402
 
 
 def card():
@@ -71,6 +76,30 @@ def kitti(pairs):
     make = lambda: [g.IntegratedVGICPFactor(t, s, maps[t], clouds[s]) for t, s in pairs]  # noqa: E731
     values = {i: z["poses"][i] for i in range(5)}
     return make, values, [g.PriorFactorPose3(0, z["poses"][0], 1e6)], (clouds, maps)
+
+
+def vgicp1m():
+    tp, tc = syn.make_cloud(1_000_000, stream=1, scale=0.25)
+    sp, sc = syn.make_cloud(1_000_000, stream=2, scale=0.25)
+    vm = g.GaussianVoxelMapGPU(0.5)
+    vm.insert(g.PointCloud(tp, tc))
+    src = g.PointCloud(sp, sc)
+    make = lambda: [g.IntegratedVGICPFactor(np.eye(4), 1, vm, src)]  # noqa: E731
+    return make, {1: syn.random_pose(np.random.default_rng(1), 0.02, 0.2)}, [], (vm, src)
+
+
+def ivoxcov():
+    z = np.load(os.path.join(ROOT, "tests", "golden", "kitti07_frames.npz"))
+    gt = z["poses_gt"]
+    iv = g.iVoxCovarianceEstimation(1.0)
+    for i in (0, 2, 3, 4):
+        p = z[f"points{i}"].astype(np.float64)
+        iv.insert(p @ gt[i][:3, :3].T + gt[i][:3, 3])
+    sp = z["points1"].astype(np.float64)
+    sp = sp[np.random.default_rng(0).permutation(len(sp))[:20000]]
+    src = g.PointCloud(sp, g.estimate_covariances(sp, 10))
+    make = lambda: [g.IntegratedGICPFactor(np.eye(4), 1, iv, src)]  # noqa: E731
+    return make, {1: gt[1] @ syn.se3_exp(np.random.default_rng(2).uniform(-0.05, 0.05, 6))}, [], (iv, src)
 
 
 def multi_frame():
@@ -126,17 +155,8 @@ def run(name, setup, reps, warmup, lm_host):
     host_set.add(fs_host)
     dev_set._ensure()
     host_set._ensure()
-    keys = sorted(values)
-    ix = {k: i for i, k in enumerate(keys)}
+    _, keys, mv, targets, pri, T0 = _graph_inputs(fs_host, values, priors)
     N, F = len(keys), len(fs_host)
-    mv = np.ascontiguousarray(np.array([(ix[f.keys()[0]], ix[f.keys()[1]]) for f in fs_host], dtype=np.int32))
-    targets = np.ascontiguousarray(np.zeros((F, 4, 4)))
-    pri = (capi.PosePriorC * len(priors))()
-    for j, p in enumerate(priors):
-        pri[j].var = ix[p.key]
-        pri[j].T_prior[:] = [float(x) for x in np.asarray(p.pose).reshape(16)]
-        pri[j].precision[:] = [float(p.precision)] * 6
-    T0 = np.ascontiguousarray(np.stack([values[k] for k in keys]))
     params = g.LevenbergMarquardtExtParams().to_c()
     # kernel launches of one pass over the set's groups (one b2_factor_set_error call)
     n0 = host_set.launch_count()
@@ -189,7 +209,8 @@ def main():
     c = card()
     print("card:", c)
     lm_host = host_loop()
-    results = [run(n, f, a.reps, a.warmup, lm_host) for n, f in (("multi_frame", multi_frame), ("full_connection", full_connection), ("ring32", ring32))]
+    workloads = (("vgicp1m", vgicp1m), ("ivoxcov", ivoxcov), ("multi_frame", multi_frame), ("full_connection", full_connection), ("ring32", ring32))
+    results = [run(n, f, a.reps, a.warmup, lm_host) for n, f in workloads]
     print(json.dumps(dict(card=c, results=results)))
 
 

@@ -1,7 +1,7 @@
 // test_optimize.cpp -- pose optimization on the device through the C++ adapters (gtsam_points_b200.hpp: optimize_pose_gpu and
 // NonlinearFactorSetGPU::optimize_pose): a unary VGICP factor and a unary GICP factor on one source key, optimized from T_init.  The pose and the accepted steps must equal,
 // bit for bit, what the Python package's optimize_pose_gpu returned for the same data (the case file's expected values); a binary
-// factor and factors on different keys are rejected.  Built standalone and with -I tests/cpp/mock_gtsam by tests/test_optimize_cpp.py.
+// factor, factors on different keys, a non-finite T_init and parameters out of range are rejected with std::invalid_argument.  Built standalone and with -I tests/cpp/mock_gtsam by tests/test_optimize_cpp.py.
 //   usage: test_optimize <case.bin>
 #include "driver.hpp"
 
@@ -41,20 +41,24 @@ int main(int argc, char** argv) {
 
   auto binary = std::make_shared<IntegratedVGICPFactor>(Key(0), Key(1), voxels, source);
   auto other_key = std::make_shared<IntegratedVGICPFactor>(fixed_pose(Tt), Key(2), voxels, source);
-  bool threw = false;
-  try {
-    optimize_pose_gpu({binary}, init);
-  } catch (const std::invalid_argument&) {
-    threw = true;
-  }
-  EXPECT(threw);
-  threw = false;
-  try {
-    optimize_pose_gpu({vgicp, other_key}, init);
-  } catch (const std::invalid_argument&) {
-    threw = true;
-  }
-  EXPECT(threw);
+  auto invalid = [](auto&& call) {
+    try {
+      call();
+    } catch (const std::invalid_argument&) {
+      return true;
+    }
+    return false;
+  };
+  EXPECT(invalid([&] { optimize_pose_gpu({binary}, init); }));
+  EXPECT(invalid([&] { optimize_pose_gpu({vgicp, other_key}, init); }));
+  // the argument errors the C ABI detects throw the same exception: a non-finite T_init, parameters out of range
+  Mat4 bad = init;
+  bad[3] = std::nan("");
+  EXPECT(invalid([&] { set.optimize_pose(bad); }));
+  b2_lm_params p;
+  b2_lm_params_default(&p);
+  p.lambda_factor = 1.0;
+  EXPECT(invalid([&] { set.optimize_pose(init, &p); }));
   std::printf("OK\n");
   return 0;
 }

@@ -1,22 +1,93 @@
 """Host restatement of b2_factor_set_optimize_poses (test infrastructure): LevenbergMarquardtOptimizerExt::optimize() on N Pose3
 variables over unary and binary matching-cost factors and Pose3 priors, with the rules include/b2points.h states and every
-floating-point operation in the device's order (csrc/b2_optimize.cu, compiled without fused multiply-adds): the assembly, the 6N
-Cholesky and substitutions, the prior, and the trial poses.  Python floats are IEEE doubles rounded per operation, so everything
-here except the sin / cos / tan / atan2 / sqrt of Exp and of the prior reproduces the device's bits.
+floating-point operation in the device's order (csrc/b2_optimize.cu, compiled without fused multiply-adds): the pose products, the
+assembly, the 6N Cholesky and substitutions, the prior, and the trial poses.  Python floats are IEEE doubles rounded per operation,
+so everything here except the sin / cos / tan / atan2 / sqrt of Exp and of the prior reproduces the device's bits.
 
 The members are given by an evaluator (linearize(deltas) -> records with H_target, H_source, H_target_source, b_target,
-b_source and error; error(deltas) -> errors, in member order), their topology [(target_var, source_var)] (target_var = -1: unary,
-against T_targets[i]) and the priors [(var, T_prior, precision[6])].  With N = 1, unary members and no prior this is lm_ext_np.
+b_source and error, of which a unary member's needs only H_source, b_source and error; error(deltas) -> errors, in member
+order), their topology [(target_var, source_var)] (target_var = -1: unary, against T_targets[i]) and the priors
+[(var, T_prior, precision[6])].  Factors() wraps a list of factors (anything with linearize(delta) -> record and error(delta) ->
+float, error() after linearize() using the correspondences of that linearize); a device test passes an evaluator backed by a
+whole factor set.  One pose over unary factors is N = 1 with the topology [(-1, 0)] * F and no prior.
 """
 import math
+from dataclasses import dataclass
 
 import numpy as np
 
-from lm_ext_np import TERMINATION, Factors, Params, _div, decide, lambda_after, pose_inv, pose_mul, se3_exp, sum_errors, termination  # noqa: F401
+DBL_EPSILON = 2.220446049250313e-16
+TERMINATION = {0: "none", 1: "max_iterations", 2: "non_finite", 3: "absolute_error_tol", 4: "relative_error_tol", 5: "error_tol"}
+
+
+@dataclass
+class Params:
+    maxIterations: int = 100
+    relativeErrorTol: float = 1e-5
+    absoluteErrorTol: float = 1e-5
+    errorTol: float = 0.0
+    lambdaInitial: float = 1e-5
+    lambdaFactor: float = 10.0
+    lambdaUpperBound: float = 1e5
+    lambdaLowerBound: float = 0.0
+    minModelFidelity: float = 1e-3
 
 
 def _flat(T):
     return [float(x) for x in np.asarray(T, dtype=np.float64).reshape(16)]
+
+
+def _mat(v):
+    return np.array(v, dtype=np.float64).reshape(4, 4)
+
+
+def pose_inv(A):
+    """[R^T | -((R_0r t0 + R_1r t1) + R_2r t2)]"""
+    A = _flat(A)
+    out = [0.0] * 16
+    for r in range(3):
+        for c in range(3):
+            out[r * 4 + c] = A[c * 4 + r]
+        out[r * 4 + 3] = -((A[0 * 4 + r] * A[3] + A[1 * 4 + r] * A[7]) + A[2 * 4 + r] * A[11])
+    out[15] = 1.0
+    return _mat(out)
+
+
+def pose_mul(A, B):
+    """((A_r0 B_0c + A_r1 B_1c) + A_r2 B_2c), plus A_r3 in the translation column; bottom row [0 0 0 1]"""
+    A, B = _flat(A), _flat(B)
+    out = [0.0] * 16
+    for r in range(3):
+        for c in range(4):
+            s = (A[r * 4 + 0] * B[0 * 4 + c] + A[r * 4 + 1] * B[1 * 4 + c]) + A[r * 4 + 2] * B[2 * 4 + c]
+            out[r * 4 + c] = s + A[r * 4 + 3] if c == 3 else s
+    out[15] = 1.0
+    return _mat(out)
+
+
+def se3_exp(xi):
+    """synthetic.se3_exp's formula in the device's operation order."""
+    w0, w1, w2, v0, v1, v2 = (float(x) for x in xi)
+    W = [0.0, -w2, w1, w2, 0.0, -w0, -w1, w0, 0.0]
+    WW = [(W[r * 3 + 0] * W[0 * 3 + c] + W[r * 3 + 1] * W[1 * 3 + c]) + W[r * 3 + 2] * W[2 * 3 + c] for r in range(3) for c in range(3)]
+    th2 = (w0 * w0 + w1 * w1) + w2 * w2
+    th = math.sqrt(th2)
+    eye = [1.0 if r == c else 0.0 for r in range(3) for c in range(3)]
+    if th < 1e-10:
+        R = [eye[k] + W[k] for k in range(9)]
+        V = [eye[k] + 0.5 * W[k] for k in range(9)]
+    else:
+        s, co = math.sin(th), math.cos(th)
+        a, b, c3 = s / th, (1.0 - co) / th2, (th - s) / (th2 * th)
+        R = [(eye[k] + a * W[k]) + b * WW[k] for k in range(9)]
+        V = [(eye[k] + b * W[k]) + c3 * WW[k] for k in range(9)]
+    T = [0.0] * 16
+    for r in range(3):
+        for c in range(3):
+            T[r * 4 + c] = R[r * 3 + c]
+        T[r * 4 + 3] = (V[r * 3 + 0] * v0 + V[r * 3 + 1] * v1) + V[r * 3 + 2] * v2
+    T[15] = 1.0
+    return _mat(T)
 
 
 def mul3(A, B):
@@ -140,8 +211,8 @@ def deltas_at(topo, T_targets, T):
 def assemble(records, topo, priors, T, N):
     """lm_reduce: -> (G (6N x 6N), g (6N), half_f).  Blocks and segments sum their contributions in set order, then prior order."""
     n = 6 * N
-    recs = [{k: [float(x) for x in np.asarray(r[k], dtype=np.float64).reshape(-1)] for k in ("H_target", "H_source", "H_target_source", "b_target", "b_source")}
-            for r in records]
+    recs = [{k: [float(x) for x in np.asarray(r[k], dtype=np.float64).reshape(-1)] for k in ("H_target", "H_source", "H_target_source", "b_target", "b_source")
+             if k in r} for r in records]
     plin = [prior_eval(pr, T[pr[0]]) for pr in priors]
     G = [0.0] * (n * n)
     for row in range(n):
@@ -240,6 +311,67 @@ def solve(G, g, lam):
 
 def trial_poses(T, d, tried):
     return [pose_mul(Tv, se3_exp(d[6 * v:6 * v + 6])) if tried else np.asarray(Tv, dtype=np.float64).copy() for v, Tv in enumerate(T)]
+
+
+def _div(a, b):
+    """IEEE a / b (Python raises on b == 0)"""
+    if b != 0.0:
+        return a / b
+    if a != a or a == 0.0:
+        return math.nan
+    return math.copysign(math.inf, a) * math.copysign(1.0, b)
+
+
+def decide(E, E_trial, lin_change, half_f, solved, p: Params):
+    """tryLambda's verdict on one step -> (tried, success, stop, fidelity)"""
+    tried = bool(solved) and lin_change >= 0.0
+    success = stop = False
+    fid = 0.0
+    if tried:
+        cost_change = E - E_trial
+        if lin_change > DBL_EPSILON * half_f:
+            fid = _div(cost_change, lin_change)
+            success = fid > p.minModelFidelity
+        stop = abs(cost_change) < p.relativeErrorTol * E
+    return tried, success, stop, fid
+
+
+def lambda_after(lam, success, stop, p: Params):
+    """-> (new lambda, tryLambda's return value)"""
+    if success:
+        return max(lam / p.lambdaFactor, p.lambdaLowerBound), True
+    if not stop:
+        lam = lam * p.lambdaFactor
+        return lam, lam >= p.lambdaUpperBound
+    return lam, True
+
+
+def termination(accepted, E_prev, E_new, p: Params):
+    delta = abs(E_prev - E_new)
+    if accepted > p.maxIterations:
+        return 1
+    if not math.isfinite(E_new):
+        return 2
+    if delta < p.absoluteErrorTol:
+        return 3
+    if _div(delta, abs(E_prev)) < p.relativeErrorTol:
+        return 4
+    if E_new < p.errorTol:
+        return 5
+    return 0
+
+
+class Factors:
+    """The evaluator of a list of factors, one call per factor."""
+
+    def __init__(self, factors):
+        self.factors = list(factors)
+
+    def linearize(self, deltas):
+        return [f.linearize(d) for f, d in zip(self.factors, deltas)]
+
+    def error(self, deltas):
+        return [f.error(d) for f, d in zip(self.factors, deltas)]
 
 
 def optimize(evaluator, topo, T_targets, priors, T_init, p: Params | None = None):

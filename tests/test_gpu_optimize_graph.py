@@ -5,8 +5,6 @@
   (and E, E') may differ, within 1e-12 relative (atan2 / sin / cos / tan); d and lin_change re-solved from the entry's own G and g
   bit for bit, T' within 1e-14, every decision and lambda exactly.  Graphs: FORWARD, BACKWARD and MULTI_FRAME on KITTI-07, the
   demo's 5-frame full connection, a mixed-kind graph, a prior with a large rotational residual and a 32-pose ring;
-* at N = 1 (unary members, no prior) b2_factor_set_optimize_poses and b2_factor_set_optimize_pose give the same pose, summary and
-  trace bytes;
 * the four AlignmentTest shapes pass the reference's gates with CUDA factors for VGICP, GICP and ICP;
 * the tolerance's frozen flags and the host state left for binary members, repeated calls with another topology and other priors
   (no re-capture unless a capacity grows), a call after an iVox insert, after a regroup and with offloaded objects;
@@ -18,7 +16,6 @@ import os
 import numpy as np
 import pytest
 
-import lm_ext_np as lm
 import lm_graph_np as lg
 import mini_lm
 from gtsam_points_b200 import capi
@@ -96,7 +93,7 @@ def graph_of(fs, values, priors):
 
 def replay(fset, fs, values, priors, res, p=None, graph=None):
     """graph: (topology, T_targets, host priors) when the call's topology is not the factors' own keys"""
-    p = p or lm.Params()
+    p = p or lg.Params()
     topo, targets, hp = graph or graph_of(fs, values, priors)
     N = len(res.keys)
     ev = SetEvaluator(fset)
@@ -131,9 +128,9 @@ def replay(fset, fs, values, priors, res, p=None, graph=None):
             assert same(Et, e["error_trial"]), (k, Et, e["error_trial"])
         else:
             assert bits(e["T_trial"], e["T_lin"]) and np.isnan(e["error_trial"])
-        _, success, stop, fid = lm.decide(e["error"], e["error_trial"], e["lin_change"], e["half_f"], e["solved"], p)
+        _, success, stop, fid = lg.decide(e["error"], e["error_trial"], e["lin_change"], e["half_f"], e["solved"], p)
         assert (success, stop) == (e["success"], e["stop"]) and bits(fid, e["fidelity"]), k
-        lam, done = lm.lambda_after(e["lam"], success, stop, p)
+        lam, done = lg.lambda_after(e["lam"], success, stop, p)
         if k + 1 < len(tr):
             assert bits(lam, tr[k + 1]["lam"]), k
             assert done == (tr[k + 1]["outer"] != e["outer"]), k
@@ -145,33 +142,21 @@ def replay(fset, fs, values, priors, res, p=None, graph=None):
     assert bits(np.stack([res.values[k] for k in res.keys]), final)
 
 
-def raw_call(g, fset, topo, targets, priors, T_init, cap=256):
+def raw_call(fset, topo, targets, priors, T_init, cap=256):
     """b2_factor_set_optimize_poses with an explicit topology and host priors [(var, pose, precision[6])] (keys 0..N-1) -> a result
     shaped as optimize_graph_gpu's"""
     from gtsam_points_b200 import optimize as opt
 
-    L = capi.lib()
     N = len(T_init)
-    mv = np.ascontiguousarray(np.array(topo, dtype=np.int32))
-    tg = np.ascontiguousarray(np.stack([np.eye(4) if t is None else t for t in targets]))
+    mv = np.array(topo, dtype=np.int32)
+    tg = np.stack([np.eye(4) if t is None else t for t in targets])
     pri = (capi.PosePriorC * max(len(priors), 1))()
     for j, (var, pose, prec) in enumerate(priors):
         pri[j].var = var
         pri[j].T_prior[:] = [float(x) for x in np.asarray(pose).reshape(16)]
         pri[j].precision[:] = [float(x) for x in prec]
-    per = L.b2_lm_graph_trace_doubles(N)
-    entries, data = (capi.LmGraphTraceEntryC * cap)(), np.zeros(cap * per)
-    out, summary, n = np.zeros((N, 4, 4)), capi.LmSummaryC(), C.c_size_t()
-    p = g.LevenbergMarquardtExtParams().to_c()
-    capi.check(L.b2_factor_set_optimize_poses(fset.h, N, mv.ctypes.data_as(C.POINTER(C.c_int32)), capi.dptr(tg), pri, len(priors),
-                                              capi.dptr(np.ascontiguousarray(np.stack(T_init))), C.byref(p), capi.dptr(out), C.byref(summary), entries,
-                                              capi.dptr(data), cap, C.byref(n)))
-    tr = [opt._graph_trace_dict(entries[i], data[i * per:(i + 1) * per], N) for i in range(min(cap, n.value))]
-    return opt.GraphOptimizationResult(values={k: out[k] for k in range(N)}, keys=list(range(N)), iterations=summary.iterations,
-                                       outer_iterations=summary.outer_iterations, inner_iterations=summary.inner_iterations,
-                                       linearizations=summary.linearizations, error_evaluations=summary.error_evaluations, error0=summary.error0,
-                                       error=summary.error, lambda_=summary.lambda_, termination=capi.B2_LM_TERMINATION[summary.termination], trace=tr,
-                                       trace_len=n.value)
+    out, result = opt._optimize(fset, fset.factors, mv, tg, pri, len(priors), np.stack(T_init), None, cap)
+    return opt.GraphOptimizationResult(values={k: out[k] for k in range(N)}, keys=list(range(N)), **result)
 
 
 def run(g, fs, values, priors=(), **kw):
@@ -243,39 +228,6 @@ def test_step_locked_replay(g, scene, shape):
     assert res.iterations >= 1
     replay(fset, fs, values, priors, res)
     del keep  # the targets outlive the call
-
-
-def test_one_pose_call_is_the_n1_graph_bit_for_bit(g, scene):
-    T0 = scene["gt"][1] @ syn.se3_exp(np.random.default_rng(5).uniform(-0.05, 0.05, 6))
-    sets = []
-    for _ in range(2):
-        fs = [factor(g, scene, "VGICP", scene["gt"][0], 1, 0, 1), factor(g, scene, "GICP", scene["gt"][0], 1, 0, 1)]
-        fset = g.NonlinearFactorSetGPU(fs[0].ctx)
-        fset.add(fs)
-        fset._ensure()
-        sets.append((fset, fs))
-    L = capi.lib()
-    targets = np.ascontiguousarray(np.stack([scene["gt"][0]] * 2))
-    p = g.LevenbergMarquardtExtParams().to_c()
-    cap = 256
-    a_T, a_sum, a_tr, a_n = np.zeros((4, 4)), capi.LmSummaryC(), (capi.LmTraceEntryC * cap)(), C.c_size_t()
-    capi.check(L.b2_factor_set_optimize_pose(sets[0][0].h, capi.dptr(targets), capi.dptr(np.ascontiguousarray(T0)), C.byref(p), capi.dptr(a_T),
-                                             C.byref(a_sum), a_tr, cap, C.byref(a_n)))
-    per = L.b2_lm_graph_trace_doubles(1)
-    b_T, b_sum, b_tr, b_n = np.zeros((1, 4, 4)), capi.LmSummaryC(), (capi.LmGraphTraceEntryC * cap)(), C.c_size_t()
-    data = np.zeros(cap * per)
-    vars_ = np.array([[-1, 0], [-1, 0]], dtype=np.int32)
-    capi.check(L.b2_factor_set_optimize_poses(sets[1][0].h, 1, vars_.ctypes.data_as(C.POINTER(C.c_int32)), capi.dptr(targets), None, 0,
-                                              capi.dptr(np.ascontiguousarray(T0[None])), C.byref(p), capi.dptr(b_T), C.byref(b_sum), b_tr, capi.dptr(data), cap,
-                                              C.byref(b_n)))
-    assert bits(a_T, b_T[0]) and bytes(a_sum) == bytes(b_sum) and a_n.value == b_n.value > 0
-    for k in range(a_n.value):
-        e = capi.LmTraceEntryC()
-        x, f = data[k * per:(k + 1) * per], b_tr[k]
-        e.outer, e.solved, e.success, e.stop, e.lambda_ = f.outer, f.solved, f.success, f.stop, f.lambda_
-        e.T_lin[:], e.G[:], e.g[:], e.d[:], e.T_trial[:] = list(x[:16]), list(x[16:52]), list(x[52:58]), list(x[58:64]), list(x[64:80])
-        e.error, e.half_f, e.lin_change, e.error_trial, e.fidelity = f.error, f.half_f, f.lin_change, f.error_trial, f.fidelity
-        assert bytes(e) == bytes(a_tr[k]), k
 
 
 @pytest.mark.parametrize("method", ["VGICP", "GICP", "ICP"])
@@ -378,7 +330,7 @@ def test_reuse_across_topologies_priors_inserts_regroups_and_offload(g, scene):
     # member on the other variable.  The topology is a per-call input: the same graph, and the replay holds for the new shape
     topo = [(1, 0), (-1, 1)]
     graph = (topo, [None, np.eye(4)], [(0, poses[1], np.full(6, 1e6))])
-    res = raw_call(g, fset, *graph, [poses[1], poses[2]])
+    res = raw_call(fset, *graph, [poses[1], poses[2]])
     assert builds() == 2 and res.termination != "none"
     replay(fset, fs, None, None, res, graph=graph)
     res = g.optimize_graph_gpu(fset, {1: poses[1], 2: poses[2]}, pri2[:1], trace=True)

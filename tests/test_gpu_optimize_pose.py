@@ -1,4 +1,5 @@
-"""Pose optimization on the device (b2_factor_set_optimize_pose, -m gpu) against the host restatement (lm_ext_np).
+"""Pose optimization on the device (optimize_pose_gpu: b2_factor_set_optimize_poses with N = 1, unary members and no prior, -m gpu)
+against the host restatement (lm_graph_np).
 
 * step-locked parity for every factor kind and for mixed sets: each trace entry is replayed on the host from the device's own
   state -- G, g, 0.5 sum f and E from b2_factor_set_linearize / _error at the entry's linearization pose, E' from
@@ -17,7 +18,7 @@ import os
 import numpy as np
 import pytest
 
-import lm_ext_np as lm
+import lm_graph_np as lg
 import mini_lm
 from gtsam_points_b200 import capi
 from gtsam_points_b200 import synthetic as syn
@@ -111,7 +112,7 @@ def make_set(g, scene, kinds):
 
 
 class SetEvaluator:
-    """lm_ext_np's evaluator over a whole factor set (b2_factor_set_linearize / _error)"""
+    """lm_graph_np's evaluator over a whole factor set (b2_factor_set_linearize / _error)"""
 
     def __init__(self, fset):
         self.fset = fset
@@ -127,13 +128,23 @@ class SetEvaluator:
         return list(out)
 
 
+def deltas(targets, T):
+    """the unary members' deltas at the one pose T"""
+    return lg.deltas_at([(-1, 0)] * len(targets), targets, [T])
+
+
+def assemble(records, T):
+    """-> (G, g, half_f) of one pose over unary members"""
+    return lg.assemble(records, [(-1, 0)] * len(records), [], [T], 1)
+
+
 def bits(a, b):
     return np.array_equal(np.asarray(a, dtype=np.float64).view(np.int64), np.asarray(b, dtype=np.float64).view(np.int64))
 
 
 def replay(fset, targets, res, p=None):
     """Replays every trace entry on the host from the device's own state."""
-    p = p or lm.Params()
+    p = p or lg.Params()
     ev = SetEvaluator(fset)
     tr = res.trace
     assert len(tr) == res.trace_len == res.inner_iterations
@@ -142,23 +153,23 @@ def replay(fset, targets, res, p=None):
         if e["outer"] != outer:
             assert e["outer"] == outer + 1
             outer = e["outer"]
-            ds = [lm.delta_of(Tt, e["T_lin"]) for Tt in targets]
-            G, gv, half_f = lm.reduce(ev.linearize(ds))
-            E = lm.sum_errors(ev.error(ds))
+            ds = deltas(targets, e["T_lin"])
+            G, gv, half_f = assemble(ev.linearize(ds), e["T_lin"])
+            E = lg.total_error(ev.error(ds), [], [e["T_lin"]])
             assert bits(G, e["G"]) and bits(gv, e["g"]) and bits(half_f, e["half_f"]), k
             assert bits(E, e["error"]), (k, E, e["error"])
-        solved, d, lin = lm.solve(e["G"], e["g"], e["lam"])
+        solved, d, lin = lg.solve(e["G"], e["g"], e["lam"])
         assert solved == e["solved"] and bits(d, e["d"]) and bits(lin, e["lin_change"]), k
         if solved and lin >= 0.0:
-            T_host = lm.pose_mul(e["T_lin"], lm.se3_exp(d))
+            T_host = lg.pose_mul(e["T_lin"], lg.se3_exp(d))
             assert np.abs(T_host - e["T_trial"]).max() <= 1e-14, k
-            Et = lm.sum_errors(ev.error([lm.delta_of(Tt, e["T_trial"]) for Tt in targets]))
+            Et = lg.total_error(ev.error(deltas(targets, e["T_trial"])), [], [e["T_trial"]])
             assert bits(Et, e["error_trial"]), (k, Et, e["error_trial"])
         else:
             assert bits(e["T_trial"], e["T_lin"]) and np.isnan(e["error_trial"])
-        _, success, stop, fid = lm.decide(e["error"], e["error_trial"], e["lin_change"], e["half_f"], e["solved"], p)
+        _, success, stop, fid = lg.decide(e["error"], e["error_trial"], e["lin_change"], e["half_f"], e["solved"], p)
         assert (success, stop) == (e["success"], e["stop"]) and bits(fid, e["fidelity"]), k
-        lam, done = lm.lambda_after(e["lam"], success, stop, p)
+        lam, done = lg.lambda_after(e["lam"], success, stop, p)
         if k + 1 < len(tr):
             assert bits(lam, tr[k + 1]["lam"]), k
             assert done == (tr[k + 1]["outer"] != e["outer"]), k
@@ -192,13 +203,13 @@ def test_end_to_end_matches_the_restatement_and_meets_the_gates(g, scene, kinds)
     res = g.optimize_pose_gpu(fset, T0, trace=True)
     assert fset.launch_count() == launches  # the call's launches are its own
     fset2, _, _, keep2 = make_set(g, scene, kinds)
-    ref = lm.optimize(SetEvaluator(fset2), targets, T0)
+    ref = lg.optimize(SetEvaluator(fset2), [(-1, 0)] * len(targets), targets, [], [T0])
     assert res.iterations == ref["iterations"] and res.inner_iterations == ref["inner_iterations"]
     assert [e["success"] for e in res.trace] == [e["success"] for e in ref["trace"]]
     assert res.termination == ref["termination"]
-    assert np.abs(res.pose - ref["pose"]).max() < 1e-9
+    assert np.abs(res.pose - ref["poses"][0]).max() < 1e-9
     gate(res.pose, scene["gt"][1])
-    gate(ref["pose"], scene["gt"][1])
+    gate(ref["poses"][0], scene["gt"][1])
 
 
 def test_correspondence_update_tolerance_follows_the_host_rule(g, scene):
@@ -215,24 +226,23 @@ def test_correspondence_update_tolerance_follows_the_host_rule(g, scene):
     res = g.optimize_pose_gpu(fa, T0, trace=True)
     # the host-driven sequence of the same calls on the twin set
     ev = SetEvaluator(fb)
-    deltas = lambda T: [lm.delta_of(Tt, T) for Tt in targets]  # noqa: E731
-    ev.error(deltas(T0))
+    ev.error(deltas(targets, T0))
     outer = -1
     for e in res.trace:
         if e["outer"] != outer:
             outer = e["outer"]
-            G, gv, half_f = lm.reduce(ev.linearize(deltas(e["T_lin"])))
+            G, gv, half_f = assemble(ev.linearize(deltas(targets, e["T_lin"])), e["T_lin"])
             assert bits(G, e["G"]) and bits(gv, e["g"]), outer
-            ev.error(deltas(e["T_lin"]))
+            ev.error(deltas(targets, e["T_lin"]))
         if e["solved"] and e["lin_change"] >= 0.0:
-            ev.error(deltas(e["T_trial"]))
+            ev.error(deltas(targets, e["T_trial"]))
     # afterwards both sets answer a linearize / error at a nearby pose with the same bits
     T1 = res.pose @ syn.se3_exp(np.full(6, 1e-3))
     for T in (T1, res.pose):
-        la, lb = SetEvaluator(fa).linearize(deltas(T)), ev.linearize(deltas(T))
+        la, lb = SetEvaluator(fa).linearize(deltas(targets, T)), ev.linearize(deltas(targets, T))
         for ra, rb in zip(la, lb):
             assert all(bits(ra[k], rb[k]) for k in ("H_source", "b_source", "error"))
-        assert bits(SetEvaluator(fa).error(deltas(T1)), ev.error(deltas(T1)))
+        assert bits(SetEvaluator(fa).error(deltas(targets, T1)), ev.error(deltas(targets, T1)))
 
 
 def test_repeated_calls_inserts_regroups_and_offload(g, scene):
@@ -307,14 +317,15 @@ def test_summary_counts_and_params(g, scene):
     fset, fs, targets, keep = make_set(g, scene, ("vgicp",))
     p = g.LevenbergMarquardtExtParams(maxIterations=2, lambdaInitial=1e3, lambdaUpperBound=1e4)
     res = g.optimize_pose_gpu(fset, init_pose(scene), p, trace=True)
-    replay(fset, targets, res, lm.Params(maxIterations=2, lambdaInitial=1e3, lambdaUpperBound=1e4))
+    replay(fset, targets, res, lg.Params(maxIterations=2, lambdaInitial=1e3, lambdaUpperBound=1e4))
     assert res.iterations <= 3
     s = capi.LmSummaryC()
     pc = p.to_c()
     pc.lambda_factor = 1.0
     T = np.eye(4)
-    st = capi.lib().b2_factor_set_optimize_pose(fset.h, capi.dptr(np.ascontiguousarray(np.stack(targets))), capi.dptr(T), C.byref(pc), capi.dptr(np.zeros((4, 4))),
-                                                C.byref(s), None, 0, None)
+    member_vars = np.array([[-1, 0]] * len(targets), dtype=np.int32)
+    st = capi.lib().b2_factor_set_optimize_poses(fset.h, 1, member_vars.ctypes.data_as(C.POINTER(C.c_int32)), capi.dptr(np.ascontiguousarray(np.stack(targets))),
+                                                 None, 0, capi.dptr(T), C.byref(pc), capi.dptr(np.zeros((4, 4))), C.byref(s), None, None, 0, None)
     assert st == 1
     # a lambda factor so close to 1 that the loop could run for days is refused, and the set still works
     with pytest.raises(capi.B2Error, match="tryLambda calls"):

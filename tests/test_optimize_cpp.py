@@ -14,7 +14,7 @@ from gtsam_points_b200 import synthetic as syn
 def test_optimize_adapter_compiles(mock_gtsam):
     exe = native.adapter_driver("test_optimize", mock_gtsam)
     syms = subprocess.run(["nm", "-C", exe], capture_output=True, text=True).stdout
-    for s in ("b2_factor_set_optimize_pose", "b2_lm_params_default"):
+    for s in ("b2_factor_set_optimize_poses", "b2_lm_params_default"):
         assert s in syms, s
 
 

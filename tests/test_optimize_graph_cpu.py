@@ -1,14 +1,14 @@
 """CPU checks of the multi-pose device optimizer's rules (b2_factor_set_optimize_poses) through their host restatement,
 lm_graph_np:
 
-* at N = 1 with unary members and no prior the restatement is lm_ext_np, bit for bit, on the same records;
 * the prior's Logmap and its derivative J against an extended-precision (mpmath) Logmap and its central difference, 1e-12
   relative, at rotation angles below 1e-10, near 1e-5, 1 and pi - 1e-6, and far from the origin; and, independently of the Logmap's
   algebra, Exp(Log(X)) = X and agreement with mpmath's matrix logarithm where that is real;
 * a G + lambda I that is not positive definite, and a graph with no prior (a free gauge) that ends finite;
 * the restatement over the CPU oracle's factors passes the reference's 0.015 rad / 0.15 m gates on KITTI-07 in the four
   AlignmentTest shapes (src/test/test_matching_cost_factors.cpp:239-303) for GICP, VGICP and ICP, with test_alignment_gates' budgets;
-* the ABI checks that run before the set is read (a set pointer that is never dereferenced shows it), and the Python argument errors.
+* the ABI's defaults and the checks that run before the set is read (a set pointer that is never dereferenced shows it): NULL
+  arguments, every parameter bound, poses and priors; and the Python argument errors.
 """
 import ctypes as C
 import math
@@ -18,7 +18,6 @@ import mpmath as mp
 import numpy as np
 import pytest
 
-import lm_ext_np as lm
 import lm_graph_np as lg
 import mini_lm
 import oracle_lib as orc
@@ -133,7 +132,7 @@ def test_prior_contribution_is_the_gauss_newton_model():
     T = T_prior @ syn.se3_exp(np.array([0.4, -0.2, 0.1, 0.3, 0.1, -0.2]))
     p = [1e6, 2e6, 3e6, 1e5, 2e5, 3e5]
     f, H, b = lg.prior_eval((0, T_prior, p), T)
-    r, th = lg.se3_log(lm.pose_mul(lm.pose_inv(T_prior), T))
+    r, th = lg.se3_log(lg.pose_mul(lg.pose_inv(T_prior), T))
     J = np.array(lg.se3_log_derivative(r, th)).reshape(6, 6)
     P = np.diag(p)
     assert np.allclose(np.array(H).reshape(6, 6), J.T @ P @ J, rtol=1e-13, atol=0)
@@ -171,19 +170,6 @@ def bits(a, b):
     return np.array_equal(np.asarray(a, dtype=np.float64).view(np.int64), np.asarray(b, dtype=np.float64).view(np.int64))
 
 
-def test_one_pose_restatement_is_lm_ext_np(kitti):
-    T0 = kitti["poses"][1]
-    # one thread: the oracle's multi-threaded sums are not reproducible from run to run
-    a = lm.optimize([oracle_factor(kitti, "GICP", 0, 1, threads=1)], [kitti["poses"][0]], T0)
-    b = lg.optimize([oracle_factor(kitti, "GICP", 0, 1, threads=1)], [(-1, 0)], [kitti["poses"][0]], [], [T0])
-    assert len(a["trace"]) == len(b["trace"]) and a["iterations"] == b["iterations"] and a["termination"] == b["termination"]
-    for x, y in zip(a["trace"], b["trace"]):
-        for k in ("G", "g", "d", "lin_change", "error", "error_trial", "half_f", "fidelity", "lam"):
-            assert bits(x[k], y[k]), k
-        assert bits(x["T_trial"], y["T_trial"][0]) and bits(x["T_lin"], y["T_lin"][0])
-    assert bits(a["pose"], b["poses"][0]) and bits(a["error"], b["error"])
-
-
 def test_solve_matches_numpy_and_refuses_a_not_positive_definite_system():
     rng = np.random.default_rng(2)
     A = rng.normal(size=(30, 30))
@@ -195,11 +181,6 @@ def test_solve_matches_numpy_and_refuses_a_not_positive_definite_system():
     G[17, 17] = -50.0
     ok, d, lin = lg.solve(G, g, 1e-3)
     assert not ok and not d.any() and lin == 0.0
-    # the 6 x 6 case is lm_ext_np's solve, bit for bit
-    G6 = G[:6, :6] @ G[:6, :6].T
-    for lam in (1e-5, 1.0):
-        x, y = lg.solve(G6, g[:6], lam), lm.solve(G6, g[:6], lam)
-        assert x[0] == y[0] and bits(x[1], y[1]) and bits(x[2], y[2])
 
 
 class QuadraticGraph:
@@ -249,7 +230,7 @@ def test_a_not_positive_definite_system_raises_lambda():
             return out
 
     ev = Indefinite([[1.0, 0, 0]])
-    r = lg.optimize(ev, [(-1, 0)], [np.eye(4)], [(0, np.eye(4), [1.0] * 6)], [np.eye(4)], lm.Params(maxIterations=0))
+    r = lg.optimize(ev, [(-1, 0)], [np.eye(4)], [(0, np.eye(4), [1.0] * 6)], [np.eye(4)], lg.Params(maxIterations=0))
     unsolved = [e for e in r["trace"] if not e["solved"]]
     assert unsolved and all(np.isnan(e["error_trial"]) and bits(e["T_trial"], e["T_lin"]) for e in unsolved)
     assert np.all(np.isfinite(r["poses"]))
@@ -258,7 +239,7 @@ def test_a_not_positive_definite_system_raises_lambda():
 def run_shapes(kitti, method, make_binary, make_unary):
     """FORWARD / BACKWARD (prior on frame i / i + 1), UNARY, MULTI_FRAME with test_alignment_gates' budgets"""
     poses, gt = kitti["poses"], kitti["gt"]
-    p = lm.Params(maxIterations=100, relativeErrorTol=1e-6) if method == "ICP" else lm.Params(maxIterations=30, relativeErrorTol=1e-4)
+    p = lg.Params(maxIterations=100, relativeErrorTol=1e-6) if method == "ICP" else lg.Params(maxIterations=30, relativeErrorTol=1e-4)
     prior = lambda var, frame: (var, poses[frame], [1e6] * 6)  # noqa: E731
 
     def check(result, fixed, note):
@@ -289,7 +270,9 @@ def test_abi_checks_before_the_set_is_read():
     import gtsam_points_b200 as g
 
     L = capi.lib()
-    p = g.LevenbergMarquardtExtParams().to_c()
+    p = capi.LmParamsC()
+    L.b2_lm_params_default(C.byref(p))
+    assert bytes(p) == bytes(g.LevenbergMarquardtExtParams().to_c())
     bogus = C.c_void_p(1)
     vars2 = np.array([[0, 1]], dtype=np.int32)
     vp = vars2.ctypes.data_as(C.POINTER(C.c_int32))
@@ -307,8 +290,14 @@ def test_abi_checks_before_the_set_is_read():
     for N in (0, capi.B2_LM_MAX_POSES + 1):
         st, err = call(N=N)
         assert st == 1 and "num_poses" in err
-    q = g.LevenbergMarquardtExtParams(lambdaFactor=1.0).to_c()
-    assert call(params=q)[0] == 1 and "lambda_factor" in L.b2_last_error().decode()
+    for kw, msg in [(dict(lambdaFactor=1.0), "lambda_factor"), (dict(absoluteErrorTol=0.0), "absolute_error_tol"), (dict(lambdaInitial=0.0), "lambda_initial"),
+                    (dict(maxIterations=-1), "max_iterations"), (dict(relativeErrorTol=math.inf), "not finite"),
+                    # lambda would underflow in max_iterations + 1 decreases (a closed form: no loop over the iterations)
+                    (dict(maxIterations=2**31 - 1), "underflows"),
+                    # more tryLambda calls than the bound allows: 1e-5 .. 1e5 in steps of 1 + 1e-12, and a 2^31-iteration budget
+                    (dict(lambdaFactor=1.0 + 1e-12), "tryLambda calls"), (dict(maxIterations=2**31 - 1, lambdaLowerBound=1e-6), "tryLambda calls")]:
+        st, err = call(params=g.LevenbergMarquardtExtParams(**kw).to_c())
+        assert st == 1 and msg in err, (kw, err)
     bad = T2.copy()
     bad[1, 0, 3] = math.inf
     assert call(T=bad)[0] == 1 and "not finite" in L.b2_last_error().decode()
